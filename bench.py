@@ -11,6 +11,7 @@ interleaved over the ranks (the CS is recomputed per rank; no data-path
 collective); a strong-scaling leg over a fixed 8192-eta grid is reported too.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+                  [--dump-outputs DIR]
 
 The b200 arm reports device-resident throughput (`value`), end-to-end
 throughput through the public API with pinned host buffers (`e2e`), the
@@ -73,7 +74,7 @@ def peak_hbm():
         with open(p) as fh:
             return float(json.load(fh)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 class ClockSampler:
@@ -274,25 +275,22 @@ def reference_arm(args):
 
 
 # --------------------------------------------------------------------------
-# B200 arm
+# GPU arm (--impl b200)
 # --------------------------------------------------------------------------
 PROF_NAMES = ["cs_rows", "cs_colA", "cs_colB", "thth_prep", "thth_build",
               "thth_eig", "sspec", "acf", "sim_screen", "sim_freq"]
 NETA_STRONG = 8192       # fixed global grid of the strong-scaling leg
+CS_SAMPLE = 1 << 18      # conjugate-spectrum elements written by --dump-outputs (2 MB)
 
 
-def ncu_traffic(kernel):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of `kernel`, read at
-    run time from the committed summary of the `ncu --set full` capture of this
-    same command (profiles/r2_ncu_traffic.json, written by profiles/ncu_traffic.py
-    from the .ncu-rep).  None when the capture does not list the kernel."""
-    path = os.path.join(ROOT, "profiles", "r2_ncu_traffic.json")
-    try:
-        with open(path) as fh:
-            d = json.load(fh)
-        return d["kernels"][kernel]["dram_bytes"], "profiles/r2_ncu_traffic.json (%s)" % d.get("source", "")
-    except Exception:
-        return None, "no committed ncu capture lists this kernel"
+def dump_outputs(out_dir, arrays):
+    """Write each array as out_dir/<name>.npy (float32 / float64 only)."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        if a.dtype not in (np.float32, np.float64):
+            a = a.astype(np.float64)
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def collect_prof(L, _lib):
@@ -406,6 +404,30 @@ def b200_arm(args):
     nred = wbuf["nred"].cpu().numpy().astype(np.int64)
     iters = wbuf["iters"].cpu().numpy()
     status = wbuf["stat"].cpu().numpy()
+    if args.dump_outputs:
+        # per-curvature results of every rank, in the order of the global grid etas_all
+        res = {"eigs": wbuf["eigs"], "status": wbuf["stat"], "nred": wbuf["nred"],
+               "iters": wbuf["iters"]}
+        if world > 1:
+            order = np.concatenate([np.arange(r, len(etas_all), world) for r in range(world)])
+            for k, t in res.items():
+                g = torch.empty((world * t.numel(),), dtype=t.dtype, device=dev)
+                dist.all_gather_into_tensor(g, t)
+                a = np.empty(len(etas_all), dtype=g.cpu().numpy().dtype)
+                a[order] = g.cpu().numpy()
+                res[k] = a
+        else:
+            res = {k: t.cpu().numpy() for k, t in res.items()}
+    if args.dump_outputs and rank == 0:
+        # d_cs still holds the last timed step's spectrum; a fixed seeded sample of its
+        # computed columns stands in for the 2.15 GB array
+        srng = np.random.default_rng(20240)
+        rows = torch.from_numpy(srng.integers(0, ntau, CS_SAMPLE)).to(dev)
+        cols = torch.from_numpy(srng.integers(0, keep or nfd // 2 + 1, CS_SAMPLE)).to(dev)
+        dump_outputs(args.dump_outputs, dict(
+            etas=etas_all, **res,
+            cs_sample_index=np.stack([rows.cpu().numpy(), cols.cpu().numpy()], axis=1),
+            cs_sample=d_cs[rows, cols].cpu().numpy()))
 
     # algorithmic bytes of one launch of the sweep kernels: one c64 gather of the
     # strict upper triangle + one f64 eigenvalue per eta (SURVEY.md 8d)
@@ -413,18 +435,16 @@ def b200_arm(args):
     dom = max((k for k in kern if k.startswith("thth")), key=lambda k: kern[k])
     peak, peak_src = peak_hbm()
     ach = alg_bytes / (kern[dom] * 1e-3) / 1e9
-    traffic, traffic_src = ncu_traffic(dom)
     roofline = {"bound": "hbm", "kernel": dom, "achieved": ach, "peak": peak,
                 "unit": "GB/s", "frac": ach / peak,
-                "traffic": traffic, "traffic_source": traffic_src,
                 "peak_source": peak_src,
                 "algorithmic_bytes_per_launch": alg_bytes,
                 "note": "iterative solver: every Lanczos step streams the triangle once "
                         "(scaled fp16 copy in 512-byte blocks for the tensor-core mat-vec, 0.54 MB at "
                         "N=511, ~19 steps + 1 surplus step of the deferred convergence check) + "
-                        "one fp32 pass for the Rayleigh quotient "
-                        "= `traffic`; kernel_ms = CUDA events on the launching stream per step, "
-                        "max over ranks",
+                        "one fp32 pass for the Rayleigh quotient, so the DRAM traffic is a "
+                        "multiple of the algorithmic bytes; kernel_ms = CUDA events on the "
+                        "launching stream per step, max over ranks",
                 "kernel_ms": kern}
 
     # ---- strong-scaling leg: fixed 8192-eta grid split over the ranks ----------
@@ -609,7 +629,14 @@ def main():
                     help="skip the strong-scaling leg (profiling runs)")
     ap.add_argument("--no-extra", action="store_true",
                     help="skip e2e_f64 and the C2/C4 extra configs (profiling runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="after the timed steps, write the results of the last step "
+                         "(eigenvalues, solver status / sizes / iterations of every rank in "
+                         "global curvature order, a seeded sample of rank 0's conjugate "
+                         "spectrum) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl != "b200":
+        ap.error("--dump-outputs applies to --impl b200")
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
     if args.impl == "reference":
         return reference_arm(args)

@@ -1,4 +1,4 @@
-/* libscint_b200 -- C ABI of the B200-native scintools arc-measurement hot path.
+/* libscint_b200 -- C ABI of the CUDA-native scintools arc-measurement hot path.
  *
  * The reference (danielreardon/scintools) is pure Python and has no FFI; each
  * entry point below names the reference callable whose arithmetic it replaces
@@ -15,7 +15,7 @@
  *  - one CUDA context per process, calls into one device from one host
  *    thread at a time (the library keeps a grow-only scratch workspace per
  *    process; sb_release() frees it).  Not fork-safe (CUDA is not).
- *  - sm_100a only; there is no CPU fallback.
+ *  - sm_90a (H100) only; there is no CPU fallback.
  */
 #ifndef SCINT_B200_H
 #define SCINT_B200_H

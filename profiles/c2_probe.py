@@ -1,6 +1,6 @@
 """calc_sspec / calc_acf at BASELINE config 2 (4096x8192), a few calls each: run under
-`ncu --metrics gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum` for the
-per-kernel launch list (profiles/r2_c2_launches.csv)."""
+`ncu --metrics gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum` for a
+per-kernel launch list."""
 import sys
 import numpy as np
 sys.path.insert(0, ".")

@@ -1,9 +1,9 @@
-"""SASS opcode histogram per kernel of the shipped library (no GPU needed):
-  python profiles/sass_histogram.py > profiles/r2_sass_histogram.txt
-Also writes profiles/r2_sass_tma.txt: every kernel that contains TMA instructions
-(UTMALDG = cp.async.bulk.tensor, UBLKCP = cp.async.bulk), LDGSTS (cp.async) or packed
-fp32 math (FFMA2 / FADD2 / FMUL2) or tensor-core instructions (LDSM = ldmatrix, HMMA = mma.sync),
-with the counts."""
+"""SASS opcode histogram per kernel of the built library (no GPU needed):
+  python profiles/sass_histogram.py [TMA_LIST] > histogram.txt
+With TMA_LIST, also writes to that file every kernel that contains TMA instructions
+(UTMALDG = cp.async.bulk.tensor, UBLKCP = cp.async.bulk), LDGSTS (cp.async), mbarrier
+operations (SYNCS) or tensor-core instructions (LDSM = ldmatrix, HMMA = mma.sync), with the
+counts."""
 import collections
 import os
 import re
@@ -32,7 +32,7 @@ def main():
             return subprocess.run(["c++filt", n], capture_output=True, text=True).stdout.strip()[:150]
         except Exception:
             return n
-    special = ("UTMALDG", "UTMASTG", "UBLKCP", "LDGSTS", "LDSM", "HMMA", "FFMA2", "FADD2", "FMUL2", "SYNCS")
+    special = ("UTMALDG", "UTMASTG", "UBLKCP", "LDGSTS", "LDSM", "HMMA", "SYNCS")
     tma_lines = []
     print("# %d kernels in %s" % (len(kernels), os.path.relpath(LIB, ROOT)))
     for name, c in kernels.items():
@@ -42,11 +42,12 @@ def main():
         hit = {k: c[k] for k in special if c.get(k)}
         if hit:
             tma_lines.append("%s\n    %s" % (d, ", ".join("%s %d" % kv for kv in hit.items())))
-    with open(os.path.join(ROOT, "profiles", "r2_sass_tma.txt"), "w") as fh:
-        fh.write("# kernels of libscint_b200.so with TMA / cp.async / packed-fp32 instructions\n"
-                 "# (cuobjdump -sass; UTMALDG = cp.async.bulk.tensor, UBLKCP = cp.async.bulk, LDSM = ldmatrix, HMMA = mma.sync,\n"
-                 "#  LDGSTS = cp.async, SYNCS = mbarrier, FFMA2/FADD2/FMUL2 = *.f32x2)\n\n")
-        fh.write("\n".join(tma_lines) + "\n")
+    if len(sys.argv) > 1:
+        with open(sys.argv[1], "w") as fh:
+            fh.write("# kernels of libscint_b200.so with TMA / cp.async / mbarrier / tensor-core instructions\n"
+                     "# (cuobjdump -sass; UTMALDG = cp.async.bulk.tensor, UBLKCP = cp.async.bulk, LDSM = ldmatrix, HMMA = mma.sync,\n"
+                     "#  LDGSTS = cp.async, SYNCS = mbarrier)\n\n")
+            fh.write("\n".join(tma_lines) + "\n")
 
 
 if __name__ == "__main__":

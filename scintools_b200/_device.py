@@ -15,7 +15,7 @@ def device():
         import torch
         if not torch.cuda.is_available():
             raise RuntimeError(
-                "scintools_b200 needs a CUDA (sm_100a) device; there is no "
+                "scintools_b200 needs a CUDA (sm_90a) device; there is no "
                 "CPU fallback")
         idx = int(os.environ.get("LOCAL_RANK", "0")) % torch.cuda.device_count()
         torch.cuda.set_device(idx)

@@ -1,7 +1,7 @@
 """ctypes binding of libscint_b200.so (C ABI in include/scint_b200.h).
 
 There is NO fallback: if the shared library is missing this module raises at
-import time; if no sm_100 device is present the first device call raises.
+import time; if no sm_90 device is present the first device call raises.
 """
 import ctypes
 import os
@@ -17,7 +17,7 @@ class SbError(RuntimeError):
 if not os.path.exists(LIB_PATH):
     raise ImportError(
         "scintools_b200: %s not found. Build it with "
-        "`python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_100a). "
+        "`python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_90a). "
         "There is no CPU fallback." % LIB_PATH)
 
 lib = ctypes.CDLL(LIB_PATH)

@@ -1,4 +1,4 @@
-"""Classical arc fit: Dynspec.norm_sspec / Dynspec.fit_arc on the B200 path
+"""Classical arc fit: Dynspec.norm_sspec / Dynspec.fit_arc on the GPU path
 (reference scintools/dynspec.py:1920-2183 and :970-1346, SURVEY.md 8f rank 2).
 
 The device does the heavy part -- every delay row of the secondary spectrum
@@ -106,10 +106,10 @@ class ArcFitMixin:
         delay (reference dynspec.py:1920-2183) -> self.normsspec (masked 2-D),
         normsspecavg, normsspec_tdel, normsspec_fdop, powerspectrum, mask, weights."""
         if plot:
-            raise NotImplementedError("plotting is outside the B200 hot path")
+            raise NotImplementedError("plotting is outside the GPU hot path")
         if velocity or logsteps or interp_nan or fit_spectrum or minnormfac > 0:
             raise NotImplementedError(
-                "norm_sspec on the B200 path: velocity, logsteps, interp_nan, "
+                "norm_sspec on the GPU path: velocity, logsteps, interp_nan, "
                 "fit_spectrum (lmfit) and minnormfac > 0 are not part of this version")
         delmax = np.max(self.tdel) if delmax is None else delmax
         if lamsteps:
@@ -202,9 +202,9 @@ class ArcFitMixin:
         sets eta / etaerr / etaerr2 (or betaeta... with lamsteps, ..._left / _right with
         asymm), eta_array, norm_sspec_avg, prob_eta_peak, noise, norm_delmax."""
         if plot or plot_spec:
-            raise NotImplementedError("plotting is outside the B200 hot path")
+            raise NotImplementedError("plotting is outside the GPU hot path")
         if velocity:
-            raise NotImplementedError("velocity rescaling is outside the B200 hot path")
+            raise NotImplementedError("velocity rescaling is outside the GPU hot path")
         if not hasattr(self, 'tdel'):
             self.calc_sspec()
         delmax = np.max(self.tdel) if delmax is None else delmax

@@ -13,7 +13,7 @@ namespace sb {
 static thread_local char g_err[512] = "";
 static void* g_ws[8] = {nullptr};
 static size_t g_ws_bytes[8] = {0};
-static int g_sms = 148;
+static int g_sms = 132;
 
 void set_error(const char* fmt, ...) {
     va_list ap;
@@ -202,8 +202,8 @@ int sb_init(int device) {
     SB_CUDA(cudaFree(0));
     cudaDeviceProp prop;
     SB_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) {
-        sb::set_error("device %d is sm_%d%d; libscint_b200 is sm_100a only",
+    if (prop.major != 9 || prop.minor != 0) {
+        sb::set_error("device %d is sm_%d%d; libscint_b200 is sm_90a only",
                       device, prop.major, prop.minor);
         return SB_ERR_UNSUPPORTED;
     }

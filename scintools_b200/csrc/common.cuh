@@ -1,4 +1,4 @@
-// Shared helpers for libscint_b200 (sm_100a only).
+// Shared helpers for libscint_b200 (sm_90a only).
 #pragma once
 #ifndef SB_HOST_EMU            // tests/host_emu compiles the device code for the CPU
 #include <cuda_runtime.h>

@@ -485,7 +485,7 @@ int eig_cluster_launch(const float2* d_M, int ld, int n_max, const int* d_nred, 
     int force = 0;
     if (const char* ev = getenv("SB_EIG_CLUSTER")) force = (ev[0] == 'a') ? 1 : atoi(ev);
     if (force <= 0) return 0;
-    const size_t smem_max = 232448;   // 227 KB opt-in limit of sm_100
+    const size_t smem_max = 232448;   // 227 KB opt-in limit of sm_90
     size_t smem = 0;
     int npair_max = 0;
     int C = pick_cluster(n_max, smem_max, &smem, &npair_max);

@@ -14,10 +14,9 @@
 //     ||A y - rho y|| / rho of 0.6e-3 .. 3e-3 and Rayleigh-quotient errors up to
 //     1.1e-5 on the 4096x8192 workload -- fp16's 11 bits give 8x / 64x less;
 //   * keeps the lane's 16 vector elements and 16 column accumulators in
-//     registers for the whole mat-vec and does the complex multiply-adds with
-//     PACKED fp32 FMAs (Blackwell FFMA2, fma.rn.f32x2, scalar operand broadcast):
-//     one LDS.128 + 8 converts + 16 FFMA2 per four complex elements; no masks
-//     except on the diagonal group;
+//     registers for the whole mat-vec and does the complex multiply-adds as
+//     fp32 FMAs: one LDS.128 + 8 converts + 32 FFMA per four complex elements;
+//     no masks except on the diagonal group;
 //   * fetches the rows with per-lane cp.async copies (every lane copies exactly
 //     the 16-byte chunks it reads itself: a wait_group is all the synchronisation
 //     a stage needs), two adjacent rows per stage, and reduces their four row
@@ -56,20 +55,10 @@ constexpr int EB_SLOTS = SB_EB_SLOTS; // tests/host_emu: few slots to exercise t
 constexpr int EB_SLOTS = 48;          // Lanczos vectors kept for the Ritz vector
 #endif
 
-// acc += a * (b, b): one packed fp32 FMA (Blackwell FFMA2; ptxas folds the
-// duplicated scalar into the .F32 broadcast operand form)
+// acc += a * (b, b): two fp32 FMAs, one per component
 __device__ __forceinline__ void ffma2(float2& acc, const float2 a, const float b) {
-#ifdef SB_HOST_EMU
     acc.x = fmaf(a.x, b, acc.x);
     acc.y = fmaf(a.y, b, acc.y);
-#else
-    unsigned long long ra, rb, rc;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(ra) : "f"(a.x), "f"(a.y));
-    asm("mov.b64 %0, {%1, %1};" : "=l"(rb) : "f"(b));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(rc) : "f"(acc.x), "f"(acc.y));
-    asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(rc) : "l"(ra), "l"(rb));
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(acc.x), "=f"(acc.y) : "l"(rc));
-#endif
 }
 
 // packed element of the fp16 triangle (thth.cu: pack_f16x2): re in the low, im in
@@ -196,8 +185,8 @@ __host__ __device__ inline size_t eig_half_smem(int ld, int mode = EB_MODE_CPA) 
 // EB_MODE_TC runs one more warp (warp EB_NW): it only joins the barriers and runs the
 // deferred convergence checks, so the eight mat-vec warps carry equal shares in every step
 // (with the check on warp 0 that warp idled through half of every step without a check and
-// was the straggler of the steps with one: 16 % of all warp samples sat at the barrier
-// that ends the mat-vec, ncu source view of call 14).
+// was the straggler of the steps with one, holding the others at the barrier that ends the
+// mat-vec).
 template <int MODE>
 __global__ void __launch_bounds__(eb_is_tc(MODE) ? EB_THREADS + 32 : EB_THREADS, 2)
 thth_eig_half_kernel(const float2* __restrict__ Mbase, const unsigned* __restrict__ Mbbase,
@@ -453,14 +442,13 @@ thth_eig_half_kernel(const float2* __restrict__ Mbase, const unsigned* __restric
     // with the vector in the n-columns of B as fp16 hi + 2^-11 lo pairs (n = 0 / 1: real /
     // imaginary part of the product from the hi halves, n = 2 / 3 from the lo halves;
     // 22 mantissa bits, the fp32 accumulators do the rest): 2 ldmatrix + 2 mma per 128
-    // matrix elements instead of 32 FFMA2 + 16 converts.
+    // matrix elements instead of 64 FFMA + 16 converts.
     // A warp walks its row blocks one after the other and the blocks of a row block left to
     // right, two adjacent blocks (1 KB, contiguous in memory) per step -- one linear stream
     // per row block, so the producer cursor is an address increment.  (The first version
-    // walked column-group major to keep the column sums in registers: its cursor search was
-    // 45 % of all instructions executed -- ncu source view, profiles/r2c13_eig_tc_lines.txt --
-    // and the kernel slower than the packed-FMA one.)  The row sums D1 of the current row
-    // block stay in registers; the column sums of every step are added to the warp's private
+    // walked column-group major to keep the column sums in registers: its cursor search
+    // dominated the instruction count and made it slower than the FMA mat-vec.)  The row
+    // sums D1 of the current row block stay in registers; the column sums of every step are added to the warp's private
     // 4 KB column buffer (one lane per slot, LDS.128 / STS.128: no hazards).  Units arrive
     // through a ring of EB_TC_NST 1 KB stages per warp (two 16-byte cp.async chunks per lane,
     // XOR-swizzled so that both ldmatrix forms are conflict free).
@@ -946,14 +934,14 @@ int eig_half_launch(const float2* d_M, const unsigned* d_Mb, int ld, const int* 
     // stopping rule of the fp16 phase: res^2 <= etol_h * theta * gap.  Its Ritz vector only
     // feeds the fp32 Rayleigh quotient (second order in the vector error), so it can stop
     // earlier than the fp32 solver's 2e-7: 1e-6 saves one step per curvature on average with
-    // the same worst-case error against dense eigenvalues (3e-6, profiles/r2_eig_truth.json)
+    // the same worst-case error against dense eigenvalues (3e-6)
     double etol_h = 1e-6;
     if (const char* ev = getenv("SB_EIG_ETOL_B")) etol_h = atof(ev);
     static const bool bulk = getenv("SB_EIG_BULK") != nullptr;   // A/B: cp.async.bulk row fetch
     const int mode = tensor ? EB_MODE_TC : (bulk ? EB_MODE_BULK : EB_MODE_CPA);
     size_t smem = eig_half_smem(ld, mode);
     // SB_EIG_SMEM_PAD=bytes: experiment switch -- extra dynamic shared memory so that only one
-    // CTA fits an SM (148 matrices x 0.52 MB in flight fit the 126 MB L2)
+    // CTA fits an SM (fewer 0.52 MB matrices in flight compete for the L2)
     if (const char* ev = getenv("SB_EIG_SMEM_PAD")) smem += (size_t)atoi(ev);
 #define SB_EIG_HALF_LAUNCH(MODE)                                                                  \
     do {                                                                                          \

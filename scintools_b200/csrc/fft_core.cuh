@@ -1,4 +1,4 @@
-// Hand-written radix-2/4/8/16 FFT building blocks for sm_100a.
+// Hand-written radix-2/4/8/16 FFT building blocks for sm_90a.
 //
 // Everything here works on a shared-memory array viewed as [fft index][batch]:
 // element (i, b) lives at s[i * fstride + b * bstride].  Lanes always run over
@@ -50,45 +50,26 @@ __device__ __forceinline__ C mul_cs(C a, T c, T s) {
     return r;
 }
 
-// ---- float2 arithmetic on Blackwell's packed fp32 pipe ---------------------
-// add / sub / mul / fma .f32x2 (SASS FADD2 / FMUL2 / FFMA2, with free swap / negate /
-// scalar-broadcast operand forms): a complex add is ONE instruction, a complex multiply
-// TWO (b * a.x + (-b.y, b.x) * a.y) instead of two and six scalar ones.  These overloads
-// are picked over the generic templates above for every fp32 transform; the fp64
-// paths are unchanged.
+// ---- fp32 complex arithmetic with a fixed rounding sequence ----------------
+// A complex multiply is b * a.x + (-b.y, b.x) * a.y: one rounded multiply and one
+// fused multiply-add per component.  The _rn intrinsics keep the compiler from
+// contracting or reordering these, so every fp32 transform rounds the same way
+// whatever the optimisation level.  These overloads are picked over the generic
+// templates above for every fp32 transform; the fp64 paths are unchanged.
 #ifndef SB_HOST_EMU
-__device__ __forceinline__ unsigned long long f2_pack(float2 a) {
-    unsigned long long r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a.x), "f"(a.y));
-    return r;
-}
-__device__ __forceinline__ float2 f2_unpack(unsigned long long r) {
-    float2 a;
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(a.x), "=f"(a.y) : "l"(r));
-    return a;
-}
 __device__ __forceinline__ float2 cadd(float2 a, float2 b) {
-    unsigned long long r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(f2_pack(a)), "l"(f2_pack(b)));
-    return f2_unpack(r);
+    return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y));
 }
 __device__ __forceinline__ float2 csub(float2 a, float2 b) {
-    unsigned long long r;
-    asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(f2_pack(a)), "l"(f2_pack(b)));
-    return f2_unpack(r);
+    return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y));
 }
 // a * (s, s)
 __device__ __forceinline__ float2 f2_scale(float2 a, float s) {
-    unsigned long long r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(f2_pack(a)), "l"(f2_pack(make_float2(s, s))));
-    return f2_unpack(r);
+    return make_float2(__fmul_rn(a.x, s), __fmul_rn(a.y, s));
 }
 // a * (s, s) + c
 __device__ __forceinline__ float2 f2_fma(float2 a, float s, float2 c) {
-    unsigned long long r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r)
-        : "l"(f2_pack(a)), "l"(f2_pack(make_float2(s, s))), "l"(f2_pack(c)));
-    return f2_unpack(r);
+    return make_float2(__fmaf_rn(a.x, s, c.x), __fmaf_rn(a.y, s, c.y));
 }
 __device__ __forceinline__ float2 cmul(float2 a, float2 b) {
     return f2_fma(make_float2(-b.y, b.x), a.y, f2_scale(b, a.x));

@@ -297,9 +297,8 @@ __global__ void __launch_bounds__(sizeof(T) == 4 ? 1024 : 512) row_fft_c2r_kerne
 
 inline int row_threads(int N, int elem_bytes = 8) {
     // N / 16 threads: one radix-16 butterfly per thread and pass, and two CTAs share an SM for
-    // rows up to 8192 points, overlapping their load / transform / store phases (measured at
-    // 4096x8192, call 15: r2c 322 -> 258 us, c2r 616 -> 444 us; 16384-point rows keep 1024
-    // threads either way).  SB_ROW_DIV=8: the round-1 geometry (N / 8 threads)
+    // rows up to 8192 points, overlapping their load / transform / store phases (16384-point
+    // rows keep 1024 threads either way).  SB_ROW_DIV=8: the round-1 geometry (N / 8 threads)
     static const int div = (getenv("SB_ROW_DIV") && atoi(getenv("SB_ROW_DIV")) == 8) ? 8 : 16;
     int t = N / div;
     if (t < 32) t = 32;

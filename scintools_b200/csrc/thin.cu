@@ -324,7 +324,7 @@ int thin_map(const ThinGeom& t, double e1, double e2, float2* d_out, int* d_err,
     SB_CUDA(cudaMemsetAsync(d_err, 0, sizeof(int), st));
     const long long total = (long long)t.g.n * t.n2;
     int blocks = (int)((total + 255) / 256);
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > num_sms() * 16) blocks = num_sms() * 16;
     thin_map_kernel<<<blocks, 256, 0, st>>>(t, e1, e2, d_out, d_err);
     SB_LAUNCH_CHECK();
     return SB_OK;

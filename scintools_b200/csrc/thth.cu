@@ -150,14 +150,19 @@ __global__ void cs_absmax_kernel(const float2* __restrict__ cs, long long rows, 
 // body runs in three phases -- (1) tau_inv and the CS offset of every row, (2) ALL the
 // gathers back to back, (3) Jacobian, clean-up, stores -- so that ROWS independent
 // L2 / DRAM gathers are in flight per thread: the kernel is bound by the latency of
-// these random 8-byte loads (ncu: long-scoreboard stalls 8.8 per issue with one load in
-// flight), not by its instruction count.
+// these random 8-byte loads (long-scoreboard stalls dominate with one load in flight),
+// not by its instruction count.
 // PACK == 2: the fp16 copy in the block layout of eig_half.cu's tensor-core mat-vec:
 // 512-byte blocks of 16 rows x 8 columns, block (I, G) at ((I * ld / 8 + G) * 512) bytes,
 // a block row = [re x 8 | im x 8] (the halves swapped in rows 4-7, 12-15); the part of a
 // diagonal block on / below the diagonal is written as zeros (the MMA has no masks).
+// ROWS == 4: three CTAs per SM (80 registers).  ptxas still spills at 80 registers, but
+// less: 40-48 bytes of stores and 56-68 bytes of loads per thread in the PACK == 2
+// instances on sm_90, against ~200 / ~150 bytes at four CTAs (64 registers), where the
+// gather runs ~15 % slower on the headline sweep (H100 SXM, 400 W power limit: 2.8-2.9 ms
+// instead of 2.4 ms per 1024-eta launch).
 template <int PACK, int ROWS, typename OFF>
-__global__ void __launch_bounds__(32 * (32 / ROWS), ROWS == 8 ? 5 : 4)
+__global__ void __launch_bounds__(32 * (32 / ROWS), ROWS == 8 ? 5 : 3)
 thth_build_kernel(ThthGeom g, const double* __restrict__ etas, int eta0, int nbatch,
                   int ld, const int* __restrict__ idx,
                   const int* __restrict__ nred, float2* __restrict__ M,
@@ -306,7 +311,7 @@ thth_build_kernel(ThthGeom g, const double* __restrict__ etas, int eta0, int nba
             if (PACK == 2) {
                 // block row of 8 columns = [re x 8 | im x 8] (32 bytes): the 8 lanes of a column
                 // group trade halves so that lane i stores 4-byte word i of it -- one store
-                // instruction, four full 32-byte sectors per warp (2-byte stores: +0.14 ms).
+                // instruction, four full 32-byte sectors per warp (2-byte stores would be slower).
                 // Elements on / below the diagonal of a diagonal block are zeros (the MMA has
                 // no masks); 16 x 16 sub-blocks entirely below the diagonal are never read.
                 const unsigned h = low ? 0u : pack_f16x2(make_float2(v.x * hscale, v.y * hscale));
@@ -846,12 +851,12 @@ int eta_sweep(const ThthGeom& g, const double* th_host, const double* d_etas,
     }
     for (int e0 = 0; e0 < neta; e0 += batch) {
         int nb = neta - e0 < batch ? neta - e0 : batch;
-        // rows per thread of thth_build_kernel: 4 (default) or 8 (SB_BUILD_ROWS=8; measured
-        // slower: 1.54 vs 1.21 ms -- the gather is bound by random DRAM sector reads, not by
-        // the number of loads a thread keeps in flight)
+        // rows per thread of thth_build_kernel: 4 (default) or 8 (SB_BUILD_ROWS=8; slower: the
+        // gather is bound by random DRAM sector reads, not by the number of loads a thread keeps
+        // in flight)
         static const int BR = (getenv("SB_BUILD_ROWS") && atoi(getenv("SB_BUILD_ROWS")) == 8) ? 8 : 4;
         // tensor-core mat-vec of the default solver (block layout of the fp16 copy);
-        // SB_EIG_NO_TC=1: the packed-FMA mat-vec on the row-major copy
+        // SB_EIG_NO_TC=1: the FMA mat-vec on the row-major copy
         const bool tensor = mixed && BR == 4 && !getenv("SB_EIG_NO_TC");
         dim3 grid((nb + SB_BUILD_EB - 1) / SB_BUILD_EB, npairs), block(32, 32 / BR);
         prof_begin(PROF_THTH_BUILD, st);
@@ -923,7 +928,7 @@ int thth_map(const ThthGeom& g, double eta, int hermitian, float2* d_out,
     SB_CUDA(cudaMemsetAsync(d_err, 0, sizeof(int), st));
     long long total = (long long)g.n * g.n;
     int blocks = (int)((total + 255) / 256);
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > num_sms() * 16) blocks = num_sms() * 16;
     thth_map_kernel<<<blocks, 256, 0, st>>>(g, eta, hermitian, d_out, d_tau_inv,
                                             d_fd_inv, d_pnts, d_err);
     SB_LAUNCH_CHECK();

@@ -1,4 +1,4 @@
-"""B200-native mirror of the FFT / theta-theta part of scintools.dynspec.
+"""CUDA-native mirror of the FFT / theta-theta part of scintools.dynspec.
 
 Keeps the ``Dynspec`` method names, signatures and attribute side effects of
 the reference for the arc-measurement hot path:
@@ -92,7 +92,7 @@ class Dynspec(ArcFitMixin):
                  mjd=None):
         if filename:
             raise NotImplementedError(
-                "psrflux file I/O is outside the B200 hot path: load with "
+                "psrflux file I/O is outside the GPU hot path: load with "
                 "scintools.Dynspec and pass the object as dyn=")
         elif dyn is not None:
             self.load_dyn_obj(dyn, verbose=verbose, process=process,
@@ -132,7 +132,7 @@ class Dynspec(ArcFitMixin):
     def _pick_dyn(self, lamsteps, velocity, trap):
         """The array calc_sspec transforms (reference dynspec.py:3642-3663): the
         wavelength-rescaled copy is made on demand (scale_dyn -> self.lamdyn);
-        velocity / trapezoid resampling is outside the B200 hot path and must have
+        velocity / trapezoid resampling is outside the GPU hot path and must have
         been set by the caller."""
         if lamsteps and not velocity and not hasattr(self, "lamdyn"):
             self.scale_dyn()
@@ -142,7 +142,7 @@ class Dynspec(ArcFitMixin):
             if flag:
                 if not hasattr(self, attr):
                     raise NotImplementedError(
-                        "velocity / trapezoid resampling is outside the B200 hot "
+                        "velocity / trapezoid resampling is outside the GPU hot "
                         "path; set self.%s first" % attr)
                 return cp(getattr(self, attr))
         return self.dyn
@@ -158,7 +158,7 @@ class Dynspec(ArcFitMixin):
         the reference's; pass dtype=np.float32 to skip the widening."""
         import torch
         if plot:
-            raise NotImplementedError("plotting is outside the B200 hot path")
+            raise NotImplementedError("plotting is outside the GPU hot path")
         dyn = self._pick_dyn(lamsteps, velocity, trap) if input_dyn is None \
             else input_dyn
         dyn = np.asarray(dyn)
@@ -270,7 +270,7 @@ class Dynspec(ArcFitMixin):
         import torch
         from scipy.constants import c as c_light
         if not (('lambda' in scale) or ('wavelength' in scale)):
-            raise NotImplementedError("only scale='lambda' is on the B200 path")
+            raise NotImplementedError("only scale='lambda' is on the GPU path")
         freqs = np.array(self.freqs, dtype=np.float64)
         nf, nt = self.dyn.shape
         lams = np.divide(c_light, freqs * 10 ** 6)
@@ -458,7 +458,7 @@ class Dynspec(ArcFitMixin):
         if not hasattr(self, 'cwf'):
             self.prep_thetatheta(verbose=verbose)
         if plot:
-            raise NotImplementedError("plotting is outside the B200 hot path")
+            raise NotImplementedError("plotting is outside the GPU hot path")
         cf = min(cf, self.ncf_fit - 1)
         ct = min(ct, self.nct_fit - 1)
         fs = slice(cf * self.cwf, (cf + 1) * self.cwf)
@@ -499,11 +499,11 @@ class Dynspec(ArcFitMixin):
         context does not survive fork; the chunks run back to back on the GPU
         (each one already fills it)."""
         if pool is not None:
-            raise ValueError("fit_thetatheta on the B200 path takes pool=None "
+            raise ValueError("fit_thetatheta on the GPU path takes pool=None "
                              "(CUDA is not fork-safe); chunks are batched on "
                              "the device instead")
         if plot:
-            raise NotImplementedError("plotting is outside the B200 hot path")
+            raise NotImplementedError("plotting is outside the GPU hot path")
         if not hasattr(self, 'cwf'):
             self.prep_thetatheta(verbose=verbose)
         self.eta_evo = np.zeros((self.ncf_fit, self.nct_fit))
@@ -569,10 +569,10 @@ class Dynspec(ArcFitMixin):
         block-partitioned over the ranks of ``group`` and all-gathered, the
         counterpart of the reference's ``pool.map`` over chunks (:1815-1828)."""
         if pool is not None:
-            raise ValueError("thetatheta_chunks on the B200 path takes pool=None "
+            raise ValueError("thetatheta_chunks on the GPU path takes pool=None "
                              "(CUDA is not fork-safe)")
         if memmap:
-            raise NotImplementedError("memmap chunk storage is outside the B200 path")
+            raise NotImplementedError("memmap chunk storage is outside the GPU path")
         if not hasattr(self, "ththeta"):
             self.fit_thetatheta(verbose=verbose)
         from . import sharding

@@ -3,7 +3,7 @@
 dynspec, dynspecs block-partitioned over ranks, one all-gather of the fitted
 curvatures at the end).
 
-This is the B200 counterpart of the reference's only parallel mode,
+This is the GPU counterpart of the reference's only parallel mode,
 ``pool.map(thth.single_search, pars)`` over independent chunks
 (scintools/dynspec.py:1715-1719): one process per GPU instead of a fork pool.
 """

@@ -1,4 +1,4 @@
-"""B200-native mirror of scintools.scint_sim.Simulation
+"""CUDA-native mirror of scintools.scint_sim.Simulation
 (reference scintools/scint_sim.py:23-311).
 
 Same constructor signature and the same attributes afterwards (w, xyp, xyi,
@@ -37,7 +37,7 @@ class Simulation():
                  verbose=False, freq=1400, dt=30, mjd=60000, nsub=None,
                  efield=False, noise=None, device_rng=False, keep_device=False, lazy=False):
         if plot:
-            raise NotImplementedError("plotting is outside the B200 hot path")
+            raise NotImplementedError("plotting is outside the GPU hot path")
         self.mb2 = mb2
         self.rf = rf
         self.ds = ds

@@ -1,4 +1,4 @@
-"""B200-native mirror of scintools.ththmod's curvature-search API.
+"""CUDA-native mirror of scintools.ththmod's curvature-search API.
 
 Same function names, argument order and failure behaviour as the reference
 (scintools/ththmod.py); the arithmetic runs in libscint_b200 on the GPU:
@@ -435,7 +435,7 @@ def _search_launch(params, staged, pinned=False):
     (dspec2, freq, time, etas, edges, name, plot, fw, npad, coher, tauMask,
      verbose) = params
     if plot:
-        raise NotImplementedError("plotting is outside the B200 hot path; "
+        raise NotImplementedError("plotting is outside the GPU hot path; "
                                   "use scintools.ththmod.plot_func on the "
                                   "returned eigenvalues")
     if staged is not None:
@@ -641,7 +641,7 @@ def single_search_thin(params):
     (dspec2, freq, time, etas, edges, name, plot, fw, npad, coher, verbose,
      edgesArclet, centerCut) = params
     if plot:
-        raise NotImplementedError("plotting is outside the B200 hot path")
+        raise NotImplementedError("plotting is outside the GPU hot path")
     time_v = U.value(time, "s")
     freq_v = U.value(freq, "MHz")
     etas_v = U.value(etas, "s3")
@@ -739,7 +739,7 @@ def modeler(CS, tau, fd, eta, edges, hermetian=True):
     if not hermetian:
         raise NotImplementedError(
             "modeler(hermetian=False) raises IndexError in the reference "
-            "(ththmod.py:316-320) and is not part of the B200 path")
+            "(ththmod.py:316-320) and is not part of the GPU path")
     tauv, fdv = U.value(tau, "us"), U.value(fd, "mHz")
     thth_red, edges_red = thth_redmap(CS, tau, fd, eta, edges, hermetian=True)
     w, V, _ = _top_eigenpair(thth_red)

@@ -163,7 +163,7 @@ def test_default_sweep_kernels_on_host(golden_dir, mixed, slots):
     emulator, launch geometry as in sb::eta_sweep, against the reference: cropped
     sizes bit-exact, eigenvalues to 1e-5.  mixed=0: the fp32 streaming solver
     thth_eig_kernel<256, TMA, 2> (SB_EIG_FP32=1); mixed=1: the default solver
-    with the packed-FMA mat-vec (fp16 iteration + fp32 Rayleigh quotient); mixed=2: its
+    with the FMA mat-vec (fp16 iteration + fp32 Rayleigh quotient); mixed=2: its
     fp32 continuation forced on every curvature; mixed=3: the tensor-core mat-vec on the
     block layout of the fp16 copy (ldmatrix / mma.sync emulated lane-exactly);
     slots=3: the fp32 restart (basis slots exhausted)."""
