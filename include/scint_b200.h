@@ -157,13 +157,17 @@ int sb_herm_eigvec(const void* a, int32_t n, int32_t ld, double tol, int32_t max
                    double* w, void* v, int32_t* info, void* stream);
 
 /* out[:crop0, :crop1] = scale * ifft2(ifftshift(in)) (centred != 0) or
- * scale * ifft2(in), in: float2 [n0][n1], powers of two (ththmod.py:321, :1462-1465).
- * real_only != 0 writes float (the real part), else float2.  crop <= 0: full. */
+ * scale * ifft2(in), in: float2 [n0][n1] (ththmod.py:321, :1462-1465).  Powers of two
+ * up to 65536 x 16384 (n0 x n1, both >= 8) take the radix path; any other size up to
+ * 32768 x 8192 runs a chirp-z transform.  real_only != 0 writes float (the real
+ * part), else float2.  crop <= 0: full. */
 int sb_ifft2_c2c_f32(const void* in, int32_t n0, int32_t n1, int32_t centred, int32_t crop0,
                      int32_t crop1, double scale, int32_t real_only, void* out, void* stream);
 
 /* The loop of Dynspec.gerchberg_saxton (scintools/dynspec.py:1883-1896), niter
- * times, in place on wavefield (float2 [n0][n1], powers of two):
+ * times, in place on wavefield (float2 [n0][n1]; sizes as sb_ifft2_c2c_f32: powers of
+ * two up to 65536 x 16384, iterated in fp64 when n1 <= 8192; other sizes up to
+ * 32768 x 8192 through the fp32 chirp-z transform):
  *   CWF = fft2(w); CWF[rowmask != 0, :] = 0; w = ifft2(CWF);
  *   w = amp * exp(i angle(w)) where amp is not NaN.
  * rowmask: uint8 [n0] over the UNSHIFTED delay rows (1 where tau < 0);
@@ -225,10 +229,10 @@ int sb_sspec_f32(const float* dyn, int32_t nf, int32_t nt, const float* win_t,
 /* Replaces Dynspec.calc_acf(method='direct') (scintools/dynspec.py:3780-3797):
  * real(fftshift(ifft2(|fft2(dyn - mean(valid), [2nf, 2nt])|^2))) [/ max].
  * acf: float32 [2nf][2nt].  subtract_mean=0 reproduces the input_dyn branch
- * (dynspec.py:3786-3789).  Any 2nf x 2nt is accepted: the transform runs on the
- * next power of two and the lags [-nf,nf) x [-nt,nt) are extracted (identical
- * by the correlation theorem).  The normalisation divides by the zero-lag
- * value, which is the maximum of an autocovariance. */
+ * (dynspec.py:3786-3789).  nf 2..32768, nt 5..16384, not only powers of two: the
+ * transform runs on the next power of two and the lags [-nf,nf) x [-nt,nt) are
+ * extracted (identical by the correlation theorem).  The normalisation divides by
+ * the zero-lag value, which is the maximum of an autocovariance. */
 int sb_acf_f32(const float* dyn, int32_t nf, int32_t nt, int32_t subtract_mean,
                int32_t normalise, float* acf, void* stream);
 
@@ -257,7 +261,7 @@ int sb_acf_sspec_f32(const float* dyn, int32_t nf, int32_t nt, const float* win_
  * the transform).  0 = all nfd/2 + 1 columns.
  * Power-of-two padded sizes take the direct radix-16 path (rows <= 65536, cols
  * <= 32768); any other size runs a chirp-z (Bluestein) transform on both axes
- * (rows <= 32768, cols <= 8192, half_plane must be 0). */
+ * (rows 3..32768, cols 3..8192, half_plane must be 0). */
 int sb_cs_f32(const float* dspec, int32_t nf, int32_t nt, int32_t npad,
               float pad_value, const uint8_t* tau_rowmask, int32_t half_plane,
               int64_t cs_pitch, int32_t ncols_keep, void* cs, void* stream);

@@ -663,7 +663,8 @@ int sspec(const float* dyn, int nf, int nt, const float* wt, const float* wf,
     ProfScope prof(PROF_SSPEC, st);
     const int NF = 2 * next_pow2(nf), NT = 2 * next_pow2(nt);  // 2^(ceil(log2 n)+1)
     if (NT / 2 < 8 || NT / 2 > 16384 || NF > 65536 || NF < 4) {
-        set_error("calc_sspec: dynspec %dx%d outside supported FFT sizes", nf, nt);
+        set_error("calc_sspec: dynspec %dx%d outside the supported sizes (nf 2..32768, nt 5..16384)",
+                  nf, nt);
         return SB_ERR_UNSUPPORTED;
     }
     const long pitch = half_pitch(NT);
@@ -849,9 +850,10 @@ static int conj_spectrum_bluestein(const float* dyn, int nf, int nt, int NF, int
                                    const unsigned char* rowmask, float2* CS,
                                    cudaStream_t st) {
     const int MT = next_pow2(2L * NT - 1), MF = next_pow2(2L * NF - 1);
-    if (MT < 8 || MT > 16384 || MF < 4 || MF > 65536) {
-        set_error("conjugate spectrum (Bluestein): padded size %dx%d too large "
-                  "(rows <= 32768, cols <= 8192 for non power-of-two sizes)", NF, NT);
+    // M >= 8 on both axes: bluestein_tables transforms the kernel with a row FFT (>= 8 points)
+    if (MT < 8 || MT > 16384 || MF < 8 || MF > 65536) {
+        set_error("conjugate spectrum (Bluestein): padded size %dx%d unsupported "
+                  "(rows 3..32768, cols 3..8192 for non power-of-two sizes)", NF, NT);
         return SB_ERR_UNSUPPORTED;
     }
     const long pt = ((long)NT + 15) & ~15L;
@@ -904,8 +906,9 @@ static int conj_spectrum_bluestein(const float* dyn, int nf, int nt, int NF, int
 int ifft2_c2c_any(const float2* in, int n0, int n1, int centred, int crop0, int crop1,
                   double scale, int real_only, void* out, cudaStream_t st, int conj_in) {
     const int MT = next_pow2(2L * n1 - 1), MF = next_pow2(2L * n0 - 1);
-    if (n0 < 2 || n1 < 2 || MT < 8 || MT > 16384 || MF < 4 || MF > 65536) {
-        set_error("ifft2 (chirp-z): %d x %d outside 2..32768 x 4..8192", n0, n1);
+    // M >= 8 on both axes: bluestein_tables transforms the kernel with a row FFT (>= 8 points)
+    if (MT < 8 || MT > 16384 || MF < 8 || MF > 65536) {
+        set_error("ifft2 (chirp-z): %d x %d outside 3..32768 x 3..8192", n0, n1);
         return SB_ERR_UNSUPPORTED;
     }
     if (crop0 <= 0 || crop0 > n0) crop0 = n0;
@@ -955,7 +958,8 @@ int acf(const float* dyn, int nf, int nt, int subtract_mean, int normalise,
     ProfScope prof(PROF_ACF, st);
     const int PF = next_pow2(2L * nf), PT = next_pow2(2L * nt);
     if (PT / 2 < 8 || PT / 2 > 16384 || PF > 65536 || PF < 4) {
-        set_error("calc_acf: dynspec %dx%d outside supported FFT sizes", nf, nt);
+        set_error("calc_acf: dynspec %dx%d outside the supported sizes (nf 2..32768, nt 5..16384)",
+                  nf, nt);
         return SB_ERR_UNSUPPORTED;
     }
     const long pitch = half_pitch(PT);

@@ -369,8 +369,9 @@ int ifft2_c2c(const float2* in, int n0, int n1, int centred, int crop0, int crop
               double scale, int real_only, void* out, cudaStream_t st) {
     if ((n0 & (n0 - 1)) || (n1 & (n1 - 1)))
         return ifft2_c2c_any(in, n0, n1, centred, crop0, crop1, scale, real_only, out, st, 0);
-    if (n0 < 8 || n1 < 8 || (n0 & (n0 - 1)) || (n1 & (n1 - 1)) || n0 > 65536 || n1 > 32768) {
-        set_error("ifft2: sizes %d x %d must be powers of two (8..65536 x 8..32768)", n0, n1);
+    // rows run in one shared-memory row transform (SB_ROW_DISPATCH: 8..16384 points)
+    if (n0 < 8 || n1 < 8 || n0 > 65536 || n1 > 16384) {
+        set_error("ifft2: power-of-two sizes %d x %d outside 8..65536 x 8..16384", n0, n1);
         return SB_ERR_UNSUPPORTED;
     }
     if (crop0 <= 0 || crop0 > n0) crop0 = n0;
@@ -438,7 +439,8 @@ template <typename T> struct AmplitudeStore {
     }
 };
 
-// ---- any-size variant on the chirp-z inverse (round-2 candidate, unverified):
+// ---- any-size variant on the chirp-z inverse (fp32; tests/test_gpu_fft_lengths.py holds
+// one iteration to a float64 loop at sizes up to 32768 x 8192):
 //   T = ifft2(conj W) = conj(fft2 W) / N;  zero the masked rows of T;
 //   W = N * ifft2(conj T) = ifft2(masked fft2 W);  amplitude step.
 __global__ void gs_rowmask_kernel(float2* T, const unsigned char* __restrict__ rowmask,
@@ -460,6 +462,12 @@ __global__ void gs_amplitude_kernel(float2* W, const float* __restrict__ amp, lo
 }
 static int gerchberg_saxton_any(float2* W, const float* amp, const unsigned char* rowmask,
                                 int n0, int n1, int niter, cudaStream_t st) {
+    // the limits of ifft2_c2c_any, checked before the workspace is allocated
+    if (n0 < 3 || n1 < 3 || n0 > 32768 || n1 > 8192) {
+        set_error("gerchberg_saxton (chirp-z): wavefield %d x %d outside 3..32768 x 3..8192",
+                  n0, n1);
+        return SB_ERR_UNSUPPORTED;
+    }
     const long count = (long)n0 * n1;
     float2* T = (float2*)workspace(2, (size_t)count * sizeof(float2));
     if (!T) return SB_ERR_NOMEM;
@@ -514,8 +522,10 @@ int gerchberg_saxton(float2* W, const float* amp, const unsigned char* rowmask, 
                      int niter, cudaStream_t st) {
     if ((n0 & (n0 - 1)) || (n1 & (n1 - 1)))
         return gerchberg_saxton_any(W, amp, rowmask, n0, n1, niter, st);
-    if (n0 < 8 || n1 < 8 || (n0 & (n0 - 1)) || (n1 & (n1 - 1)) || n0 > 65536 || n1 > 32768) {
-        set_error("gerchberg_saxton: wavefield %d x %d must have power-of-two sizes", n0, n1);
+    // checked before any workspace is allocated; rows as in ifft2_c2c (8..16384 points)
+    if (n0 < 8 || n1 < 8 || n0 > 65536 || n1 > 16384) {
+        set_error("gerchberg_saxton: power-of-two wavefield %d x %d outside 8..65536 x 8..16384",
+                  n0, n1);
         return SB_ERR_UNSUPPORTED;
     }
     if (n1 > 8192) {                  // fp64 rows of this length do not fit shared memory

@@ -140,7 +140,8 @@ int sim_screen(int nx, int ny, const double* w, const double* n1, const double* 
                unsigned long long seed, double* xyp, cudaStream_t st) {
     ProfScope prof(PROF_SIM_SCREEN, st);
     if (!is_pow2(nx) || !is_pow2(ny) || ny < 8 || ny > 8192 || nx < 4 || nx > 65536) {
-        set_error("Simulation screen: %dx%d unsupported (powers of two, ny 8..8192)", nx, ny);
+        set_error("Simulation screen: %dx%d unsupported (powers of two, nx 4..65536, ny 8..8192)",
+                  nx, ny);
         return SB_ERR_UNSUPPORTED;
     }
     double2* B1 = (double2*)workspace(3, (size_t)nx * ny * sizeof(double2));
