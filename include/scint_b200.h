@@ -156,6 +156,38 @@ int sb_rev_map(const void* thth, int32_t n, const double* th_cents, double eta, 
 int sb_herm_eigvec(const void* a, int32_t n, int32_t ld, double tol, int32_t max_iter,
                    double* w, void* v, int32_t* info, void* stream);
 
+/* Replaces the curvature loop of the chi-square search (scintools/examples/
+ * THTHSample.ipynb, "Chisquared Search"), i.e. neta calls of ththmod.chisq_calc
+ * (:330-368 -> modeler :261-327 hermitian branch -> thth_redmap, eigsh(k=1,
+ * which='LA'), rev_map of |w| V V^H, ifft2(ifftshift(recov)).real), without the
+ * division by N:
+ *   ssq[e] = sum over mask of (model_e[:nf, :nt] - dspec)^2   (float64).
+ * geom: as sb_eta_sweep (full or half-plane CS, coherent), etas: device float64
+ * [neta].  th_red: device float64 [neta][n_th], row e holding the nred[e]
+ * rev_map centres of curvature e (theta_centres of its edges_red,
+ * ththmod.py:204-205), evaluated by the host with the reference's expressions.
+ * dtau_bin = tau[1] - tau[0], dfd_bin = fd[1] - fd[0]: the histogram bin widths
+ * of rev_map (:210-215; tau[0] and fd[0] come from geom).  dspec: float32
+ * [nf][nt] with nf <= ntau, nt <= nfd; mask: uint8 [nf][nt] (non-zero = use)
+ * or NULL for isfinite(dspec).  tol (<= 0: 1e-7) and max_iter (<= 0: 96) as
+ * sb_herm_eigvec.  The eigenpair Lanczos starts from row n//2; if that row is
+ * zero it starts from a fixed non-zero vector (eigsh starts from a random one).
+ * Outputs (device, [neta] each): ssq float64 (NaN where chisq_calc raises:
+ * status bits SB_ETA_INDEX_ERROR, SB_ETA_ZERO_START = the matrix is zero --
+ * ARPACK's "starting vector is zero" --, SB_ETA_TOO_SMALL); w float64 (top
+ * eigenvalue, NaN for INDEX_ERROR / TOO_SMALL, 0 for a zero matrix); status
+ * (SB_ETA_* bits; SB_ETA_NOT_CONVERGED keeps its ssq); nred (cropped size);
+ * iters (Lanczos steps).  Curvatures run in batches whose buffers (matrix,
+ * Lanczos basis and a few CS-sized arrays per curvature) fit the 3 GiB budget
+ * of sb_eta_sweep (SB_SWEEP_SLAB_MB overrides it).  Errors: SB_ERR_ARG if dspec
+ * is larger than the CS; SB_ERR_UNSUPPORTED for more than 4096 theta centres
+ * or CS sizes outside those of sb_ifft2_c2c_f32. */
+int sb_chisq_sweep(const sb_thth_geom* geom, const double* etas, int32_t neta,
+                   const double* th_red, double dtau_bin, double dfd_bin, const float* dspec,
+                   int32_t nf, int32_t nt, const uint8_t* mask, double tol, int32_t max_iter,
+                   double* ssq, double* w, int32_t* status, int32_t* nred, int32_t* iters,
+                   void* stream);
+
 /* out[:crop0, :crop1] = scale * ifft2(ifftshift(in)) (centred != 0) or
  * scale * ifft2(in), in: float2 [n0][n1] (ththmod.py:321, :1462-1465).  Powers of two
  * up to 65536 x 16384 (n0 x n1, both >= 8) take the radix path; any other size up to

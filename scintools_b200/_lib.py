@@ -70,6 +70,8 @@ _SIGS = {
     "sb_rev_map": (c_int, [vp, c_int, vp, c_dbl, c_dbl, c_dbl, c_int, c_dbl, c_dbl, c_int,
                            c_int, vp, vp]),
     "sb_herm_eigvec": (c_int, [vp, c_int, c_int, c_dbl, c_int, vp, vp, vp, vp]),
+    "sb_chisq_sweep": (c_int, [ctypes.POINTER(ThthGeom), vp, c_int, vp, c_dbl, c_dbl, vp,
+                               c_int, c_int, vp, c_dbl, c_int, vp, vp, vp, vp, vp, vp]),
     "sb_gerchberg_saxton_f32": (c_int, [vp, vp, vp, c_int, c_int, c_int, vp]),
     "sb_scale_dyn_lambda_f32": (c_int, [vp, c_int, c_int, c_int, vp, vp, vp, vp, c_flt, c_flt,
                                         vp, vp, c_int, vp, vp]),

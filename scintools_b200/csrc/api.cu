@@ -146,6 +146,11 @@ int herm_eigvec(const float2* A, int n, int ld, double tol, int max_iter, double
                 float2* V_dev, int* info_dev, cudaStream_t st);
 int ifft2_c2c(const float2* in, int n0, int n1, int centred, int crop0, int crop1,
               double scale, int real_only, void* out, cudaStream_t st);
+int chisq_sweep(const ThthGeom& g, const double* th_host, const double* d_etas, int neta,
+                const double* d_th_red, double dtau_bin, double dfd_bin, const float* dspec,
+                const unsigned char* mask, int nf, int nt, double tol, int max_iter,
+                double* d_ssq, double* d_w, int* d_status, int* d_nred, int* d_iters,
+                cudaStream_t st);
 
 int gerchberg_saxton(float2* W, const float* amp, const unsigned char* rowmask, int n0, int n1,
                      int niter, cudaStream_t st);
@@ -194,7 +199,7 @@ static int to_geom(const sb_thth_geom* in, ThthGeom* g) {
 
 extern "C" {
 
-int sb_abi_version(void) { return 2; }
+int sb_abi_version(void) { return 3; }
 const char* sb_last_error(void) { return sb::last_error(); }
 
 int sb_init(int device) {
@@ -322,6 +327,21 @@ int sb_ifft2_c2c_f32(const void* in, int32_t n0, int32_t n1, int32_t centred, in
     SB_ARG(in && out);
     return sb::ifft2_c2c((const float2*)in, n0, n1, centred, crop0, crop1, scale, real_only,
                          out, (cudaStream_t)stream);
+}
+
+int sb_chisq_sweep(const sb_thth_geom* geom, const double* etas, int32_t neta,
+                   const double* th_red, double dtau_bin, double dfd_bin, const float* dspec,
+                   int32_t nf, int32_t nt, const uint8_t* mask, double tol, int32_t max_iter,
+                   double* ssq, double* w, int32_t* status, int32_t* nred, int32_t* iters,
+                   void* stream) {
+    sb::ThthGeom g;
+    int rc = sb::to_geom(geom, &g);
+    if (rc) return rc;
+    SB_ARG(neta >= 0 && etas && th_red && dspec && ssq && w && status && nred && iters);
+    SB_ARG(geom->cs != nullptr);
+    return sb::chisq_sweep(g, geom->th_cents_host, etas, neta, th_red, dtau_bin, dfd_bin, dspec,
+                           mask, nf, nt, tol, max_iter, ssq, w, status, nred, iters,
+                           (cudaStream_t)stream);
 }
 
 int sb_gerchberg_saxton_f32(void* wavefield, const float* amp, const uint8_t* rowmask,

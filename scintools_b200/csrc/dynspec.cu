@@ -14,6 +14,7 @@
 
 #include "fft_kernels.cuh"
 #include "chirp.cuh"
+#include "chisq.cuh"
 
 namespace sb {
 
@@ -903,16 +904,18 @@ static int conj_spectrum_bluestein(const float* dyn, int nf, int nt, int NF, int
 // ------------------------------------------------------------------------
 // conj_in != 0: returns ifft2(conj(in)) = conj(fft2(in)) / (n0 n1) (used for the
 // forward transform of the Gerchberg-Saxton loop)
-int ifft2_c2c_any(const float2* in, int n0, int n1, int centred, int crop0, int crop1,
-                  double scale, int real_only, void* out, cudaStream_t st, int conj_in) {
+// the chirp-z inverse of ifft2_c2c_any up to its final column pass, whose store is
+// mk(R1, wF, MF * n0 * n1) (wF: chirp of the column axis, the last argument the divisor
+// that normalises the transform); columns >= ncols are never stored
+template <class MakeStore>
+static int ifft2_any_core(const float2* in, int n0, int n1, int centred, int ncols, int conj_in,
+                          MakeStore mk, cudaStream_t st) {
     const int MT = next_pow2(2L * n1 - 1), MF = next_pow2(2L * n0 - 1);
     // M >= 8 on both axes: bluestein_tables transforms the kernel with a row FFT (>= 8 points)
     if (MT < 8 || MT > 16384 || MF < 8 || MF > 65536) {
         set_error("ifft2 (chirp-z): %d x %d outside 3..32768 x 3..8192", n0, n1);
         return SB_ERR_UNSUPPORTED;
     }
-    if (crop0 <= 0 || crop0 > n0) crop0 = n0;
-    if (crop1 <= 0 || crop1 > n1) crop1 = n1;
     const long pt = ((long)n1 + 15) & ~15L;
     float2* tabs = (float2*)workspace(6, (size_t)(n1 + 3L * MT + n0 + 3L * MF + 64) * sizeof(float2));
     float2* R1buf = (float2*)workspace(3, (size_t)n0 * MT * sizeof(float2));
@@ -943,13 +946,44 @@ int ifft2_c2c_any(const float2* in, int n0, int n1, int centred, int crop0, int 
     split_len(MF, &R1, &R2);
     ChirpColALoad la{Ybuf, pt, R2, n0, wF};
     MulVecColStore mc{C1, pt, R1, BF};
-    rc = cols_generic_f<-1>(la, C0, pt, MF, crop1, mc, st);
+    rc = cols_generic_f<-1>(la, C0, pt, MF, ncols, mc, st);
     if (rc) return rc;
     PlainColALoad pa{C1, pt, R2};
-    ChirpCropStore cs{real_only ? nullptr : (float2*)out, real_only ? (float*)out : nullptr, R1,
-                      crop0, crop1, wF,
-                      (float)(scale / ((double)MF * (double)n0 * (double)n1))};
-    return cols_generic_f<+1>(pa, C0, pt, MF, crop1, cs, st);
+    return cols_generic_f<+1>(pa, C0, pt, MF, ncols, mk(R1, wF, (double)MF * (double)n0 * (double)n1),
+                              st);
+}
+
+int ifft2_c2c_any(const float2* in, int n0, int n1, int centred, int crop0, int crop1,
+                  double scale, int real_only, void* out, cudaStream_t st, int conj_in) {
+    if (crop0 <= 0 || crop0 > n0) crop0 = n0;
+    if (crop1 <= 0 || crop1 > n1) crop1 = n1;
+    return ifft2_any_core(in, n0, n1, centred, crop1, conj_in,
+                          [&](int R1, const float2* wF, double den) {
+                              return ChirpCropStore{real_only ? nullptr : (float2*)out,
+                                                    real_only ? (float*)out : nullptr, R1,
+                                                    crop0, crop1, wF, (float)(scale / den)};
+                          }, st);
+}
+
+// chisq_sweep (retrieval.cu): sum over the mask of (real(ifft2(ifftshift(in)))[:nf, :nt] -
+// dspec)^2 for any size, added to the sink's partial sums
+struct ChirpResidualStore {
+    int R1;
+    const float2* w;
+    float scale;
+    ResidualSink sink;
+    __device__ __forceinline__ void operator()(int y, int k, int c, float2 v) const {
+        const int kf = y + R1 * k;
+        if (kf >= sink.nf || c >= sink.nt) return;
+        sink(kf, c, cmul(v, w[kf]).x * scale);
+    }
+};
+int ifft2_any_residual(const float2* in, int n0, int n1, const ResidualSink& sink,
+                       cudaStream_t st) {
+    return ifft2_any_core(in, n0, n1, 1, sink.nt, 0,
+                          [&](int R1, const float2* wF, double den) {
+                              return ChirpResidualStore{R1, wF, (float)(1.0 / den), sink};
+                          }, st);
 }
 
 // Dynspec.calc_acf(method='direct') (dynspec.py:3780-3797)

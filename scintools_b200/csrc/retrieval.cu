@@ -3,13 +3,16 @@
 //   herm_eigvec  ththmod.py:300-307   top eigenpair of the reduced theta-theta
 //                                     matrix (eigsh(.., 1, which='LA') in modeler)
 //   ifft2        ththmod.py:321, 1462 ifft2(ifftshift(recov)), cropped
-// used by the Python mirrors of modeler / single_chunk_retrieval.
+//   chisq_sweep  ththmod.py:330-368   chisq_calc over a batch of curvatures
+// used by the Python mirrors of modeler / single_chunk_retrieval / chisq_calc.
 #include <float.h>
 #include <math.h>
 #include <stdlib.h>
 
 #ifndef SB_HOST_EMU            // tests/host_emu runs the scatter / eigenpair kernels on the CPU
+#include "chisq.cuh"
 #include "fft_generic.cuh"
+#include "thth.cuh"
 #endif
 #include "lanczos.cuh"
 
@@ -44,6 +47,35 @@ struct RevGeom {
     int ntau, nfd;
 };
 
+// point (i, j), i != j, of the theta-theta matrix with value v into the histograms
+__device__ __forceinline__ void rev_scatter_point(const RevGeom& g, int i, int j, float2 v,
+                                                  int hermitian, float2* __restrict__ acc,
+                                                  int* __restrict__ cnt) {
+    const double ti = g.th[i], tj = g.th[j];
+    // fd_map[i][j] = th[j] - th[i];  tau_map = eta * (th[j]^2 - th[i]^2)
+    const double x = __dsub_rn(tj, ti);
+    const double y = __dmul_rn(g.eta, __dsub_rn(__dmul_rn(tj, tj), __dmul_rn(ti, ti)));
+    const double jac = sqrt(fabs(__dmul_rn(__dmul_rn(2.0, g.eta), __dsub_rn(ti, tj))));
+    const float wre = (float)((double)v.x / jac), wim = (float)((double)v.y / jac);
+    int bx = hist_bin(x, g.fd0, g.dfd, g.nfd), by = hist_bin(y, g.tau0, g.dtau, g.ntau);
+    if (bx >= 0 && by >= 0) {
+        const size_t o = (size_t)by * g.nfd + bx;
+        atomicAdd(&acc[o].x, wre);
+        atomicAdd(&acc[o].y, wim);
+        atomicAdd(&cnt[o], 1);
+    }
+    if (hermitian) {
+        bx = hist_bin(-x, g.fd0, g.dfd, g.nfd);
+        by = hist_bin(-y, g.tau0, g.dtau, g.ntau);
+        if (bx >= 0 && by >= 0) {
+            const size_t o = (size_t)by * g.nfd + bx;
+            atomicAdd(&acc[o].x, wre);
+            atomicAdd(&acc[o].y, -wim);
+            atomicAdd(&cnt[o], 1);
+        }
+    }
+}
+
 __global__ void rev_scatter_kernel(RevGeom g, const float2* __restrict__ thth, int hermitian,
                                    float2* __restrict__ acc, int* __restrict__ cnt) {
     const long total = (long)g.n * g.n;
@@ -51,56 +83,83 @@ __global__ void rev_scatter_kernel(RevGeom g, const float2* __restrict__ thth, i
          p += (long)gridDim.x * blockDim.x) {
         const int i = (int)(p / g.n), j = (int)(p - (long)i * g.n);
         if (i == j) continue;   // zero Jacobian: the DC bin is NaN -> 0 (finalise kernel)
-        const double ti = g.th[i], tj = g.th[j];
-        // fd_map[i][j] = th[j] - th[i];  tau_map = eta * (th[j]^2 - th[i]^2)
-        const double x = __dsub_rn(tj, ti);
-        const double y = __dmul_rn(g.eta, __dsub_rn(__dmul_rn(tj, tj), __dmul_rn(ti, ti)));
-        const double jac = sqrt(fabs(__dmul_rn(__dmul_rn(2.0, g.eta), __dsub_rn(ti, tj))));
-        const float2 v = thth[p];
-        const float wre = (float)((double)v.x / jac), wim = (float)((double)v.y / jac);
-        int bx = hist_bin(x, g.fd0, g.dfd, g.nfd), by = hist_bin(y, g.tau0, g.dtau, g.ntau);
-        if (bx >= 0 && by >= 0) {
-            const size_t o = (size_t)by * g.nfd + bx;
-            atomicAdd(&acc[o].x, wre);
-            atomicAdd(&acc[o].y, wim);
-            atomicAdd(&cnt[o], 1);
-        }
-        if (hermitian) {
-            bx = hist_bin(-x, g.fd0, g.dfd, g.nfd);
-            by = hist_bin(-y, g.tau0, g.dtau, g.ntau);
-            if (bx >= 0 && by >= 0) {
-                const size_t o = (size_t)by * g.nfd + bx;
-                atomicAdd(&acc[o].x, wre);
-                atomicAdd(&acc[o].y, -wim);
-                atomicAdd(&cnt[o], 1);
-            }
-        }
+        rev_scatter_point(g, i, j, thth[p], hermitian, acc, cnt);
     }
+}
+
+// the bin of (fd, tau) = (0, 0) receives the n diagonal points with an infinite / NaN
+// weight: NaN after the division, 0 after nan_to_num.  Its index, or -1.
+__device__ __forceinline__ long rev_dc_bin(const RevGeom& g) {
+    const int bx0 = hist_bin(0.0, g.fd0, g.dfd, g.nfd), by0 = hist_bin(0.0, g.tau0, g.dtau, g.ntau);
+    return (bx0 >= 0 && by0 >= 0) ? (long)by0 * g.nfd + bx0 : -1;
+}
+// bin mean of rev_map (recov /= norm; nan_to_num) from the weighted sum and the count
+__device__ __forceinline__ float2 rev_bin_value(float2 v, int c, bool dc) {
+    if (c > 0 && !dc) {
+        const float s = 1.0f / (float)c;
+        v.x *= s;
+        v.y *= s;
+        // np.nan_to_num(recov): NaN -> 0, +-inf -> +-largest float
+        v.x = (v.x != v.x) ? 0.f : fminf(fmaxf(v.x, -FLT_MAX), FLT_MAX);
+        v.y = (v.y != v.y) ? 0.f : fminf(fmaxf(v.y, -FLT_MAX), FLT_MAX);
+        return v;
+    }
+    return make_float2(0.f, 0.f);
 }
 
 __global__ void rev_finalise_kernel(RevGeom g, float2* __restrict__ acc,
                                     const int* __restrict__ cnt) {
     const long total = (long)g.ntau * g.nfd;
-    // the bin of (fd, tau) = (0, 0) receives the n diagonal points with an
-    // infinite / NaN weight: NaN after the division, 0 after nan_to_num
-    const int bx0 = hist_bin(0.0, g.fd0, g.dfd, g.nfd), by0 = hist_bin(0.0, g.tau0, g.dtau, g.ntau);
-    const long dc = (bx0 >= 0 && by0 >= 0) ? (long)by0 * g.nfd + bx0 : -1;
+    const long dc = rev_dc_bin(g);
     for (long o = blockIdx.x * (long)blockDim.x + threadIdx.x; o < total;
-         o += (long)gridDim.x * blockDim.x) {
-        const int c = cnt[o];
-        float2 v = acc[o];
-        if (c > 0 && o != dc) {
-            const float s = 1.0f / (float)c;
-            v.x *= s;
-            v.y *= s;
-            // np.nan_to_num(recov): NaN -> 0, +-inf -> +-largest float
-            v.x = (v.x != v.x) ? 0.f : fminf(fmaxf(v.x, -FLT_MAX), FLT_MAX);
-            v.y = (v.y != v.y) ? 0.f : fminf(fmaxf(v.y, -FLT_MAX), FLT_MAX);
-        } else {
-            v = make_float2(0.f, 0.f);
-        }
-        acc[o] = v;
+         o += (long)gridDim.x * blockDim.x)
+        acc[o] = rev_bin_value(acc[o], cnt[o], o == dc);
+}
+
+// --------------------------------------------------------------------------
+// chisq_sweep: rev_map of the rank-1 model |w| V V^H of every curvature of a batch
+// (blockIdx.y), computed on the fly from V; the model matrix is never stored.
+// th_red [neta][th_pitch]: the curvature's rev_map centres (theta_centres of its
+// edges_red), nred[e] of them.  Curvatures whose matrix failed (status bits 1, 2, 4)
+// scatter nothing: their model is zero.
+// --------------------------------------------------------------------------
+__global__ void rev_scatter_rank1_kernel(RevGeom g, const double* __restrict__ th_red,
+                                         int th_pitch, const double* __restrict__ etas, int e0,
+                                         const int* __restrict__ nred,
+                                         const int* __restrict__ status,
+                                         const double* __restrict__ w,
+                                         const float2* __restrict__ V, int ldv,
+                                         float2* __restrict__ acc, int* __restrict__ cnt) {
+    const int e = blockIdx.y;
+    if (status[e0 + e] & 7) return;
+    g.n = nred[e0 + e];
+    g.th = th_red + (size_t)(e0 + e) * th_pitch;
+    g.eta = etas[e0 + e];
+    const float aw = (float)fabs(w[e0 + e]);
+    const float2* v = V + (size_t)e * ldv;
+    const size_t bins = (size_t)g.ntau * g.nfd;
+    acc += e * bins;
+    cnt += e * bins;
+    const long total = (long)g.n * g.n;
+    for (long p = blockIdx.x * (long)blockDim.x + threadIdx.x; p < total;
+         p += (long)gridDim.x * blockDim.x) {
+        const int i = (int)(p / g.n), j = (int)(p - (long)i * g.n);
+        if (i == j) continue;
+        const float2 a = v[i], b = v[j];        // |w| V_i conj(V_j)
+        const float2 t = make_float2(aw * (a.x * b.x + a.y * b.y), aw * (a.y * b.x - a.x * b.y));
+        rev_scatter_point(g, i, j, t, 1, acc, cnt);
     }
+}
+
+__global__ void rev_finalise_batch_kernel(RevGeom g, float2* __restrict__ acc,
+                                          const int* __restrict__ cnt) {
+    const long total = (long)g.ntau * g.nfd;
+    const long dc = rev_dc_bin(g);
+    acc += blockIdx.y * (size_t)total;
+    cnt += blockIdx.y * (size_t)total;
+    for (long o = blockIdx.x * (long)blockDim.x + threadIdx.x; o < total;
+         o += (long)gridDim.x * blockDim.x)
+        acc[o] = rev_bin_value(acc[o], cnt[o], o == dc);
 }
 
 #ifndef SB_HOST_EMU
@@ -152,10 +211,35 @@ __device__ __forceinline__ double ev_block_sum(double x, double* red) {
     return s;
 }
 
-__global__ void __launch_bounds__(EV_THREADS)
-herm_eigvec_kernel(const float2* __restrict__ A, int n, int ld, float2* __restrict__ Q,
-                   int max_iter, double tol, double* __restrict__ w_out,
-                   float2* __restrict__ V_out, int* __restrict__ info) {
+// element (a, c) of a full row-major matrix
+struct FullMatrix {
+    const float2* A;
+    int ld;
+    __device__ __forceinline__ float2 operator()(int a, int c) const { return A[(size_t)a * ld + c]; }
+};
+// element (a, c) of a Hermitian matrix with zero diagonal stored as its strict upper
+// triangle (thth_build_kernel<PACK = 0>): the lower triangle is the conjugate mirror
+struct UpperHermitian {
+    const float2* M;
+    int ld;
+    __device__ __forceinline__ float2 operator()(int a, int c) const {
+        if (c > a) return M[(size_t)a * ld + c];
+        if (c < a) {
+            const float2 x = M[(size_t)c * ld + a];
+            return make_float2(x.x, -x.y);
+        }
+        return make_float2(0.f, 0.f);
+    }
+};
+
+// Shared body.  Start vector: row n//2.  If that row is zero, zero_start_fallback == 0
+// reports it (w = NaN, info[1] = 2); otherwise Lanczos starts from a fixed non-zero
+// vector instead, and a start vector that A maps to zero (for a zero-diagonal Hermitian
+// matrix: A == 0) gives w = 0 with that vector as V and info[1] = 2.
+template <class Mat>
+__device__ void herm_eigvec_body(Mat A, int n, float2* __restrict__ Q, int max_iter, double tol,
+                                 int zero_start_fallback, double* __restrict__ w_out,
+                                 float2* __restrict__ V_out, int* __restrict__ info) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     LanczosShared& S = *reinterpret_cast<LanczosShared*>(smem_raw);
     double* red = reinterpret_cast<double*>(smem_raw + sizeof(LanczosShared));   // [EV_NW]
@@ -170,7 +254,7 @@ herm_eigvec_kernel(const float2* __restrict__ A, int n, int ld, float2* __restri
     const int h = n / 2;
     double p0 = 0.0;
     for (int c = tid; c < n; c += EV_THREADS) {
-        const float2 x = A[(size_t)h * ld + c];
+        const float2 x = A(h, c);
         v[c] = x;
         p0 += (double)x.x * x.x + (double)x.y * x.y;
     }
@@ -178,7 +262,16 @@ herm_eigvec_kernel(const float2* __restrict__ A, int n, int ld, float2* __restri
         S.done = 0; S.lo = 0.0; S.theta = 0.0; S.res = 0.0; S.next_check = 1; S.m_last = 0; S.beta2[0] = 0.0;
         S.m_lo2 = 0; S.lo2 = 0.0;
     }
-    const double nrm2 = ev_block_sum(p0, red);
+    double nrm2 = ev_block_sum(p0, red);
+    const bool fallback = zero_start_fallback && nrm2 == 0.0 && n >= 2;
+    if (fallback) {
+        p0 = 0.0;
+        for (int c = tid; c < n; c += EV_THREADS) {
+            v[c] = make_float2(1.0f + 0.125f * (float)((c * 37) % 11), 0.f);
+            p0 += (double)v[c].x * v[c].x;
+        }
+        nrm2 = ev_block_sum(p0, red);
+    }
     if (!(nrm2 > 0.0) || !isfinite(nrm2) || n < 2) {
         if (tid == 0) { *w_out = qnan; info[0] = 0; info[1] = 2; }
         for (int c = tid; c < n; c += EV_THREADS) V_out[c] = make_float2(0.f, 0.f);
@@ -195,10 +288,9 @@ herm_eigvec_kernel(const float2* __restrict__ A, int n, int ld, float2* __restri
         for (int c = tid; c < n; c += EV_THREADS) Q[(size_t)it * n + c] = v[c];
         // w = A v : one warp per row, lanes across the columns
         for (int a = warp; a < n; a += EV_NW) {
-            const float2* row = A + (size_t)a * ld;
             float rx = 0.f, ry = 0.f;
             for (int c = lane; c < n; c += 32) {
-                const float2 q = row[c], x = v[c];
+                const float2 q = A(a, c), x = v[c];
                 rx = fmaf(q.x, x.x, rx); rx = fmaf(-q.y, x.y, rx);
                 ry = fmaf(q.x, x.y, ry); ry = fmaf(q.y, x.x, ry);
             }
@@ -259,6 +351,12 @@ herm_eigvec_kernel(const float2* __restrict__ A, int n, int ld, float2* __restri
         const double b2 = ev_block_sum(bp, red);
         const double beta = sqrt(b2);
         m = it + 1;
+        if (fallback && it == 0 && alpha == 0.0 && b2 == 0.0) {
+            // A v = 0 for the fallback vector: report w = 0, V = v
+            for (int c = tid; c < n; c += EV_THREADS) V_out[c] = v[c];
+            if (tid == 0) { *w_out = 0.0; info[0] = 1; info[1] = 2; }
+            return;
+        }
         if (tid == 0) { S.alpha[it] = alpha; S.beta[m] = beta; S.beta2[m] = b2; }
         __syncthreads();
         if (warp == 0) lanczos_check(S, m, tol, 0.0);
@@ -308,6 +406,41 @@ herm_eigvec_kernel(const float2* __restrict__ A, int n, int ld, float2* __restri
         // residual <= 2e-6 |theta| at the iteration cap is still a converged pair for every
         // consumer (eigenvalue error ~ res^2 / gap), anything worse is flagged
         info[1] = (S.done || S.res <= 2e-6 * fabs(S.theta)) ? 0 : 8;
+    }
+}
+
+__global__ void __launch_bounds__(EV_THREADS)
+herm_eigvec_kernel(const float2* __restrict__ A, int n, int ld, float2* __restrict__ Q,
+                   int max_iter, double tol, double* __restrict__ w_out,
+                   float2* __restrict__ V_out, int* __restrict__ info) {
+    herm_eigvec_body(FullMatrix{A, ld}, n, Q, max_iter, tol, 0, w_out, V_out, info);
+}
+
+// chisq_sweep: the top eigenpair of every cropped theta-theta matrix of a batch, one CTA per
+// curvature (blockIdx.x), on the strict upper triangles M [nb][ld][ld] of the sweep's gather.
+// Q: [nb][max_iter + 1][ld] Lanczos bases; V: [nb][ld].  Writes w (NaN where the reference
+// raises), iters and the SB_ETA_* bits of curvatures e0 .. e0 + nb - 1.
+__global__ void __launch_bounds__(EV_THREADS)
+herm_eigvec_batch_kernel(const float2* __restrict__ M, int ld, const int* __restrict__ nred,
+                         int e0, float2* __restrict__ Q, int max_iter, double tol,
+                         double* __restrict__ w, float2* __restrict__ V,
+                         int* __restrict__ status, int* __restrict__ iters) {
+    const int e = blockIdx.x, ge = e0 + e;
+    const int n = nred[ge];
+    if ((status[ge] & 1) || n < 3) {          // IndexError / eigsh raises for n < 3
+        if (threadIdx.x == 0) {
+            w[ge] = __longlong_as_double(0x7ff8000000000000LL);
+            iters[ge] = 0;
+            if (n < 3) status[ge] |= 4;
+        }
+        return;
+    }
+    __shared__ int info[2];
+    herm_eigvec_body(UpperHermitian{M + (size_t)e * ld * ld, ld}, n, Q + (size_t)e * (max_iter + 1) * ld,
+                     max_iter, tol, 1, w + ge, V + (size_t)e * ld, info);
+    if (threadIdx.x == 0) {        // info was written by thread 0 of the body
+        iters[ge] = info[0];
+        status[ge] |= info[1];
     }
 }
 
@@ -390,6 +523,162 @@ int ifft2_c2c(const float2* in, int n0, int n1, int centred, int crop0, int crop
     CropStore cs{real_only ? nullptr : (float2*)out, real_only ? (float*)out : nullptr, R1,
                  crop0, crop1, (float)(scale / ((double)n0 * (double)n1))};
     return cols_generic<float, +1>(la, B2, n1, n0, crop1, cs, st);
+}
+
+// --------------------------------------------------------------------------
+// ththmod.chisq_calc over a grid of curvatures (ththmod.py:330-368 with modeler
+// :261-327): per curvature the cropped theta-theta matrix, its top eigenpair, the
+// rank-1 model scattered back into the conjugate spectrum, ifft2(ifftshift(.)) and
+// sum over the mask of (model[:nf, :nt] - dspec)^2.  One launch sequence per batch of
+// curvatures, no host synchronisation.
+// --------------------------------------------------------------------------
+struct BatchShiftedRowLoad {   // row r of ifftshift(in[e]) for row = e * n0 + r (powers of two)
+    const float2* in;
+    int n0, n1;
+    __device__ __forceinline__ float2 operator()(long row, int n) const {
+        const long e = row / n0;
+        const int r = (int)((row - e * n0 + n0 / 2) & (n0 - 1));
+        const int c = (n + n1 / 2) & (n1 - 1);
+        return in[((size_t)e * n0 + r) * n1 + c];
+    }
+};
+struct ResidualStore {         // real part of out[k][c], k = k1 + R1 k2, into the sink
+    int R1;
+    float scale;
+    ResidualSink sink;
+    __device__ __forceinline__ void operator()(int y, int k, int c, float2 v) const {
+        sink(y + R1 * k, c, v.x * scale);
+    }
+};
+__global__ void chisq_finish_kernel(const double* __restrict__ part, int e0, int nb,
+                                    const int* __restrict__ status, double* __restrict__ ssq) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= nb) return;
+    double s = 0.0;
+    for (int k = 0; k < CHISQ_SLOTS; ++k) s += part[(size_t)e * CHISQ_SLOTS + k];
+    // the reference raises for these curvatures (IndexError, ARPACK error, n < 3)
+    ssq[e0 + e] = (status[e0 + e] & 7) ? __longlong_as_double(0x7ff8000000000000LL) : s;
+}
+
+// thth.cu / dynspec.cu
+int thth_prep(const ThthGeom& g, const double* th_host, const double* d_etas, int neta, int ld,
+              int* d_idx, int* d_nred, int* d_status, cudaStream_t st);
+int thth_build_f32(const ThthGeom& g, const double* d_etas, int e0, int nb, int ld,
+                   const int* d_idx, const int* d_nred, float2* d_M, cudaStream_t st);
+unsigned long long sweep_slab_bytes();
+int ifft2_any_residual(const float2* in, int n0, int n1, const ResidualSink& sink,
+                       cudaStream_t st);
+
+int chisq_sweep(const ThthGeom& g, const double* th_host, const double* d_etas, int neta,
+                const double* d_th_red, double dtau_bin, double dfd_bin, const float* dspec,
+                const unsigned char* mask, int nf, int nt, double tol, int max_iter,
+                double* d_ssq, double* d_w, int* d_status, int* d_nred, int* d_iters,
+                cudaStream_t st) {
+    if (g.n > 4096) {
+        set_error("chisq_sweep: theta-theta grid of %d centres exceeds the supported 4096", g.n);
+        return SB_ERR_UNSUPPORTED;
+    }
+    const int n0 = (int)g.ntau, n1 = (int)g.nfd;
+    if (nf < 1 || nt < 1 || nf > n0 || nt > n1) {
+        set_error("chisq_sweep: dynamic spectrum %d x %d is empty or larger than the conjugate "
+                  "spectrum %d x %d", nf, nt, n0, n1);
+        return SB_ERR_ARG;
+    }
+    if (!(dtau_bin > 0.0) || !(dfd_bin > 0.0)) {
+        set_error("chisq_sweep needs ascending tau / fd axes (bins must increase monotonically)");
+        return SB_ERR_ARG;
+    }
+    const bool pow2 = !(n0 & (n0 - 1)) && !(n1 & (n1 - 1));
+    if (pow2 ? (n0 < 8 || n1 < 8 || n0 > 65536 || n1 > 16384)
+             : (n0 < 3 || n1 < 3 || n0 > 32768 || n1 > 8192)) {
+        set_error("chisq_sweep: conjugate spectrum %d x %d outside 8..65536 x 8..16384 (powers "
+                  "of two) / 3..32768 x 3..8192 (other sizes)", n0, n1);
+        return SB_ERR_UNSUPPORTED;
+    }
+    if (neta <= 0) return SB_OK;
+    if (!(tol > 0.0)) tol = 1e-7;
+    if (max_iter <= 0 || max_iter > SB_LANCZOS_MAXIT) max_iter = 96;
+    const int ld = (g.n + 31) / 32 * 32;
+    if (max_iter > ld) max_iter = ld;
+    int* d_idx = (int*)workspace(1, (size_t)neta * ld * sizeof(int));
+    if (!d_idx) return SB_ERR_NOMEM;
+    int rc = thth_prep(g, th_host, d_etas, neta, ld, d_idx, d_nred, d_status, st);
+    if (rc) return rc;
+    // per curvature: matrix, Lanczos basis, eigenvector, bin sums, partial sums, counts
+    // (+ the row-transformed spectrum on the radix path), all under the sweep's slab budget
+    const size_t bins = (size_t)n0 * n1;
+    const size_t mat = (size_t)ld * ld, qn = (size_t)(max_iter + 1) * ld;
+    const size_t per = (mat + qn + ld + bins) * sizeof(float2) + CHISQ_SLOTS * sizeof(double) +
+                       bins * sizeof(int) + (pow2 ? bins * sizeof(float2) : 0);
+    unsigned long long b = sweep_slab_bytes() / per;
+    int batch = (int)(b < 1 ? 1 : (b > 65535 ? 65535 : b));
+    if (batch > neta) batch = neta;
+    unsigned char* ws = (unsigned char*)workspace(2, per * batch);
+    if (!ws) return SB_ERR_NOMEM;
+    float2* M = (float2*)ws;
+    float2* Q = M + mat * batch;
+    float2* V = Q + qn * batch;
+    float2* acc = V + (size_t)ld * batch;
+    double* part = (double*)(acc + bins * batch);
+    int* cnt = (int*)(part + (size_t)CHISQ_SLOTS * batch);
+    float2 *B1 = nullptr, *B2 = nullptr;
+    if (pow2) {
+        B1 = (float2*)workspace(3, bins * batch * sizeof(float2));
+        B2 = (float2*)workspace(4, bins * sizeof(float2));
+        if (!B1 || !B2) return SB_ERR_NOMEM;
+    }
+    const size_t smem = sizeof(LanczosShared) + 32 * sizeof(double) +
+                        (SB_LANCZOS_MAXIT + 1) * sizeof(double2) + 2 * (size_t)ld * sizeof(float2);
+    SB_CUDA(cudaFuncSetAttribute(herm_eigvec_batch_kernel,
+                                 cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    // rev_map bins: tau[0], tau[1] - tau[0], fd[0], fd[1] - fd[0] (ththmod.py:210-215)
+    const RevGeom rg{nullptr, 0, 0.0, g.tau0, dtau_bin, g.fd0, dfd_bin, n0, n1};
+    int sb_ = (int)((mat + 255) / 256), fb = (int)((bins + 255) / 256);
+    sb_ = sb_ > 256 ? 256 : sb_;
+    fb = fb > 1024 ? 1024 : fb;
+    int R1, R2;
+    split_len(n0, &R1, &R2);
+    const float scale = (float)(1.0 / ((double)n0 * (double)n1));
+    for (int e0 = 0; e0 < neta; e0 += batch) {
+        const int nb = neta - e0 < batch ? neta - e0 : batch;
+        rc = thth_build_f32(g, d_etas, e0, nb, ld, d_idx, d_nred, M, st);
+        if (rc) return rc;
+        herm_eigvec_batch_kernel<<<nb, EV_THREADS, smem, st>>>(M, ld, d_nred, e0, Q, max_iter, tol,
+                                                              d_w, V, d_status, d_iters);
+        SB_LAUNCH_CHECK();
+        SB_CUDA(cudaMemsetAsync(acc, 0, bins * nb * sizeof(float2), st));
+        SB_CUDA(cudaMemsetAsync(cnt, 0, bins * nb * sizeof(int), st));
+        SB_CUDA(cudaMemsetAsync(part, 0, (size_t)CHISQ_SLOTS * nb * sizeof(double), st));
+        rev_scatter_rank1_kernel<<<dim3(sb_, nb), 256, 0, st>>>(rg, d_th_red, g.n, d_etas, e0, d_nred,
+                                                               d_status, d_w, V, ld, acc, cnt);
+        SB_LAUNCH_CHECK();
+        rev_finalise_batch_kernel<<<dim3(fb, nb), 256, 0, st>>>(rg, acc, cnt);
+        SB_LAUNCH_CHECK();
+        if (pow2) {
+            // rows of every curvature in one launch, then the kept columns per curvature
+            BatchShiftedRowLoad lr{acc, n0, n1};
+            PlainRowStore<float2> rs{B1, n1};
+            SB_ROW_DISPATCH(n1, rc = (launch_row_c2c<float, N1, N2, +1>(lr, rs, (long)nb * n0, st)));
+            if (rc) return rc;
+            for (int e = 0; e < nb; ++e) {
+                StrideALoad<float2> la{B1 + bins * e, n1, R2};
+                ResidualStore cs{R1, scale,
+                                 ResidualSink{dspec, mask, nf, nt, part + (size_t)CHISQ_SLOTS * e}};
+                rc = cols_generic<float, +1>(la, B2, n1, n0, nt, cs, st);
+                if (rc) return rc;
+            }
+        } else {
+            for (int e = 0; e < nb; ++e) {
+                rc = ifft2_any_residual(acc + bins * e, n0, n1,
+                                        ResidualSink{dspec, mask, nf, nt,
+                                                     part + (size_t)CHISQ_SLOTS * e}, st);
+                if (rc) return rc;
+            }
+        }
+        chisq_finish_kernel<<<(nb + 127) / 128, 128, 0, st>>>(part, e0, nb, d_status, d_ssq);
+        SB_LAUNCH_CHECK();
+    }
+    return SB_OK;
 }
 
 // --------------------------------------------------------------------------

@@ -746,6 +746,17 @@ __global__ void thth_map_kernel(ThthGeom g, double eta, int hermitian,
 // --------------------------------------------------------------------------
 // host drivers
 // --------------------------------------------------------------------------
+// per-launch budget of the curvature-batched work buffers: 3 GiB, or SB_SWEEP_SLAB_MB
+// (tests use it to force batching)
+unsigned long long sweep_slab_bytes() {
+    unsigned long long slab = 3ull << 30;
+    if (const char* ev = getenv("SB_SWEEP_SLAB_MB")) {
+        const long mb = atol(ev);
+        if (mb > 0) slab = (unsigned long long)mb << 20;
+    }
+    return slab;
+}
+
 static bool lower_check_needed(const ThthGeom& g, const double* th_host) {
     // worst case fd argument over all (i, j): min(th) - max(th)
     double tmin = th_host[0], tmax = th_host[0];
@@ -755,6 +766,38 @@ static bool lower_check_needed(const ThthGeom& g, const double* th_host) {
     }
     double worst = floor(((tmin - tmax) - g.fd0 + g.half_dfd) / g.dfd) - 2.0;
     return !(worst >= -(double)g.nfd);
+}
+
+// crop masks (d_idx [neta][ld], d_nred) and the IndexError status bit of every eta;
+// d_status is cleared first
+int thth_prep(const ThthGeom& g, const double* th_host, const double* d_etas, int neta, int ld,
+              int* d_idx, int* d_nred, int* d_status, cudaStream_t st) {
+    SB_CUDA(cudaMemsetAsync(d_status, 0, neta * sizeof(int), st));
+    prof_begin(PROF_THTH_PREP, st);
+    thth_prep_kernel<<<neta, 32, 0, st>>>(g, d_etas, neta, ld, d_idx, d_nred);
+    prof_end(PROF_THTH_PREP, st);
+    SB_LAUNCH_CHECK();
+    if (lower_check_needed(g, th_host)) {
+        dim3 grid(64, neta);
+        thth_indexerr_kernel<<<grid, 256, 0, st>>>(g, d_etas, d_status);
+        SB_LAUNCH_CHECK();
+    }
+    return SB_OK;
+}
+
+// fp32 strict upper triangles [nb][ld][ld] of etas e0 .. e0 + nb - 1 (no fp16 copy)
+int thth_build_f32(const ThthGeom& g, const double* d_etas, int e0, int nb, int ld,
+                   const int* d_idx, const int* d_nred, float2* d_M, cudaStream_t st) {
+    const int T = ld / 32;
+    dim3 grid((nb + SB_BUILD_EB - 1) / SB_BUILD_EB, T * (T + 1) / 2), block(32, 32 / 4);
+    if ((unsigned long long)g.ntau * (unsigned long long)g.cs_pitch < (1ull << 32))
+        thth_build_kernel<0, 4, unsigned><<<grid, block, 0, st>>>(g, d_etas, e0, nb, ld, d_idx,
+                                                                  d_nred, d_M, nullptr, nullptr, 0.f);
+    else
+        thth_build_kernel<0, 4, size_t><<<grid, block, 0, st>>>(g, d_etas, e0, nb, ld, d_idx,
+                                                                d_nred, d_M, nullptr, nullptr, 0.f);
+    SB_LAUNCH_CHECK();
+    return SB_OK;
 }
 
 int eta_sweep(const ThthGeom& g, const double* th_host, const double* d_etas,
@@ -769,25 +812,11 @@ int eta_sweep(const ThthGeom& g, const double* th_host, const double* d_etas,
     }
     int* d_idx = (int*)workspace(1, (size_t)neta * ld * sizeof(int));
     if (!d_idx) return SB_ERR_NOMEM;
-    SB_CUDA(cudaMemsetAsync(d_status, 0, neta * sizeof(int), st));
-    prof_begin(PROF_THTH_PREP, st);
-    thth_prep_kernel<<<neta, 32, 0, st>>>(g, d_etas, neta, ld, d_idx, d_nred);
-    prof_end(PROF_THTH_PREP, st);
-    SB_LAUNCH_CHECK();
-    if (lower_check_needed(g, th_host)) {
-        dim3 grid(64, neta);
-        thth_indexerr_kernel<<<grid, 256, 0, st>>>(g, d_etas, d_status);
-        SB_LAUNCH_CHECK();
-    }
+    int rc = thth_prep(g, th_host, d_etas, neta, ld, d_idx, d_nred, d_status, st);
+    if (rc) return rc;
     // batch so that the matrix slab stays <= ~3 GiB
     const size_t per = (size_t)ld * ld * sizeof(float2);
-    // SB_SWEEP_SLAB_MB overrides the slab budget (tests use it to force batching)
-    unsigned long long slab = 3ull << 30;
-    if (const char* ev = getenv("SB_SWEEP_SLAB_MB")) {
-        const long mb = atol(ev);
-        if (mb > 0) slab = (unsigned long long)mb << 20;
-    }
-    int batch = (int)(slab / per);
+    int batch = (int)(sweep_slab_bytes() / per);
     if (batch < 1) batch = 1;
     if (batch > neta) batch = neta;
     float2* d_M = (float2*)workspace(2, per * batch);

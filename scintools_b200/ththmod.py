@@ -8,6 +8,9 @@ Same function names, argument order and failure behaviour as the reference
   thth_redmap    ththmod.py:119-173   -> sb_thth_map + crop
   Eval_calc      ththmod.py:371-401   -> sb_eta_sweep (one eta)
   eta_sweep      the eta loop of single_search, ththmod.py:789-811 (batched)
+  chisq_calc     ththmod.py:330-368   -> sb_chisq_sweep (one eta)
+  chisq_sweep    the chisq_calc loop of THTHSample.ipynb's chi-square search
+                 (batched; host: per-curvature rev_map centres, / N)
   single_search  ththmod.py:715-895   -> sb_cs_f32 + sb_eta_sweep + host fit
   min_edges      ththmod.py:1671-1705 (host)
   chi_par        ththmod.py:38-53     (host)
@@ -791,6 +794,110 @@ def single_chunk_retrieval(params):
         print(e, flush=True)
         model_E = np.zeros(dspec2.shape, dtype=complex)
     return (model_E, idx_f, idx_t)
+
+
+def _rev_centres(th, tau, fd, etas):
+    """rev_map bin centres of modeler for every curvature: theta_centres of the
+    edges_red of thth_redmap (ththmod.py:153-170, :204-205), with the
+    reference's expressions.  Returns float64 [neta][len(th)] (row k holds the
+    cropped count of them) and, per curvature, the exception numpy raises on the
+    way (None if none).  Crops of fewer than 3 centres are left to the device,
+    which reports them as SB_ETA_TOO_SMALL."""
+    out = np.zeros((etas.shape[0], th.shape[0]))
+    errs = [None] * etas.shape[0]
+    for k, eta in enumerate(etas):
+        sel = ((th ** 2) * eta < np.abs(tau.max())) * (np.abs(th) < np.abs(fd.max()) / 2)
+        m = int(sel.sum())
+        if m < 3:
+            continue
+        try:
+            er = th[sel]
+            er = (er[:-1] + er[1:]) / 2
+            step = np.diff(er).mean()
+            edges_red = np.concatenate((np.array([er[0] - step]), er, np.array([er[-1] + step])))
+            out[k, :m] = theta_centres(edges_red)
+        except Exception as e:  # noqa: BLE001  (raised again by chisq_calc)
+            errs[k] = e
+    return out, errs
+
+
+def _chisq_run(dspec, CS, tau, fd, etas, edges, mask, tol, max_iter):
+    """sb_chisq_sweep: unnormalised sums, eigenvalues, status, sizes, iterations
+    and the host-side errors of _rev_centres."""
+    import torch
+    d = np.asarray(dspec)
+    if d.ndim != 2:
+        raise ValueError("dspec must be 2-D, got shape %r" % (d.shape,))
+    if mask is not None:
+        mask = np.asarray(mask, dtype=bool)
+        if mask.shape != d.shape:
+            # what numpy raises for (model - dspec)[mask] (ththmod.py:367)
+            raise IndexError("mask shape %r does not match dspec shape %r"
+                             % (mask.shape, d.shape))
+    cs = _as_device_cs(CS)
+    geom = _Geom(cs, tau, fd, edges, True)
+    tauv, fdv = U.value(tau, "us"), U.value(fd, "mHz")
+    ev = np.ascontiguousarray(np.atleast_1d(U.value(etas, "s3")), dtype=np.float64)
+    neta = ev.shape[0]
+    th_red, errs = _rev_centres(geom.th, tauv, fdv, ev)
+    d_etas, d_th = D.upload(ev), D.upload(th_red)
+    d_dspec = D.upload_f32(d)
+    d_mask = D.upload(np.ascontiguousarray(mask, dtype=np.uint8)) if mask is not None else None
+    ssq = D.empty((neta,), torch.float64)
+    w = D.empty((neta,), torch.float64)
+    aux = [D.empty((neta,), torch.int32) for _ in range(3)]
+    _lib.check(_lib.lib.sb_chisq_sweep(
+        geom.ref, d_etas.data_ptr(), neta, d_th.data_ptr(), float(tauv[1] - tauv[0]),
+        float(fdv[1] - fdv[0]), d_dspec.data_ptr(), d.shape[0], d.shape[1], D.ptr(d_mask),
+        float(tol), int(max_iter), ssq.data_ptr(), w.data_ptr(), aux[0].data_ptr(),
+        aux[1].data_ptr(), aux[2].data_ptr(), D.stream_ptr()))
+    info = dict(w=w.cpu().numpy(), status=aux[0].cpu().numpy(), nred=aux[1].cpu().numpy(),
+                iters=aux[2].cpu().numpy())
+    return ssq.cpu().numpy(), info, errs
+
+
+def chisq_sweep(dspec, CS, tau, fd, etas, edges, N, mask=None, return_info=False,
+                tol=0.0, max_iter=0):
+    """chisq_calc (ththmod.py:330-368) for every curvature in ``etas``: the loop
+    of the chi-square search in the reference's THTHSample notebook, batched on
+    the device (one launch sequence, one number per curvature back).
+
+    Returns float64 ``sum over mask of (model - dspec)**2 / N`` per curvature
+    (an array ``N`` broadcasts as in numpy: shape (len(etas),) + N.shape), NaN
+    where chisq_calc would raise.  ``return_info`` adds a dict with the top
+    eigenvalues ``w``, the SB_ETA_* ``status`` bits, the cropped sizes ``nred``
+    and the Lanczos ``iters``.  ``CS`` may be a numpy array or a DeviceCS."""
+    ssq, info, errs = _chisq_run(dspec, CS, tau, fd, etas, edges, mask, tol, max_iter)
+    ssq[(info["status"] & 8) != 0] = np.nan        # ArpackNoConvergence in the reference
+    ssq[[e is not None for e in errs]] = np.nan
+    Nv = np.asarray(N, dtype=np.float64)
+    chisq = ssq.reshape(ssq.shape + (1,) * Nv.ndim) / Nv
+    if return_info:
+        return chisq, info
+    return chisq
+
+
+def chisq_calc(dspec, CS, tau, fd, eta, edges, N, mask=None):
+    """Chi-square of the rank-1 theta-theta model of the dynamic spectrum
+    (ththmod.py:330-368): np.sum((model - dspec)[mask] ** 2) / N with model =
+    modeler(...)[3][:dspec.shape[0], :dspec.shape[1]].  ``mask`` defaults to
+    np.isfinite(dspec).  Raises where the reference raises."""
+    ssq, info, errs = _chisq_run(dspec, CS, tau, fd, np.array([float(U.value(eta, "s3"))]),
+                                 edges, mask, 0.0, 0)
+    st = int(info["status"][0])
+    if st & 1:
+        raise IndexError("theta-theta point maps outside the conjugate "
+                         "spectrum (fd_inv < -nfd)")
+    if st & 4:
+        raise TypeError("theta-theta matrix too small for eigsh (n < 3)")
+    if st & 2:
+        # ARPACK error -9 in the reference: every start vector is mapped to zero
+        raise RuntimeError("starting vector is zero: the theta-theta matrix is zero")
+    if st & 8:
+        raise np.linalg.LinAlgError("top eigenpair did not converge")
+    if errs[0] is not None:
+        raise errs[0]
+    return ssq[0] / np.asarray(N, dtype=np.float64)
 
 
 def mask_func(w):
