@@ -306,6 +306,48 @@ int sb_cs_f32(const float* dspec, int32_t nf, int32_t nt, int32_t npad,
 int sb_cs_bound_f32(const float* dspec, int32_t nf, int32_t nt, int32_t npad, float pad_value,
                     float* bound_out, void* stream);
 
+/* Conjugate spectrum of a COMPLEX chunk vis (float2 [nf][nt], e.g. a VLBI
+ * visibility, ththmod.py:1313-1325): pad to (npad+1) nf x (npad+1) nt with
+ * pad_re + i pad_im (pad_re NaN: the mean of vis, computed on the device),
+ * fft2, fftshift both axes, zero the rows where tau_rowmask (uint8 [ntau],
+ * fftshifted order, or NULL) is set.  cs: float2 [ntau][nfd], always the full
+ * plane.  Padded sizes that are powers of two in 8..65536 x 8..16384 take the
+ * radix path (a complex row is one transform of nfd points, so the column limit
+ * is half that of sb_cs_f32); any other size in 3..32768 x 3..8192 runs a
+ * chirp-z transform.  Other sizes: SB_ERR_UNSUPPORTED. */
+int sb_cs_c2c_f32(const void* vis, int32_t nf, int32_t nt, int32_t npad, float pad_re,
+                  float pad_im, const uint8_t* tau_rowmask, void* cs, void* stream);
+
+/* One chunk of ththmod.VLBI_chunk_retrieval (:1223-1387), steps after the
+ * conjugate spectra, with no host synchronisation.  cs_list_host: host array of
+ * n_dish (n_dish+1)/2 device pointers to full-plane float2 [ntau][nfd] spectra in
+ * the reference's order [I1, V12, .., V1N, I2, V23, .., IN]; geom supplies the
+ * axes and the theta grid (cs_half must be 0; cs, cs_pitch, cs_valid_cols,
+ * cs_bound and coherent are not read: every spectrum is dense and complex).
+ *   - every spectrum is cropped and gathered with thth_redmap's rules (autos
+ *     hermetian=True, visibilities hermetian=False) straight into the composite
+ *     [n_dish n][n_dish n] matrix, n = the cropped size: block (d1, d1+d2) =
+ *     conj(T).T, block (d1+d2, d1) = T (:1342-1362);
+ *   - top eigenpair (w, V) as sb_herm_eigvec, starting from the sum of row n//2
+ *     of every station's block row (one row alone would keep Lanczos inside one
+ *     station's block when the visibilities are zero), or from a fixed vector if
+ *     that sum is zero;
+ *   - per station d: rev_map(hermetian=False) of the n x n matrix whose row n//2
+ *     is conj(V[d n:(d+1) n]) sqrt(w), ifft2(ifftshift(.))[:nf, :nt] nf nt / 4.
+ * th_red: device float64 [n], the rev_map centres (theta_centres of edges_red);
+ * dtau_bin, dfd_bin: as sb_chisq_sweep.  tol / max_iter as sb_herm_eigvec.
+ * Outputs (device): model_e float2 [n_dish][nf][nt]; w float64 [1] (NaN for
+ * SB_ETA_INDEX_ERROR / SB_ETA_TOO_SMALL, 0 for an all-zero composite with
+ * SB_ETA_ZERO_START); v float2 [n_dish n]; info int32 [3] = {Lanczos steps,
+ * SB_ETA_* status, n}.  A failed eigenpair leaves model_e zero.
+ * Errors: SB_ERR_ARG for n_dish < 1, nf > ntau, nt > nfd or a null spectrum;
+ * SB_ERR_UNSUPPORTED for n_dish n > 8192 or CS sizes outside those of
+ * sb_ifft2_c2c_f32.  Sizes are checked before any workspace is allocated. */
+int sb_vlbi_retrieval(const sb_thth_geom* geom, const void* const* cs_list_host, int32_t n_dish,
+                      double eta, const double* th_red, double dtau_bin, double dfd_bin,
+                      int32_t nf, int32_t nt, double tol, int32_t max_iter, void* model_e,
+                      double* w, void* v, int32_t* info, void* stream);
+
 /* ---- scint_sim.Simulation ------------------------------------------------ */
 
 typedef struct sb_sim_params {

@@ -151,6 +151,12 @@ int chisq_sweep(const ThthGeom& g, const double* th_host, const double* d_etas, 
                 const unsigned char* mask, int nf, int nt, double tol, int max_iter,
                 double* d_ssq, double* d_w, int* d_status, int* d_nred, int* d_iters,
                 cudaStream_t st);
+int conj_spectrum_c2c(const float2* in, int nf, int nt, int npad, float pad_re, float pad_im,
+                      const unsigned char* rowmask, float2* CS, cudaStream_t st);
+int vlbi_retrieval(const ThthGeom& g, const double* th_host, const float2* const* cs_host,
+                   int n_dish, double eta, const double* d_th_red, double dtau_bin,
+                   double dfd_bin, int nf, int nt, double tol, int max_iter, float2* d_model,
+                   double* d_w, float2* d_v, int* d_info, cudaStream_t st);
 
 int gerchberg_saxton(float2* W, const float* amp, const unsigned char* rowmask, int n0, int n1,
                      int niter, cudaStream_t st);
@@ -199,7 +205,7 @@ static int to_geom(const sb_thth_geom* in, ThthGeom* g) {
 
 extern "C" {
 
-int sb_abi_version(void) { return 3; }
+int sb_abi_version(void) { return 4; }
 const char* sb_last_error(void) { return sb::last_error(); }
 
 int sb_init(int device) {
@@ -415,6 +421,26 @@ int sb_cs_bound_f32(const float* dspec, int32_t nf, int32_t nt, int32_t npad, fl
                     float* bound_out, void* stream) {
     SB_ARG(dspec && bound_out && nf >= 1 && nt >= 1 && npad >= 0);
     return sb::conj_spectrum_bound(dspec, nf, nt, npad, pad_value, bound_out, (cudaStream_t)stream);
+}
+
+int sb_cs_c2c_f32(const void* vis, int32_t nf, int32_t nt, int32_t npad, float pad_re,
+                  float pad_im, const uint8_t* tau_rowmask, void* cs, void* stream) {
+    SB_ARG(vis && cs && nf >= 1 && nt >= 1 && npad >= 0);
+    return sb::conj_spectrum_c2c((const float2*)vis, nf, nt, npad, pad_re, pad_im, tau_rowmask,
+                                 (float2*)cs, (cudaStream_t)stream);
+}
+
+int sb_vlbi_retrieval(const sb_thth_geom* geom, const void* const* cs_list_host, int32_t n_dish,
+                      double eta, const double* th_red, double dtau_bin, double dfd_bin,
+                      int32_t nf, int32_t nt, double tol, int32_t max_iter, void* model_e,
+                      double* w, void* v, int32_t* info, void* stream) {
+    sb::ThthGeom g;
+    int rc = sb::to_geom(geom, &g);
+    if (rc) return rc;
+    SB_ARG(cs_list_host && th_red && model_e && w && v && info);
+    return sb::vlbi_retrieval(g, geom->th_cents_host, (const float2* const*)cs_list_host, n_dish,
+                              eta, th_red, dtau_bin, dfd_bin, nf, nt, tol, max_iter,
+                              (float2*)model_e, w, (float2*)v, info, (cudaStream_t)stream);
 }
 
 int sb_sim_weights(const sb_sim_params* p, double* w, void* stream) {

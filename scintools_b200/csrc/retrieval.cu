@@ -4,17 +4,21 @@
 //                                     matrix (eigsh(.., 1, which='LA') in modeler)
 //   ifft2        ththmod.py:321, 1462 ifft2(ifftshift(recov)), cropped
 //   chisq_sweep  ththmod.py:330-368   chisq_calc over a batch of curvatures
-// used by the Python mirrors of modeler / single_chunk_retrieval / chisq_calc.
+//   vlbi_retrieval ththmod.py:1223-1387 VLBI_chunk_retrieval after the spectra, and
+//                conj_spectrum_c2c    the conjugate spectrum of its complex visibilities
+// used by the Python mirrors of modeler / single_chunk_retrieval / chisq_calc /
+// VLBI_chunk_retrieval.
 #include <float.h>
+#include <limits.h>
 #include <math.h>
 #include <stdlib.h>
 
 #ifndef SB_HOST_EMU            // tests/host_emu runs the scatter / eigenpair kernels on the CPU
 #include "chisq.cuh"
 #include "fft_generic.cuh"
-#include "thth.cuh"
 #endif
 #include "lanczos.cuh"
+#include "thth.cuh"
 
 namespace sb {
 
@@ -47,28 +51,36 @@ struct RevGeom {
     int ntau, nfd;
 };
 
+// fd, tau and Jacobian of point (i, j) of the theta-theta matrix:
+// fd_map[i][j] = th[j] - th[i];  tau_map = eta * (th[j]^2 - th[i]^2)
+struct RevPoint { double x, y, jac; };
+__device__ __forceinline__ RevPoint rev_point(const RevGeom& g, int i, int j) {
+    const double ti = g.th[i], tj = g.th[j];
+    return {__dsub_rn(tj, ti),
+            __dmul_rn(g.eta, __dsub_rn(__dmul_rn(tj, tj), __dmul_rn(ti, ti))),
+            sqrt(fabs(__dmul_rn(__dmul_rn(2.0, g.eta), __dsub_rn(ti, tj))))};
+}
+// histogram bin of (fd, tau) = (x, y), or -1 outside
+__device__ __forceinline__ long rev_bin(const RevGeom& g, double x, double y) {
+    const int bx = hist_bin(x, g.fd0, g.dfd, g.nfd), by = hist_bin(y, g.tau0, g.dtau, g.ntau);
+    return (bx >= 0 && by >= 0) ? (long)by * g.nfd + bx : -1;
+}
+
 // point (i, j), i != j, of the theta-theta matrix with value v into the histograms
 __device__ __forceinline__ void rev_scatter_point(const RevGeom& g, int i, int j, float2 v,
                                                   int hermitian, float2* __restrict__ acc,
                                                   int* __restrict__ cnt) {
-    const double ti = g.th[i], tj = g.th[j];
-    // fd_map[i][j] = th[j] - th[i];  tau_map = eta * (th[j]^2 - th[i]^2)
-    const double x = __dsub_rn(tj, ti);
-    const double y = __dmul_rn(g.eta, __dsub_rn(__dmul_rn(tj, tj), __dmul_rn(ti, ti)));
-    const double jac = sqrt(fabs(__dmul_rn(__dmul_rn(2.0, g.eta), __dsub_rn(ti, tj))));
-    const float wre = (float)((double)v.x / jac), wim = (float)((double)v.y / jac);
-    int bx = hist_bin(x, g.fd0, g.dfd, g.nfd), by = hist_bin(y, g.tau0, g.dtau, g.ntau);
-    if (bx >= 0 && by >= 0) {
-        const size_t o = (size_t)by * g.nfd + bx;
+    const RevPoint p = rev_point(g, i, j);
+    const float wre = (float)((double)v.x / p.jac), wim = (float)((double)v.y / p.jac);
+    long o = rev_bin(g, p.x, p.y);
+    if (o >= 0) {
         atomicAdd(&acc[o].x, wre);
         atomicAdd(&acc[o].y, wim);
         atomicAdd(&cnt[o], 1);
     }
     if (hermitian) {
-        bx = hist_bin(-x, g.fd0, g.dfd, g.nfd);
-        by = hist_bin(-y, g.tau0, g.dtau, g.ntau);
-        if (bx >= 0 && by >= 0) {
-            const size_t o = (size_t)by * g.nfd + bx;
+        o = rev_bin(g, -p.x, -p.y);
+        if (o >= 0) {
             atomicAdd(&acc[o].x, wre);
             atomicAdd(&acc[o].y, -wim);
             atomicAdd(&cnt[o], 1);
@@ -232,7 +244,29 @@ struct UpperHermitian {
     }
 };
 
-// Shared body.  Start vector: row n//2.  If that row is zero, zero_start_fallback == 0
+// The composite of VLBI_chunk_retrieval: n_dish x n_dish blocks of n x n, full row-major
+struct CompositeMatrix {
+    const float2* A;
+    int ld, n_dish, n;
+    __device__ __forceinline__ float2 operator()(int a, int c) const { return A[(size_t)a * ld + c]; }
+};
+// Lanczos start vector, element c: row h of the matrix ...
+template <class Mat>
+__device__ __forceinline__ float2 start_row(const Mat& A, int h, int c) { return A(h, c); }
+// ... except for the composite: the sum of row n//2 of every station's block row.  A
+// single row lies in one block row; when the stations do not couple (zero visibilities)
+// the composite is block diagonal and Lanczos would never leave that station's block.
+__device__ __forceinline__ float2 start_row(const CompositeMatrix& A, int, int c) {
+    float2 s = make_float2(0.f, 0.f);
+    for (int d = 0; d < A.n_dish; ++d) {
+        const float2 x = A(d * A.n + A.n / 2, c);
+        s.x += x.x;
+        s.y += x.y;
+    }
+    return s;
+}
+
+// Shared body.  Start vector: row n//2 (start_row).  If it is zero, zero_start_fallback == 0
 // reports it (w = NaN, info[1] = 2); otherwise Lanczos starts from a fixed non-zero
 // vector instead, and a start vector that A maps to zero (for a zero-diagonal Hermitian
 // matrix: A == 0) gives w = 0 with that vector as V and info[1] = 2.
@@ -254,7 +288,7 @@ __device__ void herm_eigvec_body(Mat A, int n, float2* __restrict__ Q, int max_i
     const int h = n / 2;
     double p0 = 0.0;
     for (int c = tid; c < n; c += EV_THREADS) {
-        const float2 x = A(h, c);
+        const float2 x = start_row(A, h, c);
         v[c] = x;
         p0 += (double)x.x * x.x + (double)x.y * x.y;
     }
@@ -442,6 +476,133 @@ herm_eigvec_batch_kernel(const float2* __restrict__ M, int ld, const int* __rest
         iters[ge] = info[0];
         status[ge] |= info[1];
     }
+}
+
+// --------------------------------------------------------------------------
+// VLBI_chunk_retrieval (ththmod.py:1223-1387): the composite theta-theta matrix of
+// n_dish stations, its top eigenpair and one wavefield per station.
+// Spectra are in reference order [I1, V12, .., V1N, I2, V23, .., IN]; pair (d1, d1 + d2)
+// sits at index N(N+1)/2 - (N-d1)(N-d1+1)/2 + d2, autos at d2 = 0.
+// --------------------------------------------------------------------------
+__host__ __device__ __forceinline__ int vlbi_pair_index(int n_dish, int d1, int d2) {
+    return n_dish * (n_dish + 1) / 2 - (n_dish - d1) * (n_dish - d1 + 1) / 2 + d2;
+}
+
+// Composite [n_dish n][n_dish n], row-major, written whole: block (b, b + d2) is
+// conj(T_k).T and block (b + d2, b) is T_k, k = pair (b, d2); the diagonal blocks are
+// the autos' T.  T_k is thth_redmap of spectrum k on the crop idx[0..n): autos with the
+// Hermitian fill of thth_map (upper triangle mirrored, diagonal and anti-diagonal of the
+// full grid zeroed, nan_to_num), visibilities the raw Jacobian-weighted gather.
+// cs: [n_dish (n_dish + 1) / 2] full-plane spectra of the geometry g.
+__global__ void vlbi_composite_kernel(ThthGeom g, const double* __restrict__ eta_p,
+                                      const float2* const* __restrict__ cs, int n_dish,
+                                      const int* __restrict__ idx, int n,
+                                      float2* __restrict__ A) {
+    const double eta = *eta_p;
+    const long N = (long)n_dish * n;
+    for (long p = blockIdx.x * (long)blockDim.x + threadIdx.x; p < N * N;
+         p += (long)gridDim.x * blockDim.x) {
+        const int R = (int)(p / N), C = (int)(p - (long)R * N);
+        const int bi = R / n, a = R - bi * n, bj = C / n, c = C - bj * n;
+        // element (r, s) of T_k; the upper blocks read it transposed and conjugate it
+        const bool upper = bi < bj;
+        const int d1 = upper ? bi : bj, d2 = upper ? bj - bi : bi - bj;
+        const int r = upper ? c : a, s = upper ? a : c;
+        ThthGeom gk = g;
+        gk.cs = cs[vlbi_pair_index(n_dish, d1, d2)];
+        const int i = idx[r], j = idx[s];            // rows / columns of the full grid
+        const double thi = g.th[i], thj = g.th[j];
+        float2 v;
+        if (d2 != 0) {
+            v = thth_value(gk, eta, thj, thi, thth_point(gk, eta, thj, thi));
+        } else if (i == j || i + j == g.n - 1) {
+            v = make_float2(0.f, 0.f);
+        } else if (j > i) {
+            v = thth_value(gk, eta, thj, thi, thth_point(gk, eta, thj, thi));
+            v.x = nan_to_num(v.x);
+            v.y = nan_to_num(v.y);
+        } else {                                     // conj of the upper element (j, i)
+            v = thth_value(gk, eta, thi, thj, thth_point(gk, eta, thi, thj));
+            v.x = nan_to_num(v.x);
+            v.y = -nan_to_num(v.y);
+        }
+        if (upper) v.y = -v.y;
+        A[p] = v;
+    }
+}
+
+// Top eigenpair of the composite (N = n_dish n), started from the sum of the stations'
+// rows n//2 or, if that is zero, from the fixed start vector.  info = {Lanczos steps,
+// SB_ETA_* status, nred}; status bit 1 comes from thth_prep.  A matrix smaller than
+// 3 x 3 is reported as bit 4 (eigsh raises).
+__global__ void __launch_bounds__(EV_THREADS)
+vlbi_eigvec_kernel(const float2* __restrict__ A, int n_dish, int n, float2* __restrict__ Q,
+                   int max_iter, double tol, double* __restrict__ w, float2* __restrict__ V,
+                   int* __restrict__ info) {
+    const int N = n_dish * n;
+    if ((info[1] & 1) || N < 3) {
+        for (int c = threadIdx.x; c < N; c += EV_THREADS) V[c] = make_float2(0.f, 0.f);
+        if (threadIdx.x == 0) {
+            *w = __longlong_as_double(0x7ff8000000000000LL);
+            info[0] = 0;
+            if (N < 3) info[1] |= 4;
+        }
+        return;
+    }
+    __shared__ int sh_info[2];
+    herm_eigvec_body(CompositeMatrix{A, N, n_dish, n}, N, Q, max_iter < N ? max_iter : N, tol, 1,
+                     w, V, sh_info);
+    if (threadIdx.x == 0) {        // sh_info was written by thread 0 of the body
+        info[0] = sh_info[0];
+        info[1] |= sh_info[1];
+    }
+}
+
+// rev_map(hermetian=False) of every station's model, whose only non-zero row is row n//2,
+// conj(V[d n : (d + 1) n]) sqrt(w) (the zero rows still count in the bin means).
+// blockIdx.y < n_dish: station blockIdx.y adds the values of row n//2 to acc[d];
+// blockIdx.y == n_dish: the counts of all n^2 - n off-diagonal points, shared by every
+// station.  A failed eigenpair (status bits 1, 2, 4) scatters nothing.
+__global__ void vlbi_scatter_kernel(RevGeom g, int n_dish, const int* __restrict__ info,
+                                    const double* __restrict__ w,
+                                    const float2* __restrict__ V, float2* __restrict__ acc,
+                                    int* __restrict__ cnt) {
+    if (info[1] & 7) return;
+    const int n = g.n, h = n / 2, d = blockIdx.y;
+    if (d == n_dish) {
+        for (long p = blockIdx.x * (long)blockDim.x + threadIdx.x; p < (long)n * n;
+             p += (long)gridDim.x * blockDim.x) {
+            const int i = (int)(p / n), j = (int)(p - (long)i * n);
+            if (i == j) continue;
+            const RevPoint q = rev_point(g, i, j);
+            const long o = rev_bin(g, q.x, q.y);
+            if (o >= 0) atomicAdd(&cnt[o], 1);
+        }
+        return;
+    }
+    const double sw = sqrt(*w);
+    float2* out = acc + (size_t)d * g.ntau * g.nfd;
+    for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) {
+        if (j == h) continue;          // zero Jacobian: the DC bin, zeroed by the finalise step
+        const RevPoint pt = rev_point(g, h, j);
+        const long o = rev_bin(g, pt.x, pt.y);
+        if (o < 0) continue;
+        const float2 q = V[(size_t)d * n + j];
+        // the model element, rounded to fp32 as an uploaded complex128 matrix would be
+        const float tre = (float)((double)q.x * sw), tim = (float)(-(double)q.y * sw);
+        atomicAdd(&out[o].x, (float)((double)tre / pt.jac));
+        atomicAdd(&out[o].y, (float)((double)tim / pt.jac));
+    }
+}
+
+__global__ void vlbi_finalise_kernel(RevGeom g, float2* __restrict__ acc,
+                                     const int* __restrict__ cnt) {
+    const long total = (long)g.ntau * g.nfd;
+    const long dc = rev_dc_bin(g);
+    acc += blockIdx.y * (size_t)total;
+    for (long o = blockIdx.x * (long)blockDim.x + threadIdx.x; o < total;
+         o += (long)gridDim.x * blockDim.x)
+        acc[o] = rev_bin_value(acc[o], cnt[o], o == dc);
 }
 
 #ifndef SB_HOST_EMU
@@ -838,6 +999,276 @@ int gerchberg_saxton(float2* W, const float* amp, const unsigned char* rowmask, 
     if (rc) return rc;
     gs_convert_kernel<<<blocks, 256, 0, st>>>((const double*)B[3], (float*)W, count);
     SB_LAUNCH_CHECK();
+    return SB_OK;
+}
+
+// --------------------------------------------------------------------------
+// Conjugate spectrum of a complex chunk (the visibilities of VLBI_chunk_retrieval,
+// ththmod.py:1313-1325): pad to NF x NT, fft2, fftshift, zero the masked tau rows.
+// The padded chunk is materialised; power-of-two sizes run the radix rows and columns
+// forwards, other sizes the chirp-z inverse on the conjugate (fft2(x) = conj(N ifft2(conj x))).
+// --------------------------------------------------------------------------
+__global__ void c2c_sum_kernel(const float2* __restrict__ in, long count, double* __restrict__ sum) {
+    double sx = 0.0, sy = 0.0;
+    for (long o = blockIdx.x * (long)blockDim.x + threadIdx.x; o < count;
+         o += (long)gridDim.x * blockDim.x) {
+        sx += in[o].x;
+        sy += in[o].y;
+    }
+    sx = warp_sum(sx);
+    sy = warp_sum(sy);
+    if ((threadIdx.x & 31) == 0) {
+        atomicAdd(sum, sx);
+        atomicAdd(sum + 1, sy);
+    }
+}
+// P [NF][NT]: the chunk in the first nf x nt corner, pad elsewhere (sum != null: the mean)
+__global__ void c2c_pad_kernel(const float2* __restrict__ in, int nf, int nt, int NF, int NT,
+                               float2 pad, const double* __restrict__ sum, float2* __restrict__ P) {
+    if (sum) {
+        const double cnt = (double)nf * (double)nt;
+        pad = make_float2((float)(sum[0] / cnt), (float)(sum[1] / cnt));
+    }
+    const long total = (long)NF * NT;
+    for (long o = blockIdx.x * (long)blockDim.x + threadIdx.x; o < total;
+         o += (long)gridDim.x * blockDim.x) {
+        const int r = (int)(o / NT), c = (int)(o - (long)r * NT);
+        P[o] = (r < nf && c < nt) ? in[(size_t)r * nt + c] : pad;
+    }
+}
+struct CsShiftStore {     // CS[fftshift(k)][fftshift(c)] = v, masked rows zero (powers of two)
+    float2* CS;
+    int NF, NT, R1;
+    const unsigned char* rowmask;
+    __device__ __forceinline__ void operator()(int y, int k, int c, float2 v) const {
+        const int rs = (y + R1 * k + NF / 2) & (NF - 1), cs = (c + NT / 2) & (NT - 1);
+        CS[(size_t)rs * NT + cs] = (rowmask && rowmask[rs]) ? make_float2(0.f, 0.f) : v;
+    }
+};
+// CS = fftshift(conj(T)), masked rows zero (any size)
+__global__ void c2c_shift_conj_kernel(const float2* __restrict__ T, int NF, int NT,
+                                      const unsigned char* __restrict__ rowmask,
+                                      float2* __restrict__ CS) {
+    const long total = (long)NF * NT;
+    for (long o = blockIdx.x * (long)blockDim.x + threadIdx.x; o < total;
+         o += (long)gridDim.x * blockDim.x) {
+        const int r = (int)(o / NT), c = (int)(o - (long)r * NT);
+        const int rs = (r + NF / 2) % NF, cs = (c + NT / 2) % NT;
+        const float2 t = T[o];
+        CS[(size_t)rs * NT + cs] =
+            (rowmask && rowmask[rs]) ? make_float2(0.f, 0.f) : make_float2(t.x, -t.y);
+    }
+}
+
+int conj_spectrum_c2c(const float2* in, int nf, int nt, int npad, float pad_re, float pad_im,
+                      const unsigned char* rowmask, float2* CS, cudaStream_t st) {
+    const long NFl = (long)(npad + 1) * nf, NTl = (long)(npad + 1) * nt;
+    // a complex row is one row transform of NT points (8..16384), unlike the real input's
+    // half-length rows; the chirp-z path has the limits of ifft2_c2c_any
+    const bool radix = is_pow2(NFl) && is_pow2(NTl) && NFl >= 8 && NTl >= 8 && NFl <= 65536 &&
+                       NTl <= 16384;
+    if (!radix && (NFl < 3 || NTl < 3 || NFl > 32768 || NTl > 8192)) {
+        set_error("conjugate spectrum (complex input): padded size %ldx%ld outside 8..65536 x "
+                  "8..16384 (powers of two) / 3..32768 x 3..8192 (other sizes)", NFl, NTl);
+        return SB_ERR_UNSUPPORTED;
+    }
+    const int NF = (int)NFl, NT = (int)NTl;
+    const size_t count = (size_t)NF * NT;
+    double* sum = (double*)workspace(0, 64 * sizeof(double));
+    float2* P = (float2*)workspace(2, count * sizeof(float2));
+    if (!sum || !P) return SB_ERR_NOMEM;
+    int blocks = (int)((count + 255) / 256);
+    if (blocks > num_sms() * 16) blocks = num_sms() * 16;
+    const bool dev_mean = pad_re != pad_re;
+    if (dev_mean) {
+        SB_CUDA(cudaMemsetAsync(sum, 0, 2 * sizeof(double), st));
+        c2c_sum_kernel<<<num_sms() * 4, 256, 0, st>>>(in, (long)nf * nt, sum);
+        SB_LAUNCH_CHECK();
+    }
+    c2c_pad_kernel<<<blocks, 256, 0, st>>>(in, nf, nt, NF, NT, make_float2(pad_re, pad_im),
+                                           dev_mean ? sum : nullptr, P);
+    SB_LAUNCH_CHECK();
+    if (radix) {
+        float2* B1 = (float2*)workspace(3, count * sizeof(float2));
+        float2* B2 = (float2*)workspace(4, count * sizeof(float2));
+        if (!B1 || !B2) return SB_ERR_NOMEM;
+        int rc = SB_OK;
+        PitchRowLoadC<float2> lr{P, NT};
+        PlainRowStore<float2> rs{B1, NT};
+        SB_ROW_DISPATCH(NT, rc = (launch_row_c2c<float, N1, N2, -1>(lr, rs, NF, st)));
+        if (rc) return rc;
+        int R1, R2;
+        split_len(NF, &R1, &R2);
+        StrideALoad<float2> la{B1, NT, R2};
+        return cols_generic<float, -1>(la, B2, NT, NF, NT, CsShiftStore{CS, NF, NT, R1, rowmask},
+                                       st);
+    }
+    float2* T = (float2*)workspace(1, count * sizeof(float2));
+    if (!T) return SB_ERR_NOMEM;
+    const int rc = ifft2_c2c_any(P, NF, NT, 0, 0, 0, (double)count, 0, T, st, 1);
+    if (rc) return rc;
+    c2c_shift_conj_kernel<<<blocks, 256, 0, st>>>(T, NF, NT, rowmask, CS);
+    SB_LAUNCH_CHECK();
+    return SB_OK;
+}
+
+// --------------------------------------------------------------------------
+// VLBI_chunk_retrieval for one chunk, steps 3-6 (ththmod.py:1310-1383): crop, composite
+// gather, eigenpair, per-station rev_map of row n//2, ifft2(ifftshift(.)) cropped to
+// nf x nt and scaled by nf nt / 4.  No host synchronisation.
+// --------------------------------------------------------------------------
+constexpr int VLBI_PTRS = 64;
+struct VlbiArgs {          // device copies of eta and of a run of spectrum pointers
+    const float2* cs[VLBI_PTRS];
+    int base, count;
+    double eta;
+};
+__global__ void vlbi_args_kernel(VlbiArgs a, const float2** cs, double* eta) {
+    if ((int)threadIdx.x < a.count) cs[a.base + threadIdx.x] = a.cs[threadIdx.x];
+    if (threadIdx.x == 0 && a.base == 0) *eta = a.eta;
+}
+
+int vlbi_retrieval(const ThthGeom& geom, const double* th_host, const float2* const* cs_host,
+                   int n_dish, double eta, const double* d_th_red, double dtau_bin,
+                   double dfd_bin, int nf, int nt, double tol, int max_iter, float2* d_model,
+                   double* d_w, float2* d_v, int* d_info, cudaStream_t st) {
+    // every spectrum is a dense, complex, full-plane [ntau][nfd] array: the layout and
+    // mode fields of the caller's geometry do not apply
+    ThthGeom g = geom;
+    g.cs = nullptr;
+    g.cs_pitch = g.nfd;
+    g.cs_valid_cols = 0;
+    g.cs_bound = nullptr;
+    g.coherent = 1;
+    const int n0 = (int)g.ntau, n1 = (int)g.nfd;
+    if (n_dish < 1) {
+        set_error("vlbi_retrieval: n_dish = %d, needs at least one station", n_dish);
+        return SB_ERR_ARG;
+    }
+    if (nf < 1 || nt < 1 || nf > n0 || nt > n1) {
+        set_error("vlbi_retrieval: chunk %d x %d is empty or larger than the conjugate "
+                  "spectrum %d x %d", nf, nt, n0, n1);
+        return SB_ERR_ARG;
+    }
+    if (!(dtau_bin > 0.0) || !(dfd_bin > 0.0)) {
+        set_error("vlbi_retrieval needs ascending tau / fd axes (bins must increase monotonically)");
+        return SB_ERR_ARG;
+    }
+    if (g.cs_half) {
+        set_error("vlbi_retrieval needs full-plane conjugate spectra");
+        return SB_ERR_ARG;
+    }
+    const int npairs = n_dish * (n_dish + 1) / 2;
+    for (int k = 0; k < npairs; ++k)
+        if (!cs_host[k]) {
+            set_error("vlbi_retrieval: conjugate spectrum %d is null", k);
+            return SB_ERR_ARG;
+        }
+    // cropped size: the mask of thth_prep_kernel with the same (exactly rounded) expressions
+    int n = 0;
+    for (int k = 0; k < g.n; ++k) {
+        const double t = th_host[k];
+        if ((t * t) * eta < g.tau_absmax && fabs(t) < g.fd_half) ++n;
+    }
+    const long N = (long)n_dish * n;
+    if (N > 8192) {
+        set_error("vlbi_retrieval: composite theta-theta matrix of %d stations x %d centres = %ld "
+                  "exceeds the eigen solver's limit of 8192", n_dish, n, N);
+        return SB_ERR_UNSUPPORTED;
+    }
+    const bool pow2 = !(n0 & (n0 - 1)) && !(n1 & (n1 - 1));
+    if (pow2 ? (n0 < 8 || n1 < 8 || n0 > 65536 || n1 > 16384)
+             : (n0 < 3 || n1 < 3 || n0 > 32768 || n1 > 8192)) {
+        set_error("vlbi_retrieval: conjugate spectrum %d x %d outside 8..65536 x 8..16384 (powers "
+                  "of two) / 3..32768 x 3..8192 (other sizes)", n0, n1);
+        return SB_ERR_UNSUPPORTED;
+    }
+    if (!(tol > 0.0)) tol = 1e-7;
+    if (max_iter <= 0 || max_iter > SB_LANCZOS_MAXIT) max_iter = 96;
+    const size_t bins = (size_t)n0 * n1;
+    const size_t qn = (size_t)(max_iter + 1) * (N > 0 ? N : 1);
+    // slot 1: eta, spectrum pointers, crop indices; slot 2: composite, Lanczos basis,
+    // per-station bin sums, shared bin counts
+    unsigned char* s1 = (unsigned char*)workspace(
+        1, sizeof(double) + (size_t)npairs * sizeof(float2*) + (size_t)g.n * sizeof(int));
+    unsigned char* s2 = (unsigned char*)workspace(
+        2, ((size_t)N * N + qn + (size_t)n_dish * bins) * sizeof(float2) + bins * sizeof(int));
+    if (!s1 || !s2) return SB_ERR_NOMEM;
+    double* d_eta = (double*)s1;
+    const float2** d_cs = (const float2**)(d_eta + 1);
+    int* d_idx = (int*)(d_cs + npairs);
+    float2* A = (float2*)s2;
+    float2* Q = A + (size_t)N * N;
+    float2* acc = Q + qn;
+    int* cnt = (int*)(acc + (size_t)n_dish * bins);
+    float2 *B1 = nullptr, *B2 = nullptr;
+    if (pow2) {
+        B1 = (float2*)workspace(3, (size_t)n_dish * bins * sizeof(float2));
+        B2 = (float2*)workspace(4, bins * sizeof(float2));
+        if (!B1 || !B2) return SB_ERR_NOMEM;
+    }
+    for (int b = 0; b < npairs; b += VLBI_PTRS) {
+        VlbiArgs a;
+        a.base = b;
+        a.count = npairs - b < VLBI_PTRS ? npairs - b : VLBI_PTRS;
+        a.eta = eta;
+        for (int k = 0; k < a.count; ++k) a.cs[k] = cs_host[b + k];
+        vlbi_args_kernel<<<1, VLBI_PTRS, 0, st>>>(a, d_cs, d_eta);
+        SB_LAUNCH_CHECK();
+    }
+    int rc = thth_prep(g, th_host, d_eta, 1, g.n, d_idx, d_info + 2, d_info + 1, st);
+    if (rc) return rc;
+    if (N > 0) {
+        int blocks = (int)((N * N + 255) / 256);
+        if (blocks > num_sms() * 16) blocks = num_sms() * 16;
+        vlbi_composite_kernel<<<blocks, 256, 0, st>>>(g, d_eta, d_cs, n_dish, d_idx, n, A);
+        SB_LAUNCH_CHECK();
+    }
+    const size_t smem = sizeof(LanczosShared) + 32 * sizeof(double) +
+                        (SB_LANCZOS_MAXIT + 1) * sizeof(double2) + 2 * (size_t)N * sizeof(float2);
+    SB_CUDA(cudaFuncSetAttribute(vlbi_eigvec_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)smem));
+    vlbi_eigvec_kernel<<<1, EV_THREADS, smem, st>>>(A, n_dish, n, Q, max_iter, tol, d_w, d_v,
+                                                    d_info);
+    SB_LAUNCH_CHECK();
+    SB_CUDA(cudaMemsetAsync(acc, 0, (size_t)n_dish * bins * sizeof(float2), st));
+    SB_CUDA(cudaMemsetAsync(cnt, 0, bins * sizeof(int), st));
+    // rev_map bins: tau[0], tau[1] - tau[0], fd[0], fd[1] - fd[0] (ththmod.py:210-215)
+    const RevGeom rg{d_th_red, n, eta, g.tau0, dtau_bin, g.fd0, dfd_bin, n0, n1};
+    if (n > 0) {
+        int sb_ = (int)(((size_t)n * n + 255) / 256);
+        sb_ = sb_ > 256 ? 256 : sb_;
+        vlbi_scatter_kernel<<<dim3(sb_, n_dish + 1), 256, 0, st>>>(rg, n_dish, d_info, d_w, d_v,
+                                                                   acc, cnt);
+        SB_LAUNCH_CHECK();
+    }
+    int fb = (int)((bins + 255) / 256);
+    fb = fb > 1024 ? 1024 : fb;
+    vlbi_finalise_kernel<<<dim3(fb, n_dish), 256, 0, st>>>(rg, acc, cnt);
+    SB_LAUNCH_CHECK();
+    const double scale = (double)nf * (double)nt / 4.0;
+    const size_t crop = (size_t)nf * nt;
+    if (!pow2) {
+        for (int d = 0; d < n_dish; ++d) {
+            rc = ifft2_c2c_any(acc + bins * d, n0, n1, 1, nf, nt, scale, 0, d_model + crop * d, st, 0);
+            if (rc) return rc;
+        }
+        return SB_OK;
+    }
+    // rows of every station in one launch, then the kept columns per station
+    BatchShiftedRowLoad lr{acc, n0, n1};
+    PlainRowStore<float2> rs{B1, n1};
+    SB_ROW_DISPATCH(n1, rc = (launch_row_c2c<float, N1, N2, +1>(lr, rs, (long)n_dish * n0, st)));
+    if (rc) return rc;
+    int R1, R2;
+    split_len(n0, &R1, &R2);
+    for (int d = 0; d < n_dish; ++d) {
+        StrideALoad<float2> la{B1 + bins * d, n1, R2};
+        CropStore cs{d_model + crop * d, nullptr, R1, nf, nt,
+                     (float)(scale / ((double)n0 * (double)n1))};
+        rc = cols_generic<float, +1>(la, B2, n1, n0, nt, cs, st);
+        if (rc) return rc;
+    }
     return SB_OK;
 }
 

@@ -12,6 +12,8 @@ Same function names, argument order and failure behaviour as the reference
   chisq_sweep    the chisq_calc loop of THTHSample.ipynb's chi-square search
                  (batched; host: per-curvature rev_map centres, / N)
   single_search  ththmod.py:715-895   -> sb_cs_f32 + sb_eta_sweep + host fit
+  VLBI_chunk_retrieval ththmod.py:1223-1387 -> sb_cs_f32 / sb_cs_c2c_f32 +
+                 sb_vlbi_retrieval (host: rev_map centres, input checks)
   min_edges      ththmod.py:1671-1705 (host)
   chi_par        ththmod.py:38-53     (host)
 
@@ -26,6 +28,7 @@ on the host in both implementations and must give identical numbers.  Restated
 reference code, not new design.
 """
 import ctypes
+import warnings
 
 import numpy as np
 from scipy.optimize import curve_fit
@@ -365,8 +368,12 @@ def conjugate_spectrum(dspec2, npad, pad_value=None, tau=None, tau_mask=0.0,
     the fd >= 0 half on the device (the spectrum of a real array is Hermitian;
     ``.numpy()`` still returns the full array).  ``ncols_keep`` (half-plane
     only; see needed_fd_columns) restricts the transform to the fd columns a
-    given theta grid can reach."""
+    given theta grid can reach.  A complex ``dspec2`` (a VLBI visibility) goes
+    through sb_cs_c2c_f32 and always gives the full plane (``half`` and
+    ``ncols_keep`` are ignored; ``pad_value=None`` pads with its complex mean)."""
     import torch
+    if not isinstance(dspec2, torch.Tensor) and np.iscomplexobj(dspec2):
+        return _conjugate_spectrum_c2c(np.asarray(dspec2), npad, pad_value, tau, tau_mask)
     if isinstance(dspec2, torch.Tensor):     # already staged on the device (search_batch)
         dd = dspec2
         if dd.dtype != torch.float32 or not dd.is_cuda or dd.dim() != 2 or not dd.is_contiguous():
@@ -381,11 +388,7 @@ def conjugate_spectrum(dspec2, npad, pad_value=None, tau=None, tau_mask=0.0,
         half = False        # chirp-z path for arbitrary lengths: full plane
     pitch = NT // 2 + 16 if half else NT
     cs = D.empty((NF, pitch, 2), torch.float32)
-    mask = None
-    if tau is not None and tau_mask is not None:
-        m = np.abs(U.value(tau, "us")) < float(U.value(tau_mask, "us"))
-        if m.any():
-            mask = D.upload(m.astype(np.uint8))
+    mask = _tau_rowmask(tau, tau_mask)
     keep = int(ncols_keep) if (half and ncols_keep) else 0
     _lib.check(_lib.lib.sb_cs_f32(dd.data_ptr(), nf, nt, npad, float(pad_value),
                                   D.ptr(mask), 1 if half else 0, pitch, keep,
@@ -395,6 +398,30 @@ def conjugate_spectrum(dspec2, npad, pad_value=None, tau=None, tau_mask=0.0,
                                         bound.data_ptr(), D.stream_ptr()))
     return DeviceCS(cs, nfd=NT if half else None,
                     ncols_valid=keep if keep else None, bound=bound)
+
+
+def _tau_rowmask(tau, tau_mask):
+    if tau is None or tau_mask is None:
+        return None
+    m = np.abs(U.value(tau, "us")) < float(U.value(tau_mask, "us"))
+    return D.upload(m.astype(np.uint8)) if m.any() else None
+
+
+def _conjugate_spectrum_c2c(dspec2, npad, pad_value, tau, tau_mask):
+    """conjugate_spectrum of a complex chunk (a VLBI visibility) via sb_cs_c2c_f32:
+    always the full plane, no magnitude bound."""
+    import torch
+    if dspec2.ndim != 2:
+        raise ValueError("dynamic spectrum must be 2-D, got shape %r" % (dspec2.shape,))
+    nf, nt = dspec2.shape
+    dd = D.upload_f32(dspec2.astype(np.complex128))
+    pad = complex(np.nan, 0.0) if pad_value is None else complex(pad_value)
+    NF, NT = (npad + 1) * nf, (npad + 1) * nt
+    cs = D.empty((NF, NT, 2), torch.float32)
+    mask = _tau_rowmask(tau, tau_mask)
+    _lib.check(_lib.lib.sb_cs_c2c_f32(dd.data_ptr(), nf, nt, npad, pad.real, pad.imag,
+                                      D.ptr(mask), cs.data_ptr(), D.stream_ptr()))
+    return DeviceCS(cs)
 
 
 def peak_fit(etas, eigs, fw):
@@ -796,24 +823,28 @@ def single_chunk_retrieval(params):
     return (model_E, idx_f, idx_t)
 
 
-def _rev_centres(th, tau, fd, etas):
+def _rev_centres(th, tau, fd, etas, min_crop=3):
     """rev_map bin centres of modeler for every curvature: theta_centres of the
     edges_red of thth_redmap (ththmod.py:153-170, :204-205), with the
     reference's expressions.  Returns float64 [neta][len(th)] (row k holds the
     cropped count of them) and, per curvature, the exception numpy raises on the
-    way (None if none).  Crops of fewer than 3 centres are left to the device,
-    which reports them as SB_ETA_TOO_SMALL."""
+    way (None if none).  Crops of fewer than ``min_crop`` centres are skipped (the
+    chi-square path leaves them to the device, which reports SB_ETA_TOO_SMALL);
+    with ``min_crop=0`` they give the reference's own exception: IndexError from
+    edges_red for 0 or 1 centres, ValueError from the centres of 2."""
     out = np.zeros((etas.shape[0], th.shape[0]))
     errs = [None] * etas.shape[0]
     for k, eta in enumerate(etas):
         sel = ((th ** 2) * eta < np.abs(tau.max())) * (np.abs(th) < np.abs(fd.max()) / 2)
         m = int(sel.sum())
-        if m < 3:
+        if m < min_crop:
             continue
         try:
             er = th[sel]
             er = (er[:-1] + er[1:]) / 2
-            step = np.diff(er).mean()
+            with warnings.catch_warnings():      # a crop of 2: the mean of no steps is NaN
+                warnings.simplefilter("ignore", RuntimeWarning)
+                step = np.diff(er).mean()
             edges_red = np.concatenate((np.array([er[0] - step]), er, np.array([er[-1] + step])))
             out[k, :m] = theta_centres(edges_red)
         except Exception as e:  # noqa: BLE001  (raised again by chisq_calc)
@@ -898,6 +929,96 @@ def chisq_calc(dspec, CS, tau, fd, eta, edges, N, mask=None):
     if errs[0] is not None:
         raise errs[0]
     return ssq[0] / np.asarray(N, dtype=np.float64)
+
+
+def _vlbi_auto_indices(n_dish):
+    """Positions of the station spectra in [I1, V12, .., V1N, I2, V23, .., IN]
+    (ththmod.py:1289-1291)."""
+    return {n_dish * (n_dish + 1) // 2 - (n_dish - d) * (n_dish - d + 1) // 2
+            for d in range(n_dish)}
+
+
+def _vlbi_run(dspec2_list, edges, time, freq, eta, npad, n_dish, tauMask, tol=0.0, max_iter=0):
+    """Conjugate spectra (sb_cs_f32 / sb_cs_c2c_f32, full plane) and sb_vlbi_retrieval for
+    one chunk.  Returns (model_E complex128 [n_dish][nf][nt], w, V complex128
+    [n_dish nred], info dict with iters / status / nred, host-side error or None)."""
+    import torch
+    n_dish = int(n_dish)
+    if n_dish < 1:
+        raise ValueError("n_dish must be at least 1, got %d" % n_dish)
+    dl = [np.asarray(d) for d in dspec2_list]
+    if len(dl) != n_dish * (n_dish + 1) // 2:
+        raise ValueError("dspec2_list has %d entries; %d stations need n_dish (n_dish + 1) / 2 = %d"
+                         % (len(dl), n_dish, n_dish * (n_dish + 1) // 2))
+    shape = dl[0].shape
+    if len(shape) != 2:
+        raise ValueError("dynamic spectra must be 2-D, got shape %r" % (shape,))
+    for k, d in enumerate(dl):
+        if d.shape != shape:
+            raise ValueError("dspec2_list[%d] has shape %r, dspec2_list[0] %r" % (k, d.shape, shape))
+        if not np.all(np.isfinite(d)):
+            raise ValueError("dspec2_list[%d] is not finite" % k)
+    npad = int(npad)
+    time_v, freq_v = U.value(time, "s"), U.value(freq, "MHz")
+    eta_v = float(U.value(eta, "s3"))
+    fd = U.value(fft_axis(time_v, "mHz", npad), "mHz")
+    tau = U.value(fft_axis(freq_v, "us", npad), "us")
+    tm = float(U.value(tauMask, "us"))
+    autos = _vlbi_auto_indices(n_dish)
+    cs_list = [conjugate_spectrum(d, npad, None if k in autos else 0.0, tau, tm, half=False)
+               for k, d in enumerate(dl)]
+    geom = _Geom(cs_list[0], tau, fd, edges, True)
+    # min_crop=0: a crop of fewer than 3 centres raises what the reference raises there
+    th_red, errs = _rev_centres(geom.th, tau, fd, np.array([eta_v]), min_crop=0)
+    n_th = geom.th.shape[0]
+    nf, nt = shape
+    ptrs = (ctypes.c_void_p * len(cs_list))(*[c.t.data_ptr() for c in cs_list])
+    d_th = D.upload(np.ascontiguousarray(th_red[0]))
+    model = D.empty((n_dish, nf, nt, 2), torch.float32)
+    w = D.empty((1,), torch.float64)
+    V = D.zeros((n_dish * n_th, 2), torch.float32)
+    info = D.zeros((3,), torch.int32)
+    _lib.check(_lib.lib.sb_vlbi_retrieval(
+        geom.ref, ptrs, n_dish, eta_v, d_th.data_ptr(), float(tau[1] - tau[0]),
+        float(fd[1] - fd[0]), nf, nt, float(tol), int(max_iter), model.data_ptr(),
+        w.data_ptr(), V.data_ptr(), info.data_ptr(), D.stream_ptr()))
+    iv = info.cpu().numpy()
+    inf = dict(iters=int(iv[0]), status=int(iv[1]), nred=int(iv[2]))
+    return _c64(model), float(w.cpu()[0]), _c64(V)[:n_dish * inf["nred"]], inf, errs[0]
+
+
+def VLBI_chunk_retrieval(params):
+    """Phase retrieval on one chunk from several stations' dynamic spectra and their
+    visibilities (ththmod.py:1223-1387; Baker et al. 2023).  ``params`` is the
+    reference's tuple (dspec2_list, edges, time, freq, eta, idx_t, idx_f, npad,
+    n_dish, tauMask, verbose) with dspec2_list ordered [I1, V12, .., V1N, I2, V23,
+    .., IN]; returns (model_E, idx_f, idx_t), model_E a list of n_dish complex
+    wavefields.  Raises where the reference raises: IndexError when the theta grid
+    reaches past the fd axis, scipy's ArpackError when every spectrum is zero,
+    IndexError (0 or 1) or ValueError (2) when the crop keeps fewer than 3 theta
+    centres.  ValueError for a list length other than n_dish (n_dish + 1) / 2,
+    mismatched shapes or non-finite input."""
+    (dspec2_list, edges, time, freq, eta, idx_t, idx_f, npad, n_dish, tauMask,
+     verbose) = params
+    if verbose:
+        print("Starting Chunk %s-%s" % (idx_f, idx_t), flush=True)
+    model, _, _, info, err = _vlbi_run(dspec2_list, edges, time, freq, eta, npad, n_dish,
+                                       tauMask)
+    st = info["status"]
+    if st & 1:
+        raise IndexError("theta-theta point maps outside the conjugate "
+                         "spectrum (fd_inv < -nfd)")
+    if err is not None:          # fewer than 3 centres in the crop (SB_ETA_TOO_SMALL included)
+        raise err
+    if st & 2:
+        from scipy.sparse.linalg import ArpackError
+        # what eigsh raises in the reference: every start vector maps to zero
+        raise ArpackError(-9, {-9: "Starting vector is zero (the composite matrix is zero)."})
+    if st & 8:
+        raise np.linalg.LinAlgError("top eigenpair did not converge")
+    if verbose:
+        print("Chunk %s-%s success" % (idx_f, idx_t), flush=True)
+    return ([model[d] for d in range(model.shape[0])], idx_f, idx_t)
 
 
 def mask_func(w):
