@@ -348,6 +348,37 @@ int sb_vlbi_retrieval(const sb_thth_geom* geom, const void* const* cs_list_host,
                       int32_t nf, int32_t nt, double tol, int32_t max_iter, void* model_e,
                       double* w, void* v, int32_t* info, void* stream);
 
+/* ththmod.calc_asymmetry (:2385-2463) for nchunk chunks after their conjugate
+ * spectra (made by sb_cs_f32 with the chunk's mean as pad value; no tau mask),
+ * i.e. the chunk loop of Dynspec.calc_asymmetry (dynspec.py:1892-1918), in one
+ * launch sequence with no host synchronisation.  geoms_host: host array of
+ * nchunk geometries, one per chunk, each with its own cs, delay / Doppler axes
+ * and theta grid (th_cents and th_cents_host); all of them share ntau, nfd,
+ * n_th and the spectrum layout (cs_half, cs_pitch, cs_valid_cols, coherent),
+ * else SB_ERR_ARG.  etas: device float64 [nchunk].  Per chunk:
+ *   - crop and gather of thth_redmap (hermetian=True), as sb_eta_sweep;
+ *   - top eigenpair (w, V) as sb_herm_eigvec, one thread block per chunk,
+ *     starting from row n//2 or, if that row is zero, from a fixed vector;
+ *   - with m = nred and h = (m - 1) // 2, in float64:
+ *     asym = (sum |V[:h]|^2 - sum |V[h+1:]|^2) / (sum |V[:h]|^2 + sum |V[h+1:]|^2).
+ * Outputs (device, [nchunk] each): asym float64 (NaN where the reference's
+ * try/except gives NaN: status bits SB_ETA_INDEX_ERROR, SB_ETA_ZERO_START (a
+ * zero matrix), SB_ETA_TOO_SMALL (fewer than 3 centres), SB_ETA_NOT_CONVERGED;
+ * 0 / 0 is NaN); w float64 (NaN for INDEX_ERROR / TOO_SMALL, 0 for a zero
+ * matrix); status (SB_ETA_* bits); nred (cropped size); iters (Lanczos steps);
+ * v float2 [nchunk][ld], ld = n_th rounded up to a multiple of 32, or NULL:
+ * each chunk's unit eigenvector (arbitrary global phase) zero-padded to ld,
+ * zeros where none was computed.  tol (<= 0: 1e-7) and max_iter (<= 0: 96) as
+ * sb_herm_eigvec.  Chunks run in batches whose matrix, Lanczos basis and vector
+ * fit the 3 GiB budget of sb_eta_sweep (SB_SWEEP_SLAB_MB overrides it).
+ * Limits, checked before any workspace is allocated: n_th <= 4096
+ * (SB_ERR_UNSUPPORTED); spectra of the sizes sb_cs_f32 makes: powers of two in
+ * 4..65536 x 16..32768 (full or half plane), other sizes in 3..32768 x 3..8192
+ * (full plane only). */
+int sb_asymmetry_batch(const sb_thth_geom* geoms_host, int32_t nchunk, const double* etas,
+                       double tol, int32_t max_iter, double* asym, double* w, int32_t* status,
+                       int32_t* nred, int32_t* iters, void* v, void* stream);
+
 /* ---- scint_sim.Simulation ------------------------------------------------ */
 
 typedef struct sb_sim_params {

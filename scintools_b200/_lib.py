@@ -85,6 +85,8 @@ _SIGS = {
     "sb_cs_c2c_f32": (c_int, [vp, c_int, c_int, c_int, c_flt, c_flt, vp, vp, vp]),
     "sb_vlbi_retrieval": (c_int, [ctypes.POINTER(ThthGeom), vp, c_int, c_dbl, vp, c_dbl, c_dbl,
                                   c_int, c_int, c_dbl, c_int, vp, vp, vp, vp, vp]),
+    "sb_asymmetry_batch": (c_int, [ctypes.POINTER(ThthGeom), c_int, vp, c_dbl, c_int, vp, vp, vp,
+                                   vp, vp, vp, vp]),
     "sb_sim_weights": (c_int, [ctypes.POINTER(SimParams), vp, vp]),
     "sb_sim_screen": (c_int, [c_int, c_int, vp, vp, vp, ctypes.c_uint64, vp, vp]),
     "sb_sim_intensity": (c_int, [c_int, c_int, c_int, vp, vp, c_dbl, c_dbl, vp,

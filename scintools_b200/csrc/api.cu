@@ -157,6 +157,9 @@ int vlbi_retrieval(const ThthGeom& g, const double* th_host, const float2* const
                    int n_dish, double eta, const double* d_th_red, double dtau_bin,
                    double dfd_bin, int nf, int nt, double tol, int max_iter, float2* d_model,
                    double* d_w, float2* d_v, int* d_info, cudaStream_t st);
+int asymmetry_batch(const ThthGeom* geoms, const double* const* th_host, int nchunk,
+                    const double* d_etas, double tol, int max_iter, double* d_asym, double* d_w,
+                    int* d_status, int* d_nred, int* d_iters, float2* d_v, cudaStream_t st);
 
 int gerchberg_saxton(float2* W, const float* amp, const unsigned char* rowmask, int n0, int n1,
                      int niter, cudaStream_t st);
@@ -205,7 +208,7 @@ static int to_geom(const sb_thth_geom* in, ThthGeom* g) {
 
 extern "C" {
 
-int sb_abi_version(void) { return 4; }
+int sb_abi_version(void) { return 5; }
 const char* sb_last_error(void) { return sb::last_error(); }
 
 int sb_init(int device) {
@@ -441,6 +444,22 @@ int sb_vlbi_retrieval(const sb_thth_geom* geom, const void* const* cs_list_host,
     return sb::vlbi_retrieval(g, geom->th_cents_host, (const float2* const*)cs_list_host, n_dish,
                               eta, th_red, dtau_bin, dfd_bin, nf, nt, tol, max_iter,
                               (float2*)model_e, w, (float2*)v, info, (cudaStream_t)stream);
+}
+
+int sb_asymmetry_batch(const sb_thth_geom* geoms_host, int32_t nchunk, const double* etas,
+                       double tol, int32_t max_iter, double* asym, double* w, int32_t* status,
+                       int32_t* nred, int32_t* iters, void* v, void* stream) {
+    SB_ARG(nchunk >= 0 && (nchunk == 0 || geoms_host));
+    SB_ARG(etas && asym && w && status && nred && iters);
+    std::vector<sb::ThthGeom> g((size_t)nchunk);
+    std::vector<const double*> th((size_t)nchunk);
+    for (int k = 0; k < nchunk; ++k) {
+        int rc = sb::to_geom(geoms_host + k, &g[k]);
+        if (rc) return rc;
+        th[k] = geoms_host[k].th_cents_host;
+    }
+    return sb::asymmetry_batch(g.data(), th.data(), nchunk, etas, tol, max_iter, asym, w, status,
+                               nred, iters, (float2*)v, (cudaStream_t)stream);
 }
 
 int sb_sim_weights(const sb_sim_params* p, double* w, void* stream) {

@@ -6,8 +6,9 @@
 //   chisq_sweep  ththmod.py:330-368   chisq_calc over a batch of curvatures
 //   vlbi_retrieval ththmod.py:1223-1387 VLBI_chunk_retrieval after the spectra, and
 //                conj_spectrum_c2c    the conjugate spectrum of its complex visibilities
+//   asymmetry_batch ththmod.py:2385-2463 calc_asymmetry over a batch of chunks
 // used by the Python mirrors of modeler / single_chunk_retrieval / chisq_calc /
-// VLBI_chunk_retrieval.
+// VLBI_chunk_retrieval / calc_asymmetry.
 #include <float.h>
 #include <limits.h>
 #include <math.h>
@@ -479,6 +480,57 @@ herm_eigvec_batch_kernel(const float2* __restrict__ M, int ld, const int* __rest
 }
 
 // --------------------------------------------------------------------------
+// calc_asymmetry (ththmod.py:2385-2463) over a batch of chunks, each with its own
+// spectrum, axes, theta grid and curvature (geoms[e], etas[e]).
+// --------------------------------------------------------------------------
+// Strict upper triangle of every cropped matrix of chunks e0 .. e0 + gridDim.y - 1 into
+// M [nb][ld][ld] (the layout herm_eigvec_batch_kernel reads): thth_redmap's Hermitian
+// fill of the crop idx[e][0 .. nred[e]).
+__global__ void asym_gather_kernel(const ThthGeom* __restrict__ geoms,
+                                   const double* __restrict__ etas, int e0, int ld,
+                                   const int* __restrict__ idx, const int* __restrict__ nred,
+                                   float2* __restrict__ M) {
+    const int e = blockIdx.y, ge = e0 + e;
+    const ThthGeom g = geoms[ge];
+    const double eta = etas[ge];
+    const int n = nred[ge];
+    const int* id = idx + (size_t)ge * ld;
+    float2* Me = M + (size_t)e * ld * ld;
+    for (long p = blockIdx.x * (long)blockDim.x + threadIdx.x; p < (long)n * n;
+         p += (long)gridDim.x * blockDim.x) {
+        const int a = (int)(p / n), c = (int)(p - (long)a * n);
+        if (c > a) Me[(size_t)a * ld + c] = thth_herm_upper(g, eta, id[a], id[c]);
+    }
+}
+
+// asymm = (|V[:h]|^2 - |V[h+1:m]|^2) / (|V[:h]|^2 + |V[h+1:m]|^2), h = (m - 1) // 2, in fp64
+// from the fp32 eigenvector V [nb][ld] of each chunk (one warp per chunk).  NaN where the
+// reference's try/except stores NaN: IndexError, a zero matrix, m < 3, no convergence
+// (status bits 1, 2, 4, 8); 0 / 0 is NaN as in numpy.  v_out [nchunk][ld] (optional): V,
+// zero-padded, or zeros where no eigenvector was computed (bits 1, 4).
+__global__ void asym_finish_kernel(const float2* __restrict__ V, int ld,
+                                   const int* __restrict__ nred, const int* __restrict__ status,
+                                   int e0, double* __restrict__ asym, float2* __restrict__ v_out) {
+    const int e = blockIdx.x, ge = e0 + e, lane = threadIdx.x;
+    const int m = nred[ge], st = status[ge];
+    const float2* v = V + (size_t)e * ld;
+    const int h = (m - 1) / 2;
+    const bool has_v = !(st & 5);
+    double l = 0.0, r = 0.0;
+    for (int c = lane; c < ld; c += 32) {
+        const float2 x = (has_v && c < m) ? v[c] : make_float2(0.f, 0.f);
+        const double p = (double)x.x * x.x + (double)x.y * x.y;
+        if (c < h) l += p;
+        else if (c > h) r += p;
+        if (v_out) v_out[(size_t)ge * ld + c] = x;
+    }
+    l = warp_sum(l);
+    r = warp_sum(r);
+    if (lane == 0)
+        asym[ge] = (st & 15) ? __longlong_as_double(0x7ff8000000000000LL) : (l - r) / (l + r);
+}
+
+// --------------------------------------------------------------------------
 // VLBI_chunk_retrieval (ththmod.py:1223-1387): the composite theta-theta matrix of
 // n_dish stations, its top eigenpair and one wavefield per station.
 // Spectra are in reference order [I1, V12, .., V1N, I2, V23, .., IN]; pair (d1, d1 + d2)
@@ -515,16 +567,13 @@ __global__ void vlbi_composite_kernel(ThthGeom g, const double* __restrict__ eta
         float2 v;
         if (d2 != 0) {
             v = thth_value(gk, eta, thj, thi, thth_point(gk, eta, thj, thi));
-        } else if (i == j || i + j == g.n - 1) {
+        } else if (i == j) {
             v = make_float2(0.f, 0.f);
         } else if (j > i) {
-            v = thth_value(gk, eta, thj, thi, thth_point(gk, eta, thj, thi));
-            v.x = nan_to_num(v.x);
-            v.y = nan_to_num(v.y);
+            v = thth_herm_upper(gk, eta, i, j);
         } else {                                     // conj of the upper element (j, i)
-            v = thth_value(gk, eta, thi, thj, thth_point(gk, eta, thi, thj));
-            v.x = nan_to_num(v.x);
-            v.y = -nan_to_num(v.y);
+            v = thth_herm_upper(gk, eta, j, i);
+            v.y = -v.y;
         }
         if (upper) v.y = -v.y;
         A[p] = v;
@@ -1268,6 +1317,93 @@ int vlbi_retrieval(const ThthGeom& geom, const double* th_host, const float2* co
                      (float)(scale / ((double)n0 * (double)n1))};
         rc = cols_generic<float, +1>(la, B2, n1, n0, nt, cs, st);
         if (rc) return rc;
+    }
+    return SB_OK;
+}
+
+// --------------------------------------------------------------------------
+// calc_asymmetry over nchunk chunks after their spectra (ththmod.py:2385-2463): crop and
+// gather, top eigenpair, asymmetry of V.  Chunks run in batches under the sweep's slab
+// budget; one launch sequence, no host synchronisation, nchunk numbers per output.
+// --------------------------------------------------------------------------
+int thth_prep_table(const ThthGeom* geoms, const double* const* th_host, const ThthGeom* d_geoms,
+                    const double* d_etas, int n, int ld, int* d_idx, int* d_nred, int* d_status,
+                    cudaStream_t st);
+
+int asymmetry_batch(const ThthGeom* geoms, const double* const* th_host, int nchunk,
+                    const double* d_etas, double tol, int max_iter, double* d_asym, double* d_w,
+                    int* d_status, int* d_nred, int* d_iters, float2* d_v, cudaStream_t st) {
+    if (nchunk <= 0) return SB_OK;
+    const ThthGeom& g0 = geoms[0];
+    for (int k = 0; k < nchunk; ++k) {
+        const ThthGeom& g = geoms[k];
+        if (!g.cs) {
+            set_error("asymmetry_batch: conjugate spectrum of chunk %d is null", k);
+            return SB_ERR_ARG;
+        }
+        if (g.ntau != g0.ntau || g.nfd != g0.nfd || g.n != g0.n || g.cs_half != g0.cs_half ||
+            g.cs_pitch != g0.cs_pitch || g.cs_valid_cols != g0.cs_valid_cols ||
+            g.coherent != g0.coherent) {
+            set_error("asymmetry_batch: chunk %d differs from chunk 0 in spectrum size, theta "
+                      "grid size or spectrum layout", k);
+            return SB_ERR_ARG;
+        }
+    }
+    if (g0.n > 4096) {
+        set_error("asymmetry_batch: theta-theta grid of %d centres exceeds the supported 4096",
+                  g0.n);
+        return SB_ERR_UNSUPPORTED;
+    }
+    // the spectra sb_cs_f32 makes: powers of two up to 65536 x 32768 (radix path, full or
+    // half plane), any other size in 3..32768 x 3..8192 (chirp-z path, full plane)
+    const long long n0 = g0.ntau, n1 = g0.nfd;
+    const bool radix = is_pow2(n0) && is_pow2(n1) && n0 >= 4 && n1 >= 16;
+    if (radix ? (n0 > 65536 || n1 > 32768)
+              : (g0.cs_half || n0 < 3 || n1 < 3 || n0 > 32768 || n1 > 8192)) {
+        set_error("asymmetry_batch: conjugate spectrum %lld x %lld outside 4..65536 x 16..32768 "
+                  "(powers of two) / 3..32768 x 3..8192 (other sizes, full plane)", n0, n1);
+        return SB_ERR_UNSUPPORTED;
+    }
+    if (!(tol > 0.0)) tol = 1e-7;
+    if (max_iter <= 0 || max_iter > SB_LANCZOS_MAXIT) max_iter = 96;
+    const int ld = (g0.n + 31) / 32 * 32;
+    if (max_iter > ld) max_iter = ld;
+    // per chunk: matrix, Lanczos basis, eigenvector, under the sweep's slab budget
+    const size_t mat = (size_t)ld * ld, qn = (size_t)(max_iter + 1) * ld;
+    const size_t per = (mat + qn + ld) * sizeof(float2);
+    unsigned long long b = sweep_slab_bytes() / per;
+    int batch = (int)(b < 1 ? 1 : (b > 65535 ? 65535 : b));
+    if (batch > nchunk) batch = nchunk;
+    // slot 1: geometry table and crop indices; slot 2: the batch's matrices, bases, vectors
+    const size_t tab = ((size_t)nchunk * sizeof(ThthGeom) + 255) / 256 * 256;
+    unsigned char* s1 = (unsigned char*)workspace(1, tab + (size_t)nchunk * ld * sizeof(int));
+    unsigned char* s2 = (unsigned char*)workspace(2, per * batch);
+    if (!s1 || !s2) return SB_ERR_NOMEM;
+    ThthGeom* d_geoms = (ThthGeom*)s1;
+    int* d_idx = (int*)(s1 + tab);
+    float2* M = (float2*)s2;
+    float2* Q = M + mat * batch;
+    float2* V = Q + qn * batch;
+    SB_CUDA(cudaMemcpyAsync(d_geoms, geoms, (size_t)nchunk * sizeof(ThthGeom),
+                            cudaMemcpyHostToDevice, st));
+    int rc = thth_prep_table(geoms, th_host, d_geoms, d_etas, nchunk, ld, d_idx, d_nred, d_status,
+                             st);
+    if (rc) return rc;
+    const size_t smem = sizeof(LanczosShared) + 32 * sizeof(double) +
+                        (SB_LANCZOS_MAXIT + 1) * sizeof(double2) + 2 * (size_t)ld * sizeof(float2);
+    SB_CUDA(cudaFuncSetAttribute(herm_eigvec_batch_kernel,
+                                 cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int gb = (int)((mat + 255) / 256);
+    gb = gb > 32 ? 32 : gb;
+    for (int e0 = 0; e0 < nchunk; e0 += batch) {
+        const int nb = nchunk - e0 < batch ? nchunk - e0 : batch;
+        asym_gather_kernel<<<dim3(gb, nb), 256, 0, st>>>(d_geoms, d_etas, e0, ld, d_idx, d_nred, M);
+        SB_LAUNCH_CHECK();
+        herm_eigvec_batch_kernel<<<nb, EV_THREADS, smem, st>>>(M, ld, d_nred, e0, Q, max_iter, tol,
+                                                              d_w, V, d_status, d_iters);
+        SB_LAUNCH_CHECK();
+        asym_finish_kernel<<<nb, 32, 0, st>>>(V, ld, d_nred, d_status, e0, d_asym, d_v);
+        SB_LAUNCH_CHECK();
     }
     return SB_OK;
 }

@@ -41,15 +41,11 @@ enum { ST_OK = 0, ST_INDEX_ERROR = 1, ST_ZERO_START = 2, ST_TOO_SMALL = 4,
 // crop mask + compaction: th_pnts of thth_redmap (ththmod.py:153-156)
 // one warp per eta
 // --------------------------------------------------------------------------
-__global__ void thth_prep_kernel(ThthGeom g, const double* __restrict__ etas,
-                                 int neta, int ld, int* __restrict__ idx,
-                                 int* __restrict__ nred) {
-    int e = blockIdx.x;
-    if (e >= neta) return;
-    double eta = etas[e];
+// one warp: the kept centres of geometry g at curvature eta into out[0 .. *nred)
+__device__ __forceinline__ void thth_crop_warp(const ThthGeom& g, double eta,
+                                               int* __restrict__ out, int* __restrict__ nred) {
     int lane = threadIdx.x;
     int base = 0;
-    int* out = idx + (size_t)e * ld;
     for (int k0 = 0; k0 < g.n; k0 += 32) {
         int k = k0 + lane;
         bool keep = false;
@@ -62,17 +58,32 @@ __global__ void thth_prep_kernel(ThthGeom g, const double* __restrict__ etas,
         if (keep) out[base + __popc(m & ((1u << lane) - 1u))] = k;
         base += __popc(m);
     }
-    if (lane == 0) nred[e] = base;
+    if (lane == 0) *nred = base;
+}
+
+__global__ void thth_prep_kernel(ThthGeom g, const double* __restrict__ etas,
+                                 int neta, int ld, int* __restrict__ idx,
+                                 int* __restrict__ nred) {
+    int e = blockIdx.x;
+    if (e >= neta) return;
+    thth_crop_warp(g, etas[e], idx + (size_t)e * ld, nred + e);
+}
+
+// the same for a table of geometries, one per item (sb_asymmetry_batch: one per chunk)
+__global__ void thth_prep_table_kernel(const ThthGeom* __restrict__ geoms,
+                                       const double* __restrict__ etas, int ld,
+                                       int* __restrict__ idx, int* __restrict__ nred) {
+    const int e = blockIdx.x;
+    const ThthGeom g = geoms[e];
+    thth_crop_warp(g, etas[e], idx + (size_t)e * ld, nred + e);
 }
 
 // --------------------------------------------------------------------------
 // rare path: would numpy raise IndexError anywhere in the full N x N map?
 // (fd_inv < -nfd on a point that passes the pnts mask, ththmod.py:100-104)
 // --------------------------------------------------------------------------
-__global__ void thth_indexerr_kernel(ThthGeom g, const double* __restrict__ etas,
-                                     int* __restrict__ status) {
-    int e = blockIdx.y;
-    double eta = etas[e];
+__device__ __forceinline__ void thth_indexerr_body(const ThthGeom& g, double eta,
+                                                   int* __restrict__ status) {
     long long total = (long long)g.n * g.n;
     bool bad = false;
     for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -82,7 +93,22 @@ __global__ void thth_indexerr_kernel(ThthGeom g, const double* __restrict__ etas
         bad |= pt.index_error;
     }
     if (__any_sync(0xffffffffu, bad) && (threadIdx.x & 31) == 0)
-        atomicOr(status + e, ST_INDEX_ERROR);
+        atomicOr(status, ST_INDEX_ERROR);
+}
+
+__global__ void thth_indexerr_kernel(ThthGeom g, const double* __restrict__ etas,
+                                     int* __restrict__ status) {
+    int e = blockIdx.y;
+    thth_indexerr_body(g, etas[e], status + e);
+}
+
+// per item e0 + blockIdx.y of a geometry table
+__global__ void thth_indexerr_table_kernel(const ThthGeom* __restrict__ geoms,
+                                           const double* __restrict__ etas, int e0,
+                                           int* __restrict__ status) {
+    const int e = e0 + blockIdx.y;
+    const ThthGeom g = geoms[e];
+    thth_indexerr_body(g, etas[e], status + e);
 }
 
 // --------------------------------------------------------------------------
@@ -780,6 +806,24 @@ int thth_prep(const ThthGeom& g, const double* th_host, const double* d_etas, in
     if (lower_check_needed(g, th_host)) {
         dim3 grid(64, neta);
         thth_indexerr_kernel<<<grid, 256, 0, st>>>(g, d_etas, d_status);
+        SB_LAUNCH_CHECK();
+    }
+    return SB_OK;
+}
+
+// thth_prep for a table of n geometries, one curvature each: geoms / th_host on the host,
+// the same geometries in d_geoms on the device
+int thth_prep_table(const ThthGeom* geoms, const double* const* th_host, const ThthGeom* d_geoms,
+                    const double* d_etas, int n, int ld, int* d_idx, int* d_nred, int* d_status,
+                    cudaStream_t st) {
+    SB_CUDA(cudaMemsetAsync(d_status, 0, n * sizeof(int), st));
+    thth_prep_table_kernel<<<n, 32, 0, st>>>(d_geoms, d_etas, ld, d_idx, d_nred);
+    SB_LAUNCH_CHECK();
+    bool check = false;
+    for (int k = 0; k < n && !check; ++k) check = lower_check_needed(geoms[k], th_host[k]);
+    for (int e0 = 0; check && e0 < n; e0 += 65535) {
+        const int nb = n - e0 < 65535 ? n - e0 : 65535;
+        thth_indexerr_table_kernel<<<dim3(64, nb), 256, 0, st>>>(d_geoms, d_etas, e0, d_status);
         SB_LAUNCH_CHECK();
     }
     return SB_OK;

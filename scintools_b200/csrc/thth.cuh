@@ -83,4 +83,15 @@ __device__ __forceinline__ float nan_to_num(float x) {
     return x;
 }
 
+// Element (i, j), i < j, of thth_map(hermetian=True) on the full grid (ththmod.py:108-114):
+// the gathered value with nan_to_num, zero on the anti-diagonal i + j == n - 1.
+__device__ __forceinline__ float2 thth_herm_upper(const ThthGeom& g, double eta, int i, int j) {
+    if (i + j == g.n - 1) return make_float2(0.f, 0.f);
+    const double thi = g.th[i], thj = g.th[j];
+    float2 v = thth_value(g, eta, thj, thi, thth_point(g, eta, thj, thi));
+    v.x = nan_to_num(v.x);
+    v.y = nan_to_num(v.y);
+    return v;
+}
+
 }  // namespace sb

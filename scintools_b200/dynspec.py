@@ -561,6 +561,41 @@ class Dynspec(ArcFitMixin):
         self.ththeta = A / self.fref ** 2
         self.ththetaerr = A_err / self.fref ** 2
 
+    def _asymmetry_params(self, verbose=False):
+        """The reference's calc_asymmetry chunk list (dynspec.py:1895-1913), including its
+        time slice ct*cwt//2 : (ct+1)*cwt, whose width grows with ct (cwt + ct*cwt/2)."""
+        pars = []
+        for cf in range(self.ncf_fit):
+            fs = slice(cf * self.cwf, (cf + 1) * self.cwf)
+            freq2 = np.copy(self.freqs[fs]).astype(np.float64)
+            freq = freq2.mean()
+            eta = self.ththeta * (self.fref / freq) ** 2
+            for ct in range(self.nct_fit):
+                ts = slice(ct * self.cwt // 2, (ct + 1) * self.cwt)
+                time2 = np.copy(self.times[ts]).astype(np.float64)
+                dspec2 = np.copy(self.dyn[fs, ts]).astype(np.float64)
+                dspec2 -= np.nanmean(dspec2)
+                dspec2 = np.nan_to_num(dspec2)
+                pars.append((dspec2, self.edges * (freq / self.fref), time2, freq2, eta, ct, cf,
+                             self.npad, verbose))
+        return pars
+
+    def calc_asymmetry(self, verbose=False, pool=None):
+        """Arc asymmetry of every fitting chunk (reference dynspec.py:1892-1918) ->
+        self.asymmetry, complex [ncf_fit][nct_fit] like the reference's array (the values
+        are real; NaN where a chunk fails).  Runs fit_thetatheta first if ththeta is not
+        set.  All chunks run through ththmod.asymmetry_batch; ``pool`` must be None (see
+        fit_thetatheta)."""
+        if pool is not None:
+            raise ValueError("calc_asymmetry on the GPU path takes pool=None "
+                             "(CUDA is not fork-safe); chunks are batched on "
+                             "the device instead")
+        if not hasattr(self, "ththeta"):
+            self.fit_thetatheta(verbose=verbose)
+        self.asymmetry = np.zeros((self.ncf_fit, self.nct_fit), dtype=complex)
+        for a, cf, ct in thth.asymmetry_batch(self._asymmetry_params(verbose)):
+            self.asymmetry[cf, ct] = a
+
     def thetatheta_chunks(self, verbose=False, pool=None, memmap=False, group=None):
         """Phase retrieval on every half-overlapping retrieval chunk
         (reference dynspec.py:1765-1828) -> self.chunks [ncf_ret][nct_ret][cwf][cwt].

@@ -14,6 +14,8 @@ Same function names, argument order and failure behaviour as the reference
   single_search  ththmod.py:715-895   -> sb_cs_f32 + sb_eta_sweep + host fit
   VLBI_chunk_retrieval ththmod.py:1223-1387 -> sb_cs_f32 / sb_cs_c2c_f32 +
                  sb_vlbi_retrieval (host: rev_map centres, input checks)
+  calc_asymmetry ththmod.py:2385-2463 -> sb_cs_f32 + sb_asymmetry_batch (one chunk)
+  asymmetry_batch the chunk loop of Dynspec.calc_asymmetry (batched per padded shape)
   min_edges      ththmod.py:1671-1705 (host)
   chi_par        ththmod.py:38-53     (host)
 
@@ -1019,6 +1021,120 @@ def VLBI_chunk_retrieval(params):
     if verbose:
         print("Chunk %s-%s success" % (idx_f, idx_t), flush=True)
     return ([model[d] for d in range(model.shape[0])], idx_f, idx_t)
+
+
+# messages printed for the chunks whose asymmetry the reference's try/except turns into NaN
+_ASYM_FAILURES = (
+    (1, "theta-theta point maps outside the conjugate spectrum (fd_inv < -nfd)"),
+    (4, "theta-theta matrix too small for eigsh (n < 3)"),
+    (2, "starting vector is zero: the theta-theta matrix is zero"),
+    (8, "top eigenpair did not converge"),
+)
+
+
+def _asym_check_sizes(NF, NT, n_th):
+    """The limits of sb_asymmetry_batch for spectra of NF x NT and n_th theta centres."""
+    if n_th > 4096:
+        raise _lib.SbError("calc_asymmetry: theta-theta grid of %d centres exceeds the "
+                           "supported 4096" % n_th)
+    pow2 = not (NF & (NF - 1)) and not (NT & (NT - 1))
+    if pow2 and NF >= 4 and NT >= 16:
+        ok = NF <= 65536 and NT <= 32768
+    else:
+        ok = 3 <= NF <= 32768 and 3 <= NT <= 8192
+    if not ok:
+        raise _lib.SbError("calc_asymmetry: padded chunk %d x %d outside 4..65536 x 16..32768 "
+                           "(powers of two) / 3..32768 x 3..8192 (other sizes)" % (NF, NT))
+
+
+def asymmetry_batch(params_list, return_info=False, tol=0.0, max_iter=0):
+    """calc_asymmetry (ththmod.py:2385-2463) over a sequence of chunks: the loop of
+    Dynspec.calc_asymmetry (dynspec.py:1892-1918).  Each entry is the reference's tuple
+    (dspec2, edges, time, freq, eta, idx_t, idx_f, npad, verbose).
+
+    Chunks are grouped by padded shape and theta grid size; per group the spectra are made
+    (sb_cs_f32, padded with each chunk's mean) and one sb_asymmetry_batch call crops,
+    gathers, solves and reduces every chunk.  Every group's sizes are checked before any
+    device work.  Returns [(asymm, idx_f, idx_t), ...] in input order; a chunk the
+    reference cannot recover prints the reason and gives NaN.  Library errors
+    (_lib.SbError) are raised.  ``return_info`` adds a dict of per-chunk arrays ``w``,
+    ``status``, ``nred``, ``iters`` and the list ``V`` of eigenvectors (length nred,
+    arbitrary global phase)."""
+    import torch
+    params_list = list(params_list)
+    prep, groups = [], {}
+    for k, p in enumerate(params_list):
+        dspec2, edges, time, freq, eta, idx_t, idx_f, npad, verbose = p
+        d = np.asarray(dspec2, dtype=np.float64)
+        if d.ndim != 2:
+            raise ValueError("dynamic spectrum must be 2-D, got shape %r" % (d.shape,))
+        npad = int(npad)
+        ev = U.value(edges, "mHz")
+        NF, NT = (npad + 1) * d.shape[0], (npad + 1) * d.shape[1]
+        prep.append((d, ev, U.value(time, "s"), U.value(freq, "MHz"),
+                     float(U.value(eta, "s3")), npad))
+        groups.setdefault((NF, NT, len(ev) - 1), []).append(k)
+    for NF, NT, n_th in groups:
+        _asym_check_sizes(NF, NT, n_th)
+    n = len(params_list)
+    asym = np.full(n, np.nan)
+    info = dict(w=np.full(n, np.nan), status=np.zeros(n, np.int32), nred=np.zeros(n, np.int32),
+                iters=np.zeros(n, np.int32), V=[None] * n)
+    for p in params_list:
+        if p[8]:
+            print("Starting Chunk %s-%s" % (p[6], p[5]), flush=True)
+    for (NF, NT, n_th), ks in groups.items():
+        keep = []
+        for k in ks:
+            d, ev, time_v, freq_v, _, npad = prep[k]
+            fd = U.value(fft_axis(time_v, "mHz", npad), "mHz")
+            tau = U.value(fft_axis(freq_v, "us", npad), "us")
+            cs = conjugate_spectrum(d, npad, None)
+            keep.append(_Geom(cs, tau, fd, ev, True))
+        nb = len(ks)
+        geoms = (_lib.ThthGeom * nb)(*[g.g for g in keep])
+        d_etas = D.upload(np.array([prep[k][4] for k in ks]))
+        ld = (n_th + 31) // 32 * 32
+        out = D.empty((nb,), torch.float64)
+        w = D.empty((nb,), torch.float64)
+        aux = [D.empty((nb,), torch.int32) for _ in range(3)]
+        V = D.empty((nb, ld, 2), torch.float32) if return_info else None
+        _lib.check(_lib.lib.sb_asymmetry_batch(
+            geoms, nb, d_etas.data_ptr(), float(tol), int(max_iter), out.data_ptr(),
+            w.data_ptr(), aux[0].data_ptr(), aux[1].data_ptr(), aux[2].data_ptr(), D.ptr(V),
+            D.stream_ptr()))
+        asym[ks] = out.cpu().numpy()
+        for key, t in zip(("w", "status", "nred", "iters"), [w] + aux):
+            info[key][ks] = t.cpu().numpy()
+        if return_info:
+            Vh = _c64(V)
+            for j, k in enumerate(ks):
+                info["V"][k] = Vh[j, :info["nred"][k]]
+        del keep
+    res = []
+    for k, p in enumerate(params_list):
+        idx_t, idx_f, verbose = p[5], p[6], p[8]
+        st = int(info["status"][k])
+        msg = [m for bit, m in _ASYM_FAILURES if st & bit]
+        if msg:
+            print(msg[0], flush=True)
+        elif verbose:       # 0 / 0 (no weight off the centre element) is NaN without an error
+            print("Chunk %s-%s success" % (idx_f, idx_t), flush=True)
+        res.append((float(asym[k]), idx_f, idx_t))
+    if return_info:
+        return res, info
+    return res
+
+
+def calc_asymmetry(params):
+    """Arc asymmetry of one chunk from its theta-theta eigenvector (ththmod.py:2385-2463).
+    ``params`` is the reference's tuple (dspec2, edges, time, freq, eta, idx_t, idx_f,
+    npad, verbose); returns (asymm, idx_f, idx_t).  The chunk is padded with its mean;
+    the eigenvector V of the cropped matrix (m centres) gives
+    (|V[:(m-1)//2]|^2 - |V[(m+1)//2:]|^2) / (|V[:(m-1)//2]|^2 + |V[(m+1)//2:]|^2).
+    A chunk the reference cannot recover prints the reason and gives NaN; library errors
+    (_lib.SbError: unsupported size, CUDA) are raised.  Same kernels as asymmetry_batch."""
+    return asymmetry_batch([params])[0]
 
 
 def mask_func(w):
