@@ -210,24 +210,20 @@ def test_default_sweep_kernels_on_host(golden_dir, mixed, slots):
     assert (np.abs(eigs - ref) / ref).max() < 1e-5, (eigs, ref)
 
 
-def test_thin_kernels_on_host(golden_dir):
-    """csrc/thin.cu (prep, index check, two-curvature gather, sigma_max by
-    Lanczos on A^H A) under the SIMT emulator against the reference's
-    singularvalue_calc values (tests/golden/thth_thin_64x150.npz)."""
+def _thin_emu(golden_dir, e1, e2, etas, cut):
+    """sigma_max of every curvature from csrc/thin.cu under the SIMT emulator, on the
+    tutorial chunk of thth_sample_64x150.npz; returns (sv, status, CS, tau, fd)."""
     from oracle import thth_oracle as TO
     lib = _build("thin_emu")
     g = np.load(os.path.join(golden_dir, "thth_sample_64x150.npz"))
-    t = np.load(os.path.join(golden_dir, "thth_thin_64x150.npz"))
     d0 = g["dspec2"] - g["dspec2"].mean()
     CS = TO.conjugate_spectrum(d0, int(g["npad"]), 0.0)
     cs32 = np.ascontiguousarray(CS.astype(np.complex64))
     tau, fd = g["tau"], g["fd"]
-    e1, e2 = t["edges"], t["arc"]
     th1 = np.ascontiguousarray((e1[1:] + e1[:-1]) / 2)
     th2 = np.ascontiguousarray((e2[1:] + e2[:-1]) / 2)
-    sel = [2, 8, 15]
-    etas = np.ascontiguousarray(t["etas"][sel])
-    neta = len(sel)
+    etas = np.ascontiguousarray(etas)
+    neta = len(etas)
     sv = np.zeros(neta)
     status = np.zeros(neta, np.int32)
     n1r = np.zeros(neta, np.int32)
@@ -240,11 +236,38 @@ def test_thin_kernels_on_host(golden_dir):
     rc = lib.emu_thin_sweep(P(cs32), CS.shape[0], CS.shape[1], float(tau[1]),
                             float(np.diff(tau).mean()), float(tau.max()), float(fd[1]),
                             float(np.diff(fd).mean()), P(th1), len(th1), P(th2), len(th2),
-                            float(t["cut"]), 0, P(etas), P(etas), neta, 2e-5, 0, P(sv), P(status),
+                            float(cut), 0, P(etas), P(etas), neta, 2e-5, 0, P(sv), P(status),
                             P(n1r), P(n2r), P(iters))
     assert rc == 0
+    return sv, status, n1r, CS, tau, fd
+
+
+def test_thin_kernels_on_host(golden_dir):
+    """csrc/thin.cu (prep, index check, two-curvature gather, sigma_max by
+    Lanczos on A^H A) under the SIMT emulator against the reference's
+    singularvalue_calc values (tests/golden/thth_thin_64x150.npz)."""
+    t = np.load(os.path.join(golden_dir, "thth_thin_64x150.npz"))
+    sel = [2, 8, 15]
+    sv, status, _, _, _, _ = _thin_emu(golden_dir, t["edges"], t["arc"], t["etas"][sel], t["cut"])
     assert (status == 0).all(), status
     ref = t["sv"][sel]
+    assert (np.abs(sv - ref) / ref).max() < 1e-5, (sv, ref)
+
+
+def test_thin_three_column_chunks_on_host(golden_dir):
+    """1025 theta1 columns: thin_sv_kernel walks three column chunks of 512 (the last
+    one column wide) in its row dot products and its conjugate accumulation.  The
+    center cut zeroes columns of the first two chunks.  Against the oracle's
+    singularvalue_calc on the same spectrum."""
+    from oracle import thth_oracle as TO
+    e1 = np.linspace(-0.4, 0.4, 1026)
+    e2 = np.linspace(-0.25, 0.25, 34)
+    etas = np.array([15.0, 20.0])          # below tau.max / 0.4^2: no column is cropped
+    sv, status, n1, CS, tau, fd = _thin_emu(golden_dir, e1, e2, etas, 0.01)
+    assert (status == 0).all(), status
+    assert (n1 == 1025).all(), n1
+    ref = np.array([TO.singularvalue_calc(CS.astype(np.complex64), tau, fd, e, e1, e, e2, 0.01)
+                    for e in etas])
     assert (np.abs(sv - ref) / ref).max() < 1e-5, (sv, ref)
 
 
