@@ -55,15 +55,17 @@ __global__ void spline_eval_kernel(const float* __restrict__ dyn, const float* _
                                    const float4* __restrict__ W, int nlam,
                                    float* __restrict__ out) {
     const int t = blockIdx.x * blockDim.x + threadIdx.x;
-    const int k = blockIdx.y;
-    if (t >= nt || k >= nlam) return;
-    const int i = idx[k];
-    const float4 w = W[k];
-    const size_t r0 = (size_t)(flip ? nf - 1 - i : i) * nt + t;
-    const size_t r1 = (size_t)(flip ? nf - 2 - i : i + 1) * nt + t;
-    const float v = w.x * dyn[r0] + w.y * dyn[r1] + w.z * M[(size_t)i * nt + t] +
-                    w.w * M[(size_t)(i + 1) * nt + t];
-    out[(size_t)(nlam - 1 - k) * nt + t] = v;     // np.flipud: wavelength ascending
+    if (t >= nt) return;
+    // rows k = blockIdx.y + m gridDim.y: gridDim.y is capped at 65535, nlam is not
+    for (int k = blockIdx.y; k < nlam; k += gridDim.y) {
+        const int i = idx[k];
+        const float4 w = W[k];
+        const size_t r0 = (size_t)(flip ? nf - 1 - i : i) * nt + t;
+        const size_t r1 = (size_t)(flip ? nf - 2 - i : i + 1) * nt + t;
+        const float v = w.x * dyn[r0] + w.y * dyn[r1] + w.z * M[(size_t)i * nt + t] +
+                        w.w * M[(size_t)(i + 1) * nt + t];
+        out[(size_t)(nlam - 1 - k) * nt + t] = v;     // np.flipud: wavelength ascending
+    }
 }
 
 #ifndef SB_HOST_EMU
@@ -79,7 +81,7 @@ int scale_dyn_lambda(const float* dyn, int nf, int nt, int flip, const float* a,
     spline_moments_kernel<<<(nt + 127) / 128, 128, 0, st>>>(dyn, nf, nt, flip, a, cp, inv, g, p0,
                                                            pn, M);
     SB_LAUNCH_CHECK();
-    dim3 grid((nt + 255) / 256, nlam);
+    dim3 grid((nt + 255) / 256, nlam < 65535 ? nlam : 65535);
     spline_eval_kernel<<<grid, 256, 0, st>>>(dyn, M, nf, nt, flip, idx, W, nlam, out);
     SB_LAUNCH_CHECK();
     return SB_OK;

@@ -348,9 +348,11 @@ int thin_sweep(const ThinGeom& t, const double* d_eta1, const double* d_eta2, in
     thin_prep_kernel<<<neta, 32, 0, st>>>(t, d_eta1, d_eta2, neta, ld1, ld2, d_idx1, d_idx2,
                                           d_n1, d_n2);
     SB_LAUNCH_CHECK();
-    {
-        dim3 grid(64, neta);
-        thin_indexerr_kernel<<<grid, 256, 0, st>>>(t, d_eta1, d_eta2, d_status);
+    // one pair per gridDim.y row, which CUDA caps at 65535: launches of at most 65535
+    for (int e0 = 0; e0 < neta; e0 += 65535) {
+        const int nb = neta - e0 < 65535 ? neta - e0 : 65535;
+        thin_indexerr_kernel<<<dim3(64, nb), 256, 0, st>>>(t, d_eta1 + e0, d_eta2 + e0,
+                                                           d_status + e0);
         SB_LAUNCH_CHECK();
     }
     const size_t per = (size_t)ld1 * ld2 * sizeof(float2);

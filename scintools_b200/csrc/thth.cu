@@ -803,9 +803,11 @@ int thth_prep(const ThthGeom& g, const double* th_host, const double* d_etas, in
     thth_prep_kernel<<<neta, 32, 0, st>>>(g, d_etas, neta, ld, d_idx, d_nred);
     prof_end(PROF_THTH_PREP, st);
     SB_LAUNCH_CHECK();
-    if (lower_check_needed(g, th_host)) {
-        dim3 grid(64, neta);
-        thth_indexerr_kernel<<<grid, 256, 0, st>>>(g, d_etas, d_status);
+    // one curvature per gridDim.y row, which CUDA caps at 65535: launches of at most 65535
+    const bool check = lower_check_needed(g, th_host);
+    for (int e0 = 0; check && e0 < neta; e0 += 65535) {
+        const int nb = neta - e0 < 65535 ? neta - e0 : 65535;
+        thth_indexerr_kernel<<<dim3(64, nb), 256, 0, st>>>(g, d_etas + e0, d_status + e0);
         SB_LAUNCH_CHECK();
     }
     return SB_OK;
