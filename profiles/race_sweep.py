@@ -1,4 +1,4 @@
-"""Small eta sweep through the three eigen solvers (tensor-core default, packed-FMA, fp32):
+"""Small eta sweep through the two eigen solvers (tensor-core default, fp32):
 run under `compute-sanitizer --tool racecheck|memcheck`."""
 import os
 import sys
@@ -13,7 +13,5 @@ fd = thth.fft_axis(t, "mHz", npad); tau = thth.fft_axis(f, "us", npad)
 edges = np.linspace(-20, 20, 96); etas = np.linspace(0.002, 0.02, 4)
 cs = thth.conjugate_spectrum(d0, npad, 0.0)
 print("tensor-core", thth.eta_sweep(cs, tau, fd, etas, edges))
-os.environ["SB_EIG_NO_TC"] = "1"
-print("packed-FMA ", thth.eta_sweep(cs, tau, fd, etas, edges))
 os.environ["SB_EIG_FP32"] = "1"
 print("fp32       ", thth.eta_sweep(cs, tau, fd, etas, edges))

@@ -2,27 +2,20 @@
 // (ththmod.Eval_calc, scintools/ththmod.py:371-401): the DEFAULT solver of
 // sb::eta_sweep for ld <= 512.
 //
-// Why: the fp32 streaming solver (thth_eig_kernel, thth.cu) re-reads the 1 MB
-// fp32 triangle on every Lanczos step (19.3 GB per 1024-eta sweep) and spends
-// ~32 thread-instructions per matrix element (masks, shared-memory loads of
-// the vector, per-row reductions, one-lane bulk-copy bookkeeping).  This kernel
-//   * iterates on an fp16 copy of the triangle (re | im << 16, 4 B per complex
-//     element: half the bytes) written by thth_build_kernel<true>, scaled per
-//     curvature by a power of two so that the largest element stays below 2^15
-//     (the scale cancels: only the Ritz VECTOR of this phase is used).  A bf16
-//     copy was measured first: its 8-bit mantissa leaves a residual
-//     ||A y - rho y|| / rho of 0.6e-3 .. 3e-3 and Rayleigh-quotient errors up to
-//     1.1e-5 on the 4096x8192 workload -- fp16's 11 bits give 8x / 64x less;
-//   * keeps the lane's 16 vector elements and 16 column accumulators in
-//     registers for the whole mat-vec and does the complex multiply-adds as
-//     fp32 FMAs: one LDS.128 + 8 converts + 32 FFMA per four complex elements;
-//     no masks except on the diagonal group;
-//   * fetches the rows with per-lane cp.async copies (every lane copies exactly
-//     the 16-byte chunks it reads itself: a wait_group is all the synchronisation
-//     a stage needs), two adjacent rows per stage, and reduces their four row
-//     sums with six shuffles;
-//   * runs the convergence check of step m on warp 0 DURING mat-vec m+1 (warp 0
-//     gets half the rows), so nobody idles behind the Sturm sweeps;
+// Why: the fp32 solver (thth_eig_kernel, thth.cu) re-reads the 1 MB fp32
+// triangle on every Lanczos step (19.3 GB per 1024-eta sweep) and spends ~16 FFMA
+// plus masks and shuffles per matrix element.  This kernel
+//   * iterates on an fp16 copy of the triangle (4 B per complex element: half the
+//     bytes) written by thth_build_kernel<2>, scaled per curvature by a power of two
+//     so that the largest element stays below 2^15 (the scale cancels: only the
+//     Ritz VECTOR of this phase is used).  A bf16 copy was measured first: its 8-bit
+//     mantissa leaves a residual ||A y - rho y|| / rho of 0.6e-3 .. 3e-3 and
+//     Rayleigh-quotient errors up to 1.1e-5 on the 4096x8192 workload -- fp16's
+//     11 bits give 8x / 64x less;
+//   * does the mat-vec on the tensor cores (mma.sync m16n8k16, fp16 x fp16 -> fp32,
+//     see matvec_t), fetching the blocks with per-lane cp.async copies;
+//   * runs the convergence check of step m on a ninth warp DURING mat-vec m+1, so
+//     nobody idles behind the Sturm sweeps;
 //   * keeps the Lanczos vectors (fp32) in global memory, forms the Ritz vector
 //     y and reports the Rayleigh quotient <y, A y> / <y, y> with the FP32
 //     triangle in one extra pass (second order in the vector error);
@@ -48,7 +41,7 @@ enum { EB_ST_INDEX_ERROR = 1, EB_ST_ZERO_START = 2, EB_ST_TOO_SMALL = 4,
 
 constexpr int EB_THREADS = 256;
 constexpr int EB_NW = EB_THREADS / 32;
-constexpr int EB_NST = 2;             // ring stages per warp, 4 KB each
+constexpr int EB_NST = 2;             // fp32 pass: ring stages per warp, 4 KB each
 #ifdef SB_EB_SLOTS
 constexpr int EB_SLOTS = SB_EB_SLOTS; // tests/host_emu: few slots to exercise the fp32 restart
 #else
@@ -81,8 +74,8 @@ __device__ __forceinline__ unsigned pack_h2(const float lo, const float hi) {
 #endif
 }
 
-// ---- tensor-core mat-vec (EB_MODE_TC) -------------------------------------
-// The fp16 copy is then stored in 512-byte BLOCKS of 16 rows x 8 complex columns
+// ---- tensor-core mat-vec ---------------------------------------------------
+// The fp16 copy is stored in 512-byte BLOCKS of 16 rows x 8 complex columns
 // (thth_build_kernel<2>): block (I, G) = rows 16 I .., columns 8 G .., at byte
 // ((I * ld / 8 + G) * 512); a block row is [re x 8 | im x 8] (planar, 32 bytes).
 // One block is one m16n8k16 A operand (k < 8: re, k >= 8: im of column k - 8)
@@ -161,59 +154,48 @@ __device__ __forceinline__ void mma16816(float (&d)[4], const unsigned (&a)[4], 
 }
 #endif
 
-enum { EB_MODE_BULK = 0, EB_MODE_CPA = 1, EB_MODE_TC = 2 };
-__host__ __device__ constexpr bool eb_is_tc(int mode) { return mode == EB_MODE_TC; }
-
 // shared-memory bytes of one CTA (host + device agree through this)
-// bytes of a warp's slice of the ring: two 4 KB row stages, or (tensor-core mat-vec)
-// EB_TC_NST 1 KB stages + the 4 KB column-sum buffer (the fp32 pass re-uses the first 8 KB)
-__host__ __device__ constexpr size_t eig_half_slice(int mode) {
-    return eb_is_tc(mode) ? (size_t)EB_TC_NST * 1024 + 4096 : (size_t)EB_NST * 4096;
+// bytes of a warp's slice of the ring: EB_TC_NST 1 KB stages + the 4 KB column-sum buffer
+// (the fp32 pass re-uses the first 8 KB as two 4 KB row stages)
+__host__ __device__ constexpr size_t eig_half_slice() {
+    return (size_t)EB_TC_NST * 1024 + 4096;
 }
-__host__ __device__ inline size_t eig_half_smem(int ld, int mode = EB_MODE_CPA) {
+__host__ __device__ inline size_t eig_half_smem(int ld) {
     return sizeof(LanczosShared) + 4 * (size_t)ld * sizeof(float2) +
-           (size_t)EB_NW * eig_half_slice(mode) + (size_t)EB_NW * EB_NST * 8 + 16 +
-           (eb_is_tc(mode) ? 4 * (size_t)(ld / 2) * 8 : 0);
+           (size_t)EB_NW * eig_half_slice() + (size_t)EB_NW * EB_NST * 8 + 16 +
+           4 * (size_t)(ld / 2) * 8;
 }
 
-// CPA: the bf16 rows are fetched with per-lane cp.async (LDGSTS) copies -- every lane
-// copies exactly the 16-byte chunks it will read itself, so a wait_group is all the
-// synchronisation a stage needs -- instead of cp.async.bulk + mbarrier (one lane issues,
-// ~70 instructions per row pair of address / election bookkeeping).
-// MODE = EB_MODE_TC: the mat-vec runs on the tensor cores (mma.sync m16n8k16, fp16 x fp16
-// -> fp32): see matvec_t below.
-// EB_MODE_TC runs one more warp (warp EB_NW): it only joins the barriers and runs the
-// deferred convergence checks, so the eight mat-vec warps carry equal shares in every step
-// (with the check on warp 0 that warp idled through half of every step without a check and
-// was the straggler of the steps with one, holding the others at the barrier that ends the
-// mat-vec).
-template <int MODE>
-__global__ void __launch_bounds__(eb_is_tc(MODE) ? EB_THREADS + 32 : EB_THREADS, 2)
+// One more warp than the mat-vec needs (warp EB_NW): it only joins the barriers and runs
+// the deferred convergence checks, so the eight mat-vec warps carry equal shares in every
+// step (with the check on warp 0 that warp idled through half of every step without a
+// check and was the straggler of the steps with one, holding the others at the barrier
+// that ends the mat-vec).
+__global__ void __launch_bounds__(EB_THREADS + 32, 2)
 thth_eig_half_kernel(const float2* __restrict__ Mbase, const unsigned* __restrict__ Mbbase,
                      int ld, const int* __restrict__ nred, int eta0,
                      double* __restrict__ eigs, int* __restrict__ status,
                      int* __restrict__ iters, double tol, double etol, double etol_h, double rtol_r,
                      int max_iter, float2* __restrict__ gbasis) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    constexpr bool CPA = MODE != EB_MODE_BULK;
     LanczosShared& S = *reinterpret_cast<LanczosShared*>(smem_raw);
     float2* v = reinterpret_cast<float2*>(smem_raw + sizeof(LanczosShared));
     float2* vp = v + ld;
     float2* w = vp + ld;          // row sums, then the new Lanczos vector
     float2* u = w + ld;           // column sums
-    unsigned char* ring = reinterpret_cast<unsigned char*>(u + ld);     // [NW][NST][4096]
+    unsigned char* ring = reinterpret_cast<unsigned char*>(u + ld);     // [NW][WSL]
     float2* part = reinterpret_cast<float2*>(ring);                      // [NW][512] scratch (aliases the ring)
-    constexpr int WSL = (int)eig_half_slice(MODE);                       // bytes per warp
+    constexpr int WSL = (int)eig_half_slice();                           // bytes per warp
     static_assert(WSL >= EB_NST * 4096, "the fp32 pass needs two 4 KB stages per warp");
     unsigned long long* mbar = reinterpret_cast<unsigned long long*>(ring + (size_t)EB_NW * WSL);
-    // EB_MODE_TC: fp16 operand forms of the vector, [4 variants][ld / 2] x {b0, b1}
+    // fp16 operand forms of the vector, [4 variants][ld / 2] x {b0, b1}
     uint2* P = reinterpret_cast<uint2*>(reinterpret_cast<unsigned char*>(mbar) +
                                         (size_t)EB_NW * EB_NST * 8 + 16);
     const int tid = threadIdx.x, lane = tid & 31;
     // warp index through a shuffle: tells the compiler it is warp-uniform, so the
     // bulk-copy addresses below live in uniform registers (no per-lane election loops)
     const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
-    constexpr int CHKW = eb_is_tc(MODE) ? EB_NW : 0;      // the warp that runs the deferred checks
+    constexpr int CHKW = EB_NW;                              // the warp that runs the deferred checks
     const bool worker = warp < EB_NW;
     const int tidw = worker ? tid : (1 << 24);               // strided loops: worker threads only
     const int e = blockIdx.x;
@@ -245,197 +227,12 @@ thth_eig_half_kernel(const float2* __restrict__ Mbase, const unsigned* __restric
     fence_proxy_async();
     __syncthreads();
     const int ncol4 = (n + 1) >> 1;            // fp32 rows: float4 groups = two complex columns
-    const int ncolq = ((n + 3) >> 2) << 2;     // fp16 rows are fetched in multiples of 4 columns
     unsigned char* mystage = ring + (size_t)warp * WSL;
     unsigned long long* mybar = mbar + EB_NST * warp;
     unsigned phbits = 0;                       // bit s: phase parity of this warp's barrier s
 
     // ------------------------------------------------------------------
-    // fp16 mat-vec: w = (strict upper triangle) v row sums, u = column sums.
-    // Warp `warp` owns the row pairs p = warp + NW k, rows (2p, 2p+1); a lane
-    // owns the columns 4 (lane + 32 j) + i, j < 4, i < 4, of every row.
-    // ------------------------------------------------------------------
-    // Row pairs are dealt in a pattern of 15: warp 0 takes 1, warps 1..7 take 2, because
-    // warp 0 also runs the (deferred) convergence check of the previous step while
-    // the others are already in this mat-vec (check_m > 0).
-    auto pair_of = [&](int k) -> int {
-        return warp == 0 ? 7 + 15 * k : 15 * (k >> 1) + ((k & 1) ? warp + 7 : warp - 1);
-    };
-    auto matvec_b = [&](int check_m, double et) {
-        for (int c = tidw; c < ld; c += EB_THREADS) w[c] = make_float2(0.f, 0.f);
-        float2 X[4][4];                        // v at the lane's columns
-        float2 yc[4][4];                       // column accumulators
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const int c0 = 4 * (lane + 32 * j);
-            float4 a = make_float4(0.f, 0.f, 0.f, 0.f), b = a;
-            if (c0 < ld) {
-                a = *reinterpret_cast<const float4*>(v + c0);
-                b = *reinterpret_cast<const float4*>(v + c0 + 2);
-            }
-            X[j][0] = make_float2(a.x, a.y); X[j][1] = make_float2(a.z, a.w);
-            X[j][2] = make_float2(b.x, b.y); X[j][3] = make_float2(b.z, b.w);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) yc[j][i] = make_float2(0.f, 0.f);
-        }
-        __syncthreads();
-        const int npair = n >> 1;              // rows 0 .. n-2  ->  pairs 0 .. (n-2)/2
-        int K;
-        if (warp == 0) K = npair > 7 ? (npair - 8) / 15 + 1 : 0;
-        else K = (npair > warp - 1 ? (npair - warp) / 15 + 1 : 0) +
-                 (npair > warp + 7 ? (npair - 8 - warp) / 15 + 1 : 0);
-        auto issue = [&](int k) {          // cp.async.bulk: one lane, two copies on one barrier
-            const int a0 = 2 * pair_of(k);
-            const int c0 = a0 & ~3;            // = (a0 + 1) & ~3 for even a0
-            const int c1 = (a0 + 2) & ~3;
-            const unsigned b0 = (unsigned)(ncolq - c0) * 4u;
-            const bool has1 = a0 + 1 <= n - 2;
-            const unsigned b1 = has1 ? (unsigned)(ncolq - c1) * 4u : 0u;
-            unsigned char* dst = mystage + (k % EB_NST) * 4096;
-            const unsigned* src = Mb + (unsigned)(a0 * ld);
-            mbar_expect_tx(mybar + k % EB_NST, b0 + b1);
-            bulk_g2s(dst + c0 * 4, src + c0, b0, mybar + k % EB_NST);
-            if (has1) bulk_g2s(dst + 2048 + c1 * 4, src + ld + c1, b1, mybar + k % EB_NST);
-        };
-        // cp.async: every lane copies its own chunks.  gsrc / sdst are per-lane bases kept
-        // in registers (the empty asm stops the compiler from re-deriving them from
-        // blockIdx every time); per pair only a0 * ld and the two diagonal compares remain.
-        const unsigned* gsrc = Mb + 4 * lane;
-        smem_addr sdst = smem_addr_of(mystage) + lane * 16;
-#ifndef SB_HOST_EMU
-        asm volatile("" : "+l"(gsrc), "+r"(sdst));
-#endif
-        const int cb0 = 4 * lane + 3;      // last column of the lane's chunk in group 0
-        auto fetch = [&](int k) {
-            if (k < K) {
-                const int a0 = 2 * pair_of(k);
-                const int JS = (a0 + 1) >> 7;
-                const unsigned* src = gsrc + (unsigned)(a0 * ld);
-                const smem_addr dst = sdst + (k % EB_NST) * 4096;
-                const int lim1 = (a0 + 1 <= n - 2) ? a0 + 2 : 0x7fffffff;   // row 1 absent: never
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    if (j < JS) continue;
-                    const int cend = cb0 + 128 * j;
-                    if (cend - 3 < ncolq) {
-                        if (cend >= a0 + 1) cp_async16_s(dst + j * 512, src + j * 128);
-                        if (cend >= lim1) cp_async16_s(dst + 2048 + j * 512, src + ld + j * 128);
-                    }
-                }
-            }
-            cp_async_commit();             // (an empty group keeps the wait count uniform)
-        };
-        if (CPA) {
-            for (int k = 0; k < EB_NST; ++k) fetch(k);
-        } else if (lane == 0) {
-            for (int k = 0; k < EB_NST && k < K; ++k) issue(k);
-        }
-        if (check_m > 0 && warp == 0) lanczos_check(S, check_m, tol, et);
-        float* wflat = reinterpret_cast<float*>(w);
-        for (int k = 0; k < K; ++k) {
-            const int a0 = 2 * pair_of(k);
-            const bool has1 = a0 + 1 <= n - 2;
-            float4 xa = *reinterpret_cast<const float4*>(v + a0);     // v[a0], v[a0 + 1]
-            if (!has1) { xa.z = 0.f; xa.w = 0.f; }
-            // column part: yc += conj(A[a][c]) v[a] = (xa.x, xa.y) q.re + (xa.y, -xa.x) q.im
-            const float2 XA0 = make_float2(xa.x, xa.y), XB0 = make_float2(xa.y, -xa.x);
-            const float2 XA1 = make_float2(xa.z, xa.w), XB1 = make_float2(xa.w, -xa.z);
-            const int st = k % EB_NST;
-            if (CPA) {
-                cp_async_wait<EB_NST - 1>();    // this lane's copies of pair k have landed
-            } else {
-                while (!mbar_try_wait(mybar + st, (phbits >> st) & 1u)) {}
-                phbits ^= 1u << st;
-            }
-            const uint4* s0 = reinterpret_cast<const uint4*>(mystage + st * 4096);
-            const uint4* s1 = s0 + 128;
-            const int JS = (a0 + 1) >> 7;       // column groups entirely left of the diagonal
-            // row part: sum += (v.re, v.im) q.re + (-v.im, v.re) q.im  (scalar q operands:
-            // the packed word needs no pairing, only one shift for q.re)
-            float2 S0a = make_float2(0.f, 0.f), S0b = S0a, S1a = S0a, S1b = S0a;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                if (j < JS) continue;           // warp-uniform
-                const int c16 = lane + 32 * j;
-                uint4 q0 = s0[c16], q1 = s1[c16];
-                if (j == JS) {                  // the group the diagonal crosses
-                    const int rel0 = a0 + 1 - 4 * c16, rel1 = rel0 + 1;
-                    if (rel0 > 0) q0.x = 0u;
-                    if (rel0 > 1) q0.y = 0u;
-                    if (rel0 > 2) q0.z = 0u;
-                    if (rel0 > 3) q0.w = 0u;
-                    if (rel1 > 0) q1.x = 0u;
-                    if (rel1 > 1) q1.y = 0u;
-                    if (rel1 > 2) q1.z = 0u;
-                    if (rel1 > 3) q1.w = 0u;
-                }
-                const unsigned p0[4] = {q0.x, q0.y, q0.z, q0.w};
-                const unsigned p1[4] = {q1.x, q1.y, q1.z, q1.w};
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    const float2 x = X[j][i];
-                    const float2 xrot = make_float2(-x.y, x.x);
-                    const float2 Q0 = unpack_f16x2(p0[i]);
-                    ffma2(S0a, x, Q0.x);
-                    ffma2(S0b, xrot, Q0.y);
-                    ffma2(yc[j][i], XA0, Q0.x);
-                    ffma2(yc[j][i], XB0, Q0.y);
-                    const float2 Q1 = unpack_f16x2(p1[i]);
-                    ffma2(S1a, x, Q1.x);
-                    ffma2(S1b, xrot, Q1.y);
-                    ffma2(yc[j][i], XA1, Q1.x);
-                    ffma2(yc[j][i], XB1, Q1.y);
-                }
-            }
-            if (CPA) {
-                fetch(k + EB_NST);              // refill this lane's chunks of the stage
-            } else {
-                __syncwarp();                   // every lane is done reading the stage
-                if (lane == 0 && k + EB_NST < K) issue(k + EB_NST);
-            }
-            // four row sums (re0, im0, re1, im1) with six shuffles: lanes 0-15 keep
-            // row 0, lanes 16-31 row 1; then bit 3 splits re / im
-            const float r0x = S0a.x + S0b.x, r0y = S0a.y + S0b.y;
-            const float r1x = S1a.x + S1b.x, r1y = S1a.y + S1b.y;
-            const bool h16 = lane & 16;
-            float kx = h16 ? r1x : r0x, ky = h16 ? r1y : r0y;
-            kx += __shfl_xor_sync(0xffffffffu, h16 ? r0x : r1x, 16);
-            ky += __shfl_xor_sync(0xffffffffu, h16 ? r0y : r1y, 16);
-            const bool h8 = lane & 8;
-            float kk = h8 ? ky : kx;
-            kk += __shfl_xor_sync(0xffffffffu, h8 ? kx : ky, 8);
-            kk += __shfl_xor_sync(0xffffffffu, kk, 4);
-            kk += __shfl_xor_sync(0xffffffffu, kk, 2);
-            kk += __shfl_xor_sync(0xffffffffu, kk, 1);
-            // lanes 0 / 8 / 16 / 24 hold re0, im0, re1, im1 = 4 consecutive floats of w
-            if ((lane & 7) == 0 && (has1 || lane < 16)) wflat[2 * a0 + (lane >> 3)] = kk;
-        }
-        if (CPA) cp_async_wait<0>();            // (only empty groups are left)
-        __syncthreads();                        // every warp is done with its stages
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            float4* dst = reinterpret_cast<float4*>(part + warp * 512 + 4 * (lane + 32 * j));
-            dst[0] = make_float4(yc[j][0].x, yc[j][0].y, yc[j][1].x, yc[j][1].y);
-            dst[1] = make_float4(yc[j][2].x, yc[j][2].y, yc[j][3].x, yc[j][3].y);
-        }
-        __syncthreads();
-        for (int c = tidw; c < 512; c += EB_THREADS) {
-            float sx = 0.f, sy = 0.f;
-#pragma unroll
-            for (int kk = 0; kk < EB_NW; ++kk) { sx += part[kk * 512 + c].x; sy += part[kk * 512 + c].y; }
-            if (c < ld) u[c] = make_float2(sx, sy);
-        }
-        __syncthreads();
-        // the scratch aliased the ring: back to zeros (finite, harmless under a
-        // zero vector element), ordered before the next bulk copies (async proxy)
-        for (int i = tidw; i < EB_NW * 256; i += EB_THREADS)
-            reinterpret_cast<float4*>(ring)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-        fence_proxy_async();
-        __syncthreads();
-    };
-
-    // ------------------------------------------------------------------
-    // fp16 mat-vec on the TENSOR CORES (EB_MODE_TC).  The triangle is a set of
+    // fp16 mat-vec on the TENSOR CORES.  The triangle is a set of
     // 16-row x 8-column blocks (I, G), G >= 2 I; for every block
     //   rows:    D1[r][n] += sum_k A[r][k] B_G[k][n]     A = the block, k = (re | im) x column
     //   columns: D2[m][n]  = sum_r A[r][m] B_I[r][n]     A^T through ldmatrix.trans
@@ -688,15 +485,15 @@ thth_eig_half_kernel(const float2* __restrict__ Mbase, const unsigned* __restric
     };
 
     // ------------------------------------------------------------------
-    // Lanczos from the normalised vector in v (vp = 0).  BF: iterate on the
-    // bf16 triangle and keep the basis; returns false if the basis slots ran
+    // Lanczos from the normalised vector in v (vp = 0).  lanczos_b: iterate on
+    // the fp16 triangle and keep the basis; returns false if the basis slots ran
     // out.  S.done / S.theta / m describe the outcome.
     // ------------------------------------------------------------------
     int m = 0;
     int mv = 0;                                 // mat-vecs done (reported as iters)
     auto lanczos_init = [&]() {
         if (tid == 0) {
-            S.done = 0; S.lo = 0.0; S.theta = 0.0; S.res = 0.0; S.m_lo2 = 0; S.lo2 = 0.0;
+            S.done = 0; S.lo = 0.0; S.theta = 0.0; S.res = 0.0;
             S.next_check = 1; S.m_last = 0; S.beta2[0] = 0.0;
         }
         __syncthreads();
@@ -745,7 +542,7 @@ thth_eig_half_kernel(const float2* __restrict__ Mbase, const unsigned* __restric
     };
     // ------------------------------------------------------------------
     // fp16 Lanczos from the normalised vector in v (vp = 0), basis kept.  The
-    // convergence check of the tridiagonal T_it runs on warp 0 DURING mat-vec it
+    // convergence check of the tridiagonal T_it runs on warp CHKW DURING mat-vec it
     // (one step late), so nobody idles behind its Sturm sweeps; when it reports
     // convergence the step just taken is surplus and m = it.  Returns false if
     // the basis slots ran out.
@@ -758,8 +555,7 @@ thth_eig_half_kernel(const float2* __restrict__ Mbase, const unsigned* __restric
             if (it >= EB_SLOTS) return false;
             for (int c = tidw; c < ld; c += EB_THREADS) basis[(size_t)it * ld + c] = v[c];
             const bool chk = it >= 1 && it >= S.next_check;
-            if (eb_is_tc(MODE)) matvec_t(chk ? it : 0, et);
-            else matvec_b(chk ? it : 0, et);
+            matvec_t(chk ? it : 0, et);
             ++mv;
             double alpha, beta;
             step_scalars(it, beta_prev, alpha, beta);
@@ -913,7 +709,7 @@ thth_eig_half_kernel(const float2* __restrict__ Mbase, const unsigned* __restric
         ++mv;                                  // the fp32 Rayleigh-quotient pass
         plain = true;
     } else {
-        // iteration cap on the bf16 matrix: report what thth_eig_kernel would
+        // iteration cap on the fp16 matrix: report what thth_eig_kernel would
     }
     if (plain && tid == 0) {
         eigs[eta0 + e] = fabs(S.theta);
@@ -923,10 +719,10 @@ thth_eig_half_kernel(const float2* __restrict__ Mbase, const unsigned* __restric
 }
 
 #ifndef SB_HOST_EMU
-// d_Mb: the scaled fp16 copy of d_M written by thth_build_kernel<true>.
+// d_Mb: the scaled fp16 copy of d_M written by thth_build_kernel<2>.
 int eig_half_launch(const float2* d_M, const unsigned* d_Mb, int ld, const int* d_nred, int e0,
                     int nb, double* d_eigs, int* d_status, int* d_iters, double tol, double etol,
-                    int max_iter, bool tensor, cudaStream_t st) {
+                    int max_iter, cudaStream_t st) {
     float2* d_basis = (float2*)workspace(7, (size_t)nb * EB_SLOTS * ld * sizeof(float2));
     if (!d_basis) return SB_ERR_NOMEM;
     double rtol_r = 1e-3;
@@ -937,26 +733,14 @@ int eig_half_launch(const float2* d_M, const unsigned* d_Mb, int ld, const int* 
     // the same worst-case error against dense eigenvalues (3e-6)
     double etol_h = 1e-6;
     if (const char* ev = getenv("SB_EIG_ETOL_B")) etol_h = atof(ev);
-    static const bool bulk = getenv("SB_EIG_BULK") != nullptr;   // A/B: cp.async.bulk row fetch
-    const int mode = tensor ? EB_MODE_TC : (bulk ? EB_MODE_BULK : EB_MODE_CPA);
-    size_t smem = eig_half_smem(ld, mode);
-    // SB_EIG_SMEM_PAD=bytes: experiment switch -- extra dynamic shared memory so that only one
-    // CTA fits an SM (fewer 0.52 MB matrices in flight compete for the L2)
-    if (const char* ev = getenv("SB_EIG_SMEM_PAD")) smem += (size_t)atoi(ev);
-#define SB_EIG_HALF_LAUNCH(MODE)                                                                  \
-    do {                                                                                          \
-        SB_CUDA(cudaFuncSetAttribute(thth_eig_half_kernel<MODE>,                                  \
-                                     cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));    \
-        thth_eig_half_kernel<MODE><<<nb, eb_is_tc(MODE) ? EB_THREADS + 32 : EB_THREADS, smem, st>>>( \
-            d_M, d_Mb, ld, d_nred, e0, d_eigs, d_status, d_iters, tol, etol, etol_h, rtol_r,      \
-            max_iter, d_basis);                                                                   \
-    } while (0)
-    if (mode == EB_MODE_TC) SB_EIG_HALF_LAUNCH(EB_MODE_TC);
-    else if (mode == EB_MODE_BULK) SB_EIG_HALF_LAUNCH(EB_MODE_BULK);
-    else SB_EIG_HALF_LAUNCH(EB_MODE_CPA);
-#undef SB_EIG_HALF_LAUNCH
+    const size_t smem = eig_half_smem(ld);
+    SB_CUDA(cudaFuncSetAttribute(thth_eig_half_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)smem));
+    thth_eig_half_kernel<<<nb, EB_THREADS + 32, smem, st>>>(d_M, d_Mb, ld, d_nred, e0, d_eigs,
+                                                            d_status, d_iters, tol, etol, etol_h,
+                                                            rtol_r, max_iter, d_basis);
     SB_LAUNCH_CHECK();
-    return 1;
+    return SB_OK;
 }
 #endif  // SB_HOST_EMU
 

@@ -10,17 +10,20 @@ namespace sb {
 
 #define SB_LANCZOS_MAXIT 256
 
+// The reserved members are unused.  They keep the size the struct had when a second
+// check routine needed them: 2 KB less lets thin_sv_kernel (128 registers, 256 threads)
+// fit two CTAs per SM instead of one at 3008 .. 3072 theta1 columns, which is not measured.
 struct alignas(16) LanczosShared {
     double alpha[SB_LANCZOS_MAXIT];
     double beta[SB_LANCZOS_MAXIT + 1];
     double beta2[SB_LANCZOS_MAXIT + 1];
     double piv[SB_LANCZOS_MAXIT];
-    double sc2[SB_LANCZOS_MAXIT];   // lanczos_check_fast: scaled beta^2 (piv: scaled alpha)
+    double reserved0[SB_LANCZOS_MAXIT];
     double red[2][32];
     double theta, lo, res;
-    double lo2;              // lanczos_check_fast: lower bound of the 2nd Ritz value (m_lo2 > 0)
+    double reserved1;
     int done, next_check;
-    int m_lo2;
+    int reserved2;
     int m_last;              // lanczos_check: step of the previous check (0: none)
 };
 
@@ -178,174 +181,6 @@ __device__ inline void lanczos_check(LanczosShared& S, int m, double tol, double
         S.done = done ? 1 : 0;
         S.m_last = m;
         S.next_check = m + skip;
-    }
-}
-
-// ---------------------------------------------------------------------------
-// Latency-tuned variant used by the on-chip solver (eig_cluster.cu), where the
-// check runs on one warp concurrently with a mat-vec and must not outlast it.
-// Same stopping rule as lanczos_check, but
-//  * T is scaled by its Gershgorin radius once per check (S.piv / S.sc2), so
-//    the Sturm recurrence is 3 FP64 ops per step with a range check every 8;
-//  * the bracket starts from the previous step: theta_m >= theta_{m-1}
-//    (interlacing) and, once converging, theta_m <= theta_{m-1} + res_{m-1},
-//    verified by the count itself;
-//  * multisection only narrows the bracket to 1e-3; the top root is then
-//    polished by Newton's method on p_m from above (monotone, quadratic), whose
-//    last evaluation also yields |s_m|^2 = -p_{m-1}(theta) / p_m'(theta);
-//  * the second Ritz value is bracketed from its previous lower bound and only
-//    to a few percent of the gap.
-// Init: S.lo = S.theta = S.res = 0, S.m_lo2 = 0, S.next_check = 1, S.done = 0.
-// ---------------------------------------------------------------------------
-__device__ __forceinline__ int sturm_count_scaled(const LanczosShared& S, int m, double x) {
-    double q0 = 1.0, q1 = S.piv[0] - x;
-    bool neg = !(q1 > 0.0);
-    int cnt = neg ? 1 : 0;
-    for (int i0 = 1; i0 < m; i0 += 8) {
-        const int i1 = min(m, i0 + 8);
-#pragma unroll 4
-        for (int i = i0; i < i1; ++i) {
-            const double q2 = fma(S.piv[i] - x, q1, -(S.sc2[i] * q0));
-            const bool neg2 = (q2 == 0.0) ? !neg : (q2 < 0.0);
-            cnt += (neg2 != neg);
-            neg = neg2;
-            q0 = q1;
-            q1 = q2;
-        }
-        // |a| <= 2, b2 <= 1 after scaling: at most 3^8 growth between checks
-        const double aq = fmax(fabs(q1), fabs(q0));
-        const double sc = aq > 1e100 ? 1e-100 : (aq < 1e-100 ? 1e100 : 1.0);
-        q0 *= sc;
-        q1 *= sc;
-    }
-    return cnt;
-}
-
-// one multisection round over per-lane abscissae (ascending in lane, scaled units)
-__device__ __forceinline__ void sturm_round(const LanczosShared& S, int m, int want, double x,
-                                            double& lo, double& hi) {
-    const int cnt = sturm_count_scaled(S, m, x);
-    const unsigned ok = __ballot_sync(0xffffffffu, cnt >= want);
-    const int f = ok ? __ffs(ok) - 1 : 32;
-    const double nhi = f < 32 ? __shfl_sync(0xffffffffu, x, f & 31) : hi;
-    const double nlo = f > 0 ? __shfl_sync(0xffffffffu, x, (f - 1) & 31) : lo;
-    hi = nhi;
-    lo = nlo;
-}
-
-__device__ inline void lanczos_check_fast(LanczosShared& S, int m, double tol, double etol) {
-    const int lane = threadIdx.x & 31;
-    __syncwarp();
-    const double bnew = S.beta[m];
-    double gh = -DBL_MAX, gl = DBL_MAX;
-    for (int i = lane; i < m; i += 32) {
-        const double b0 = i > 0 ? fabs(S.beta[i]) : 0.0;
-        const double b1 = i + 1 < m ? fabs(S.beta[i + 1]) : 0.0;
-        gh = fmax(gh, S.alpha[i] + b0 + b1);
-        gl = fmin(gl, S.alpha[i] - b0 - b1);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        gh = fmax(gh, __shfl_xor_sync(0xffffffffu, gh, o));
-        gl = fmin(gl, __shfl_xor_sync(0xffffffffu, gl, o));
-    }
-    double scale = fmax(fabs(gh), fabs(gl));
-    if (!(scale > 0.0) || !isfinite(scale)) scale = 1.0;
-    const double inv = 1.0 / scale, inv2 = inv * inv;
-    for (int i = lane; i < m; i += 32) {
-        S.piv[i] = S.alpha[i] * inv;
-        S.sc2[i] = S.beta2[i] * inv2;
-    }
-    __syncwarp();
-    // everything below in scaled units x = sigma / scale, |x| <= 1 + 1e-9
-    double hi = (gh + 1e-9 * fabs(gh) + 1e-290) * inv + 1e-15;
-    double lo = (m == 1) ? S.piv[0] - fabs(S.piv[0]) * 1e-9 - 1e-15 : S.lo * inv - 1e-15;
-    if (lo > hi) lo = hi - 2.5;
-    const double f33 = (double)(lane + 1) * (1.0 / 33.0);
-    // first round: dense inside [lo, theta_prev + res_prev], last lane on the
-    // Gershgorin bound (catches a top Ritz value that moved further)
-    if (m > 1 && S.res > 0.0) {
-        const double h2 = (S.theta + 1.0001 * S.res) * inv + 1e-12;
-        if (h2 > lo && h2 < hi) {
-            const double x = lane < 31 ? lo + (h2 - lo) * ((double)(lane + 1) * (1.0 / 31.0)) : hi;
-            sturm_round(S, m, m, x, lo, hi);
-        }
-    }
-    for (int round = 0; round < 4 && (hi - lo) > 1e-3; ++round)
-        sturm_round(S, m, m, lo + (hi - lo) * f33, lo, hi);
-    // Newton from above on p_m(x) = det(T - x): x <- x - p/p' decreases
-    // monotonically to the largest root.  p, p' by the three-term recurrence.
-    double x = hi, pm1 = 1.0, dm = -1.0;
-    bool polished = false;
-    for (int it = 0; it < 6; ++it) {
-        double p0 = 1.0, p1 = S.piv[0] - x, d0 = 0.0, d1 = -1.0;
-        for (int i = 1; i < m; ++i) {
-            const double a = S.piv[i] - x, b2 = S.sc2[i];
-            const double p2 = fma(a, p1, -(b2 * p0));
-            const double d2 = fma(a, d1, -fma(b2, d0, p1));
-            p0 = p1; p1 = p2; d0 = d1; d1 = d2;
-            if ((i & 7) == 0) {
-                const double aq = fmax(fmax(fabs(p1), fabs(p0)), fmax(fabs(d1), fabs(d0)));
-                const double sc = aq > 1e100 ? 1e-100 : (aq < 1e-100 ? 1e100 : 1.0);
-                p0 *= sc; p1 *= sc; d0 *= sc; d1 *= sc;
-            }
-        }
-        pm1 = p0;     // p_{m-1}(x)  (m == 1: 1)
-        dm = d1;      // p_m'(x)
-        const double step = (d1 != 0.0) ? p1 / d1 : 0.0;
-        if (!(step >= 0.0) || !(x - step >= lo)) break;   // left the bracket: not trusted
-        x -= step;
-        if (step <= 1e-11) { polished = true; break; }
-    }
-    if (!polished) {
-        // (near-)multiple top root or rounding trouble: finish by multisection
-        hi = fmin(hi, fmax(x, lo));
-        for (int round = 0; round < 8 && (hi - lo) > 1e-10; ++round)
-            sturm_round(S, m, m, lo + (hi - lo) * f33, lo, hi);
-        x = hi;
-        double p0 = 1.0, p1 = S.piv[0] - x, d0 = 0.0, d1 = -1.0;
-        for (int i = 1; i < m; ++i) {
-            const double a = S.piv[i] - x, b2 = S.sc2[i];
-            const double p2 = fma(a, p1, -(b2 * p0));
-            const double d2 = fma(a, d1, -fma(b2, d0, p1));
-            p0 = p1; p1 = p2; d0 = d1; d1 = d2;
-            if ((i & 7) == 0) {
-                const double aq = fmax(fmax(fabs(p1), fabs(p0)), fmax(fabs(d1), fabs(d0)));
-                const double sc = aq > 1e100 ? 1e-100 : (aq < 1e-100 ? 1e100 : 1.0);
-                p0 *= sc; p1 *= sc; d0 *= sc; d1 *= sc;
-            }
-        }
-        pm1 = p0;
-        dm = d1;
-    }
-    const double theta = x * scale;
-    // residual beta_{m+1} |s_m|, s_m^2 = -p_{m-1}(theta) / p_m'(theta)
-    const double s2 = (dm != 0.0) ? fabs(pm1 / dm) : 1.0;
-    const double res = bnew * sqrt(fmin(s2, 1.0));
-    bool done = (res <= tol * fabs(theta)) || !(bnew > 1e-30 * fabs(theta));
-    double lo2 = 0.0;
-    int m_lo2 = 0;
-    if (!done && m >= 3 && res <= 3e-2 * fabs(theta)) {
-        // theta2 of T_m: >= theta2 of T_{m'} for m' < m (interlacing)
-        lo2 = S.m_lo2 > 0 ? S.lo2 * inv - 1e-15 : (gl - 1e-9 * fabs(gl) - 1e-290) * inv - 1e-15;
-        double hi2 = x;
-        if (lo2 > hi2) lo2 = hi2 - 2.5;
-        for (int round = 0; round < 4; ++round) {
-            sturm_round(S, m, m - 1, lo2 + (hi2 - lo2) * f33, lo2, hi2);
-            if ((hi2 - lo2) <= 0.02 * (x - hi2)) break;
-        }
-        const double gap = (x - hi2) * scale;
-        done = gap > 0.0 && res * res <= etol * fabs(theta) * gap;
-        m_lo2 = m;
-    }
-    __syncwarp();
-    if (lane == 0) {
-        S.theta = theta;
-        S.lo = lo * scale;
-        S.res = res;
-        S.done = done ? 1 : 0;
-        if (m_lo2) { S.lo2 = lo2 * scale; S.m_lo2 = m_lo2; }
-        S.next_check = m + ((res > 0.3 * fabs(theta)) ? 2 : 1);
     }
 }
 

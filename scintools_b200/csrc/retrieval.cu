@@ -295,7 +295,6 @@ __device__ void herm_eigvec_body(Mat A, int n, float2* __restrict__ Q, int max_i
     }
     if (tid == 0) {
         S.done = 0; S.lo = 0.0; S.theta = 0.0; S.res = 0.0; S.next_check = 1; S.m_last = 0; S.beta2[0] = 0.0;
-        S.m_lo2 = 0; S.lo2 = 0.0;
     }
     double nrm2 = ev_block_sum(p0, red);
     const bool fallback = zero_start_fallback && nrm2 == 0.0 && n >= 2;

@@ -11,26 +11,16 @@
 #include <math.h>
 #include <stdlib.h>
 
-#include <type_traits>
-
-#include "bf16_pack.cuh"
 #include "lanczos.cuh"
 #include "thth.cuh"
-#include "tma.cuh"
 
 namespace sb {
 
 #ifndef SB_HOST_EMU
-// eig_cluster.cu: on-chip (cluster shared memory) solver for ld <= 512
-int eig_cluster_launch(const float2* d_M, int ld, int n_max, const int* d_nred, int e0,
-                       int nb, double* d_eigs, int* d_status, int* d_iters, double tol,
-                       double etol, int max_iter, cudaStream_t st);
-
-// eig_half.cu: bf16 iteration + fp32 Rayleigh quotient (default for ld <= 512)
+// eig_half.cu: fp16 iteration + fp32 Rayleigh quotient (default for ld <= 512)
 int eig_half_launch(const float2* d_M, const unsigned* d_Mb, int ld, const int* d_nred, int e0,
                     int nb, double* d_eigs, int* d_status, int* d_iters, double tol, double etol,
-                    int max_iter, bool tensor, cudaStream_t st);
-
+                    int max_iter, cudaStream_t st);
 #endif  // SB_HOST_EMU
 
 // status codes per eta (also in include/scint_b200.h)
@@ -160,7 +150,7 @@ __global__ void cs_absmax_kernel(const float2* __restrict__ cs, long long rows, 
     if ((threadIdx.x & 31) == 0) atomicMax(out, __float_as_uint(m));
 }
 
-// PACK: also write the fp16 copy Mb (re | im << 16) that eig_half.cu iterates on,
+// PACK == 2: also write the fp16 copy Mb that eig_half.cu iterates on,
 // scaled by the power of two that puts absmax * max Jacobian of this curvature just
 // below 2^15 (absmax: device scalar from cs_absmax_kernel, span: max |theta2 - theta1|).
 //
@@ -172,23 +162,24 @@ __global__ void cs_absmax_kernel(const float2* __restrict__ cs, long long rows, 
 // the same order as thth_point, so the bins stay bit-exact), one gather and the
 // Jacobian remain.  The cached pair is re-derived whenever the crop of the next
 // curvature moves the pair (idx differs).
-// ROWS rows of the tile per thread (block = 32 x 32/ROWS threads).  Per curvature the
+// ROWS = 4 rows of the tile per thread (block = 32 x 8 threads).  Per curvature the
 // body runs in three phases -- (1) tau_inv and the CS offset of every row, (2) ALL the
 // gathers back to back, (3) Jacobian, clean-up, stores -- so that ROWS independent
 // L2 / DRAM gathers are in flight per thread: the kernel is bound by the latency of
 // these random 8-byte loads (long-scoreboard stalls dominate with one load in flight),
 // not by its instruction count.
-// PACK == 2: the fp16 copy in the block layout of eig_half.cu's tensor-core mat-vec:
-// 512-byte blocks of 16 rows x 8 columns, block (I, G) at ((I * ld / 8 + G) * 512) bytes,
-// a block row = [re x 8 | im x 8] (the halves swapped in rows 4-7, 12-15); the part of a
-// diagonal block on / below the diagonal is written as zeros (the MMA has no masks).
-// ROWS == 4: three CTAs per SM (80 registers).  ptxas still spills at 80 registers, but
+// PACK == 0: the fp32 triangle only.  PACK == 2: also the fp16 copy in the block layout
+// of eig_half.cu's tensor-core mat-vec: 512-byte blocks of 16 rows x 8 columns, block
+// (I, G) at ((I * ld / 8 + G) * 512) bytes, a block row = [re x 8 | im x 8] (the halves
+// swapped in rows 4-7, 12-15); the part of a diagonal block on / below the diagonal is
+// written as zeros (the MMA has no masks).
+// Three CTAs per SM (80 registers).  ptxas still spills at 80 registers, but
 // less: 40-48 bytes of stores and 56-68 bytes of loads per thread in the PACK == 2
 // instances on sm_90, against ~200 / ~150 bytes at four CTAs (64 registers), where the
 // gather runs ~15 % slower on the headline sweep (H100 SXM, 400 W power limit: 2.8-2.9 ms
 // instead of 2.4 ms per 1024-eta launch).
-template <int PACK, int ROWS, typename OFF>
-__global__ void __launch_bounds__(32 * (32 / ROWS), ROWS == 8 ? 5 : 3)
+template <int PACK, typename OFF>
+__global__ void __launch_bounds__(256, 3)
 thth_build_kernel(ThthGeom g, const double* __restrict__ etas, int eta0, int nbatch,
                   int ld, const int* __restrict__ idx,
                   const int* __restrict__ nred, float2* __restrict__ M,
@@ -197,7 +188,7 @@ thth_build_kernel(ThthGeom g, const double* __restrict__ etas, int eta0, int nba
     // same 32x32 tile for neighbouring curvatures, whose gathers fall on
     // the same / adjacent CS rows for small |theta1^2 - theta2^2| (L2 reuse)
     // pair index -> (ta <= tb)
-    constexpr int TY = 32 / ROWS;
+    constexpr int ROWS = 4, TY = 32 / ROWS;
     int p = blockIdx.y, ta = 0;
     const int T = ld / 32;
     while (p >= T - ta) { p -= T - ta; ++ta; }
@@ -332,7 +323,6 @@ thth_build_kernel(ThthGeom g, const double* __restrict__ etas, int eta0, int nba
                 }
                 const unsigned o = foff0 + (unsigned)k * frow;
                 Me[o] = v;
-                if (PACK == 1) Mb[(size_t)e * ld * ld + o] = pack_f16x2(make_float2(v.x * hscale, v.y * hscale));
             }
             if (PACK == 2) {
                 // block row of 8 columns = [re x 8 | im x 8] (32 bytes): the 8 lanes of a column
@@ -370,56 +360,38 @@ thth_build_kernel(ThthGeom g, const double* __restrict__ etas, int eta0, int nba
 //   A[a][b] * v[b]        to the row sum of a   (warp-shuffle reduction), and
 //   conj(A[a][b]) * v[a]  to a per-lane accumulator of column b,
 // so each element is read once per Lanczos step (half the traffic of a full
-// mat-vec).  TMA = true (ld <= 512): every row segment is fetched with one
-// cp.async.bulk into a per-warp ring of NST 4 KB shared-memory stages
-// (mbarrier complete_tx), so ~NST row fetches per warp are in flight while the
-// warp does FMAs.  TMA = false: direct 16-byte loads, any ld, columns in
-// chunks of 512.
-template <int THREADS, bool TMA, int NST, bool FAST = false>
-__global__ void __launch_bounds__(THREADS)
+// mat-vec).  Direct 16-byte loads, any ld <= 4096, columns in chunks of 512.
+constexpr int EIG_THREADS = 512;
+
+__global__ void __launch_bounds__(EIG_THREADS)
 thth_eig_kernel(const float2* __restrict__ Mbase, int ld,
                 const int* __restrict__ nred, int eta0,
                 double* __restrict__ eigs, int* __restrict__ status,
-                int* __restrict__ iters, double tol, double etol, int max_iter, int nb) {
+                int* __restrict__ iters, double tol, double etol, int max_iter) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    constexpr int NW = THREADS / 32;
+    constexpr int THREADS = EIG_THREADS, NW = THREADS / 32;
     LanczosShared& S = *reinterpret_cast<LanczosShared*>(smem_raw);
     float2* v = reinterpret_cast<float2*>(smem_raw + sizeof(LanczosShared));
     float2* vp = v + ld;
     float2* w = vp + ld;          // row sums, then the new Lanczos vector
     float2* u = w + ld;           // column sums
-    // TMA: [NW][NST][256] float4 stages, re-used as the column-partial scratch
-    float4* stages = reinterpret_cast<float4*>(u + ld);
-    float2* part = reinterpret_cast<float2*>(stages);   // [NW][512]
-    unsigned long long* mbar = reinterpret_cast<unsigned long long*>(
-        reinterpret_cast<unsigned char*>(stages) +
-        (TMA ? (size_t)NW * NST * 4096 : (size_t)NW * 4096));
+    float2* part = u + ld;        // [NW][512] per-warp column partials
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (TMA) {
-        if (tid == 0) {
-            for (int i = 0; i < NW * NST; ++i) mbar_init(mbar + i, 1);
-            fence_mbarrier_init();
-        }
-    }
-    unsigned gi = 0, gc = 0;             // ring producer / consumer counters
-    // grid-stride over the curvatures: gridDim.x == nb (one CTA per eta) or a
-    // persistent grid sized so that the matrices in flight stay L2-resident
-    for (int e = blockIdx.x; e < nb; e += gridDim.x) {
-    __syncthreads();                     // the previous eta is done with the shared buffers
+    const int e = blockIdx.x;
     const int n = nred[eta0 + e];
     const float2* M = Mbase + (size_t)e * ld * ld;
     const double qnan = __longlong_as_double(0x7ff8000000000000LL);
 
     if (status[eta0 + e] & ST_INDEX_ERROR) {
         if (tid == 0) { eigs[eta0 + e] = qnan; iters[eta0 + e] = 0; }
-        continue;
+        return;
     }
     if (n < 3) {
         if (tid == 0) {
             eigs[eta0 + e] = qnan; iters[eta0 + e] = 0;
             status[eta0 + e] |= ST_TOO_SMALL;
         }
-        continue;
+        return;
     }
     // v0 = row n//2 of the Hermitian matrix (ththmod.py:398-399)
     const int h = n / 2;
@@ -435,7 +407,7 @@ thth_eig_kernel(const float2* __restrict__ Mbase, int ld,
     part0 = warp_sum(part0);
     if (lane == 0) S.red[0][warp] = part0;
     if (tid == 0) {
-        S.done = 0; S.lo = 0.0; S.theta = 0.0; S.res = 0.0; S.m_lo2 = 0; S.lo2 = 0.0;
+        S.done = 0; S.lo = 0.0; S.theta = 0.0; S.res = 0.0;
         S.next_check = 1; S.m_last = 0; S.beta2[0] = 0.0;
     }
     __syncthreads();
@@ -446,7 +418,7 @@ thth_eig_kernel(const float2* __restrict__ Mbase, int ld,
             eigs[eta0 + e] = qnan; iters[eta0 + e] = 0;
             status[eta0 + e] |= ST_ZERO_START;
         }
-        continue;
+        return;
     }
     {
         float s = (float)(1.0 / sqrt(nrm2));
@@ -455,120 +427,12 @@ thth_eig_kernel(const float2* __restrict__ Mbase, int ld,
     __syncthreads();
 
     const int ncol4 = (n + 1) >> 1;      // float4 = two complex columns
-    const int nchunk = (n + 511) / 512;  // column chunks of 512 (1 when TMA)
-    float4* mystage = stages + (size_t)warp * NST * 256;
-    unsigned long long* mybar = mbar + warp * NST;
+    const int nchunk = (n + 511) / 512;  // column chunks of 512
     float beta_prev = 0.f;
     int m = 0;
     for (int it = 0; it < max_iter; ++it) {
         for (int c = tid; c < ld; c += THREADS) w[c] = make_float2(0.f, 0.f);
         __syncthreads();
-        if constexpr (TMA) {
-            // ---- single column chunk (ld <= 512).  Rows are grouped by JS =
-            // number of 32-float4 column groups entirely left of the diagonal,
-            // and the row body is specialised on JS (no per-group branches,
-            // masks only on the boundary group); row sums use split
-            // accumulators and one 5-step shuffle tree for (re, im) together.
-            float4 yc[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) yc[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-            const int K = (n - 2 >= warp) ? (n - 2 - warp) / NW + 1 : 0;
-            const bool tail = ncol4 < 256;        // cropped matrix: mask the right edge too
-            const float4* v4 = reinterpret_cast<const float4*>(v);
-            // prologue: fill the ring
-            for (int k = 0; k < NST && k < K; ++k) {
-                const int st = gi % NST;
-                ++gi;
-                if (lane == 0) {
-                    const int a = warp + NW * k;
-                    const int c_lo = (a + 1) & ~1;
-                    const unsigned bytes = (unsigned)(2 * ncol4 - c_lo) * 8u;
-                    mbar_expect_tx(mybar + st, bytes);
-                    bulk_g2s(reinterpret_cast<float2*>(mystage + st * 256) + c_lo,
-                             M + (size_t)a * ld + c_lo, bytes, mybar + st);
-                }
-            }
-            int k = 0;
-            auto run_rows = [&](auto JSc) {
-                constexpr int JS = decltype(JSc)::value;
-                for (; k < K && ((warp + NW * k + 1) >> 6) == JS; ++k) {
-                    const int a = warp + NW * k;
-                    const int first4 = (a + 1) >> 1;
-                    const float2 xa = v[a];
-                    const int st = gc % NST;
-                    const unsigned par = (gc / NST) & 1u;
-                    ++gc;
-                    while (!mbar_try_wait(mybar + st, par)) {}
-                    const float4* sg = mystage + st * 256;
-                    float rxa = 0.f, rxb = 0.f, rya = 0.f, ryb = 0.f;
-#pragma unroll
-                    for (int j = JS; j < 8; ++j) {
-                        const int c4 = lane + 32 * j;
-                        float4 q = sg[c4];
-                        bool ok = (j > JS) || (c4 >= first4);
-                        if (tail) ok = ok && (c4 < ncol4);
-                        if (!ok) q = make_float4(0.f, 0.f, 0.f, 0.f);
-                        // only the live columns are read: past ld the float4 would alias w / the
-                        // other warps' stages (racecheck flags that even though it was discarded)
-                        float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
-                        if (ok) x = v4[c4];
-                        rxa = fmaf(q.x, x.x, rxa); rxb = fmaf(-q.y, x.y, rxb);
-                        rxa = fmaf(q.z, x.z, rxa); rxb = fmaf(-q.w, x.w, rxb);
-                        rya = fmaf(q.x, x.y, rya); ryb = fmaf(q.y, x.x, ryb);
-                        rya = fmaf(q.z, x.w, rya); ryb = fmaf(q.w, x.z, ryb);
-                        // conj(A) * v[a]
-                        yc[j].x = fmaf(q.x, xa.x, yc[j].x); yc[j].x = fmaf(q.y, xa.y, yc[j].x);
-                        yc[j].y = fmaf(q.x, xa.y, yc[j].y); yc[j].y = fmaf(-q.y, xa.x, yc[j].y);
-                        yc[j].z = fmaf(q.z, xa.x, yc[j].z); yc[j].z = fmaf(q.w, xa.y, yc[j].z);
-                        yc[j].w = fmaf(q.z, xa.y, yc[j].w); yc[j].w = fmaf(-q.w, xa.x, yc[j].w);
-                    }
-                    __syncwarp();
-                    const bool more = k + NST < K;
-                    const int st2 = gi % NST;   // == the stage just consumed
-                    if (more) ++gi;
-                    if (lane == 0 && more) {
-                        const int a2 = warp + NW * (k + NST);
-                        const int c_lo = (a2 + 1) & ~1;
-                        const unsigned bytes = (unsigned)(2 * ncol4 - c_lo) * 8u;
-                        mbar_expect_tx(mybar + st2, bytes);
-                        bulk_g2s(reinterpret_cast<float2*>(mystage + st2 * 256) + c_lo,
-                                 M + (size_t)a2 * ld + c_lo, bytes, mybar + st2);
-                    }
-                    // (re, im) reduced together: upper half-warp keeps im, lower re
-                    const float rx = rxa + rxb, ry = rya + ryb;
-                    const bool hi = lane & 16;
-                    float keep = hi ? ry : rx;
-                    keep += __shfl_xor_sync(0xffffffffu, hi ? rx : ry, 16);
-                    keep += __shfl_xor_sync(0xffffffffu, keep, 8);
-                    keep += __shfl_xor_sync(0xffffffffu, keep, 4);
-                    keep += __shfl_xor_sync(0xffffffffu, keep, 2);
-                    keep += __shfl_xor_sync(0xffffffffu, keep, 1);
-                    if (lane == 0) w[a].x += keep;
-                    if (lane == 16) w[a].y += keep;
-                }
-            };
-            run_rows(std::integral_constant<int, 0>{});
-            run_rows(std::integral_constant<int, 1>{});
-            run_rows(std::integral_constant<int, 2>{});
-            run_rows(std::integral_constant<int, 3>{});
-            run_rows(std::integral_constant<int, 4>{});
-            run_rows(std::integral_constant<int, 5>{});
-            run_rows(std::integral_constant<int, 6>{});
-            run_rows(std::integral_constant<int, 7>{});
-            __syncthreads();   // every warp is done with its stages
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-                *reinterpret_cast<float4*>(part + warp * 512 + 2 * (lane + 32 * j)) = yc[j];
-            __syncthreads();
-            for (int c = tid; c < 512; c += THREADS) {
-                float sx = 0.f, sy = 0.f;
-#pragma unroll
-                for (int kk = 0; kk < NW; ++kk) { sx += part[kk * 512 + c].x; sy += part[kk * 512 + c].y; }
-                if (c < ld) u[c] = make_float2(sx, sy);
-            }
-            fence_proxy_async();
-            __syncthreads();
-        } else {
         for (int cb = 0; cb < nchunk; ++cb) {
             float4 yc[8];
 #pragma unroll
@@ -576,47 +440,17 @@ thth_eig_kernel(const float2* __restrict__ Mbase, int ld,
             const int chunk_end = min(n, (cb + 1) * 512);
             // rows a = warp + NW*k with a + 1 < chunk_end
             const int K = (chunk_end - 2 >= warp) ? (chunk_end - 2 - warp) / NW + 1 : 0;
-            if (TMA) {
-                // prologue: fill the ring
-                for (int k = 0; k < NST && k < K; ++k) {
-                    const int st = gi % NST;
-                    ++gi;
-                    if (lane == 0) {
-                        const int a = warp + NW * k;
-                        const int c_lo = (a + 1) & ~1;
-                        const unsigned bytes = (unsigned)(2 * ncol4 - c_lo) * 8u;
-                        mbar_expect_tx(mybar + st, bytes);
-                        bulk_g2s(reinterpret_cast<float2*>(mystage + st * 256) + c_lo,
-                                 M + (size_t)a * ld + c_lo, bytes, mybar + st);
-                    }
-                }
-            }
             for (int k = 0; k < K; ++k) {
                 const int a = warp + NW * k;
                 const int first4 = (a + 1) >> 1;
                 const float2 xa = v[a];
                 float4 mm[8];
-                if (TMA) {
-                    const int st = gc % NST;
-                    const unsigned par = (gc / NST) & 1u;
-                    ++gc;
-                    while (!mbar_try_wait(mybar + st, par)) {}
-                    const float4* sg = mystage + st * 256;
-                    // lane-local group range [jlo, jhi) that lies inside [first4, ncol4)
-                    const int jlo = max(0, (first4 - lane + 31) >> 5);
-                    const int jhi = (ncol4 - lane + 31) >> 5;
+                const float4* row = reinterpret_cast<const float4*>(M + (size_t)a * ld);
 #pragma unroll
-                    for (int j = 0; j < 8; ++j)
-                        mm[j] = (j >= jlo && j < jhi) ? sg[lane + 32 * j]
-                                                      : make_float4(0.f, 0.f, 0.f, 0.f);
-                } else {
-                    const float4* row = reinterpret_cast<const float4*>(M + (size_t)a * ld);
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const int c4 = cb * 256 + lane + 32 * j;
-                        mm[j] = (c4 >= first4 && c4 < ncol4) ? __ldg(row + c4)
-                                                             : make_float4(0.f, 0.f, 0.f, 0.f);
-                    }
+                for (int j = 0; j < 8; ++j) {
+                    const int c4 = cb * 256 + lane + 32 * j;
+                    mm[j] = (c4 >= first4 && c4 < ncol4) ? __ldg(row + c4)
+                                                         : make_float4(0.f, 0.f, 0.f, 0.f);
                 }
                 float rx = 0.f, ry = 0.f;
                 const int jskip = (first4 - cb * 256) >> 5;   // groups entirely left of the diagonal
@@ -638,25 +472,10 @@ thth_eig_kernel(const float2* __restrict__ Mbase, int ld,
                     yc[j].z = fmaf(q.z, xa.x, yc[j].z); yc[j].z = fmaf(q.w, xa.y, yc[j].z);
                     yc[j].w = fmaf(q.z, xa.y, yc[j].w); yc[j].w = fmaf(-q.w, xa.x, yc[j].w);
                 }
-                if (TMA) {
-                    __syncwarp();
-                    const bool more = k + NST < K;
-                    const int st = gi % NST;   // == the stage just consumed
-                    if (more) ++gi;
-                    if (lane == 0 && more) {
-                        const int a2 = warp + NW * (k + NST);
-                        const int c_lo = (a2 + 1) & ~1;
-                        const unsigned bytes = (unsigned)(2 * ncol4 - c_lo) * 8u;
-                        mbar_expect_tx(mybar + st, bytes);
-                        bulk_g2s(reinterpret_cast<float2*>(mystage + st * 256) + c_lo,
-                                 M + (size_t)a2 * ld + c_lo, bytes, mybar + st);
-                    }
-                }
                 rx = warp_sum(rx);
                 ry = warp_sum(ry);
                 if (lane == 0) { w[a].x += rx; w[a].y += ry; }
             }
-            if (TMA) __syncthreads();   // every warp is done with its stages
 #pragma unroll
             for (int j = 0; j < 8; ++j)
                 *reinterpret_cast<float4*>(part + warp * 512 + 2 * (lane + 32 * j)) = yc[j];
@@ -667,9 +486,7 @@ thth_eig_kernel(const float2* __restrict__ Mbase, int ld,
                 for (int k = 0; k < NW; ++k) { sx += part[k * 512 + c].x; sy += part[k * 512 + c].y; }
                 if (cb * 512 + c < ld) u[cb * 512 + c] = make_float2(sx, sy);
             }
-            if (TMA) fence_proxy_async();
             __syncthreads();
-        }
         }
         // ---- alpha = Re <v, A v>
         double apart = 0.0;
@@ -705,10 +522,8 @@ thth_eig_kernel(const float2* __restrict__ Mbase, int ld,
         if (tid == 0) { S.alpha[it] = alpha; S.beta[m] = beta; S.beta2[m] = b2; }
         __syncthreads();
         const bool last = (it + 1 == max_iter);
-        if (warp == 0 && (m >= S.next_check || last || !(beta > 0.0))) {
-            if (FAST) lanczos_check_fast(S, m, tol, etol);
-            else lanczos_check(S, m, tol, etol);
-        }
+        if (warp == 0 && (m >= S.next_check || last || !(beta > 0.0)))
+            lanczos_check(S, m, tol, etol);
         __syncthreads();
         if (S.done || !isfinite(alpha)) break;
         // ---- rotate: vp = v, v = w / beta
@@ -726,7 +541,6 @@ thth_eig_kernel(const float2* __restrict__ Mbase, int ld,
         iters[eta0 + e] = m;
         if (!S.done) status[eta0 + e] |= ST_NOT_CONVERGED;
     }
-    }   // eta loop
 }
 
 // --------------------------------------------------------------------------
@@ -831,17 +645,27 @@ int thth_prep_table(const ThthGeom* geoms, const double* const* th_host, const T
     return SB_OK;
 }
 
+// gather of etas e0 .. e0 + nb - 1 into the fp32 strict upper triangles d_M [nb][ld][ld]
+// and, PACK == 2, the fp16 copy d_Mb; 32-bit CS offsets whenever the spectrum has fewer
+// than 2^32 elements
+template <int PACK>
+static void thth_build_launch(const ThthGeom& g, const double* d_etas, int e0, int nb, int ld,
+                              const int* d_idx, const int* d_nred, float2* d_M, unsigned* d_Mb,
+                              const unsigned* d_absmax, float span, cudaStream_t st) {
+    const int T = ld / 32;
+    const dim3 grid((nb + SB_BUILD_EB - 1) / SB_BUILD_EB, T * (T + 1) / 2), block(32, 8);
+    if ((unsigned long long)g.ntau * (unsigned long long)g.cs_pitch < (1ull << 32))
+        thth_build_kernel<PACK, unsigned><<<grid, block, 0, st>>>(g, d_etas, e0, nb, ld, d_idx,
+                                                                  d_nred, d_M, d_Mb, d_absmax, span);
+    else
+        thth_build_kernel<PACK, size_t><<<grid, block, 0, st>>>(g, d_etas, e0, nb, ld, d_idx,
+                                                                d_nred, d_M, d_Mb, d_absmax, span);
+}
+
 // fp32 strict upper triangles [nb][ld][ld] of etas e0 .. e0 + nb - 1 (no fp16 copy)
 int thth_build_f32(const ThthGeom& g, const double* d_etas, int e0, int nb, int ld,
                    const int* d_idx, const int* d_nred, float2* d_M, cudaStream_t st) {
-    const int T = ld / 32;
-    dim3 grid((nb + SB_BUILD_EB - 1) / SB_BUILD_EB, T * (T + 1) / 2), block(32, 32 / 4);
-    if ((unsigned long long)g.ntau * (unsigned long long)g.cs_pitch < (1ull << 32))
-        thth_build_kernel<0, 4, unsigned><<<grid, block, 0, st>>>(g, d_etas, e0, nb, ld, d_idx,
-                                                                  d_nred, d_M, nullptr, nullptr, 0.f);
-    else
-        thth_build_kernel<0, 4, size_t><<<grid, block, 0, st>>>(g, d_etas, e0, nb, ld, d_idx,
-                                                                d_nred, d_M, nullptr, nullptr, 0.f);
+    thth_build_launch<0>(g, d_etas, e0, nb, ld, d_idx, d_nred, d_M, nullptr, nullptr, 0.f, st);
     SB_LAUNCH_CHECK();
     return SB_OK;
 }
@@ -867,45 +691,18 @@ int eta_sweep(const ThthGeom& g, const double* th_host, const double* d_etas,
     if (batch > neta) batch = neta;
     float2* d_M = (float2*)workspace(2, per * batch);
     if (!d_M) return SB_ERR_NOMEM;
-    // default solver for ld <= 512 (eig_half.cu): iterates on the bf16 copy written by the
-    // build kernel; SB_EIG_FP32=1 selects the fp32 streaming solver below instead
-    const bool mixed = (ld <= 512) && !getenv("SB_EIG_FP32") && !getenv("SB_EIG_CLUSTER") &&
-                       !getenv("SB_EIG_PERSIST") && !getenv("SB_EIG_NO_TMA");
+    // default solver for ld <= 512 (eig_half.cu): iterates on the fp16 copy written by the
+    // build kernel.  Larger grids, and every grid with SB_EIG_FP32=1, run the fp32
+    // thth_eig_kernel, the reference the default solver is checked against.
+    const bool fp16 = (ld <= 512) && !getenv("SB_EIG_FP32");
     unsigned* d_Mb = nullptr;
-    if (mixed) {
-        d_Mb = (unsigned*)workspace(6, per / 2 * batch);
-        if (!d_Mb) return SB_ERR_NOMEM;
-    }
-    const int T = ld / 32;
-    const int npairs = T * (T + 1) / 2;
-    // TMA ring variant (ld <= 512): 256 threads, 2 stages -> 2 CTAs per SM so
-    // one CTA streams while the other is in its serial Lanczos bookkeeping
-    constexpr int TT = 256, TS = 2;      // TMA: threads, stages
-    constexpr int DT = 512;              // direct-load variant
-    const bool use_tma = (ld <= 512) && !getenv("SB_EIG_NO_TMA");
-    const size_t smem = sizeof(LanczosShared) + 4 * (size_t)ld * sizeof(float2) +
-                        (use_tma ? (size_t)(TT / 32) * TS * 4096 + 512
-                                 : (size_t)(DT / 32) * 4096 + 512);
-    // SB_EIG_PERSIST=N: N persistent CTAs (1 per SM, 4-stage ring) walk the curvatures,
-    // so that only N matrices (N MB) are in flight and re-reads hit the L2
-    int persist = 0;
-    if (const char* ev = getenv("SB_EIG_PERSIST")) persist = atoi(ev);
-    constexpr int PS = 4;
-    const size_t smem_p = sizeof(LanczosShared) + 4 * (size_t)ld * sizeof(float2) +
-                          (size_t)(TT / 32) * PS * 4096 + 512;
-    if (use_tma && persist > 0)
-        SB_CUDA(cudaFuncSetAttribute(thth_eig_kernel<TT, true, PS, true>,
-                                     cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_p));
-    if (use_tma)
-        SB_CUDA(cudaFuncSetAttribute(thth_eig_kernel<TT, true, TS>,
-                                     cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    else
-        SB_CUDA(cudaFuncSetAttribute(thth_eig_kernel<DT, false, 1>,
-                                     cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     // scale of the fp16 copy: max |CS| over what the gather can reach, max |theta2 - theta1|
     unsigned* d_absmax = nullptr;
     float span = 0.f;
-    if (mixed) {
+    size_t smem = 0;
+    if (fp16) {
+        d_Mb = (unsigned*)workspace(6, per / 2 * batch);
+        if (!d_Mb) return SB_ERR_NOMEM;
         d_absmax = (unsigned*)workspace(0, 64 * sizeof(double)) + 32;   // behind the dynspec stats
         if (!d_absmax) return SB_ERR_NOMEM;
         if (g.cs_bound) {       // the caller knows a bound (sb_cs_bound_f32): no scan
@@ -923,60 +720,31 @@ int eta_sweep(const ThthGeom& g, const double* th_host, const double* d_etas,
             tmax = th_host[k] > tmax ? th_host[k] : tmax;
         }
         span = (float)((tmax - tmin) * 1.0001);
+    } else {
+        // Lanczos state, v, vp, w, u and the per-warp column partials
+        smem = sizeof(LanczosShared) + 4 * (size_t)ld * sizeof(float2) +
+               (size_t)(EIG_THREADS / 32) * 4096;
+        SB_CUDA(cudaFuncSetAttribute(thth_eig_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)smem));
     }
     for (int e0 = 0; e0 < neta; e0 += batch) {
-        int nb = neta - e0 < batch ? neta - e0 : batch;
-        // rows per thread of thth_build_kernel: 4 (default) or 8 (SB_BUILD_ROWS=8; slower: the
-        // gather is bound by random DRAM sector reads, not by the number of loads a thread keeps
-        // in flight)
-        static const int BR = (getenv("SB_BUILD_ROWS") && atoi(getenv("SB_BUILD_ROWS")) == 8) ? 8 : 4;
-        // tensor-core mat-vec of the default solver (block layout of the fp16 copy);
-        // SB_EIG_NO_TC=1: the FMA mat-vec on the row-major copy
-        const bool tensor = mixed && BR == 4 && !getenv("SB_EIG_NO_TC");
-        dim3 grid((nb + SB_BUILD_EB - 1) / SB_BUILD_EB, npairs), block(32, 32 / BR);
+        const int nb = neta - e0 < batch ? neta - e0 : batch;
         prof_begin(PROF_THTH_BUILD, st);
-        // 32-bit CS offsets whenever the spectrum has fewer than 2^32 elements
-        const bool small = (unsigned long long)g.ntau * (unsigned long long)g.cs_pitch < (1ull << 32);
-#define SB_BUILD_LAUNCH(PACK, ROWS, OFF, MB, AM, SP)                                        \
-        thth_build_kernel<PACK, ROWS, OFF><<<grid, block, 0, st>>>(g, d_etas, e0, nb, ld, d_idx, \
-                                                                   d_nred, d_M, MB, AM, SP)
-        if (BR == 8) {
-            if (mixed && small) SB_BUILD_LAUNCH(1, 8, unsigned, d_Mb, d_absmax, span);
-            else if (mixed) SB_BUILD_LAUNCH(1, 8, size_t, d_Mb, d_absmax, span);
-            else if (small) SB_BUILD_LAUNCH(0, 8, unsigned, nullptr, nullptr, 0.f);
-            else SB_BUILD_LAUNCH(0, 8, size_t, nullptr, nullptr, 0.f);
-        } else if (tensor) {
-            if (small) SB_BUILD_LAUNCH(2, 4, unsigned, d_Mb, d_absmax, span);
-            else SB_BUILD_LAUNCH(2, 4, size_t, d_Mb, d_absmax, span);
-        } else {
-            if (mixed && small) SB_BUILD_LAUNCH(1, 4, unsigned, d_Mb, d_absmax, span);
-            else if (mixed) SB_BUILD_LAUNCH(1, 4, size_t, d_Mb, d_absmax, span);
-            else if (small) SB_BUILD_LAUNCH(0, 4, unsigned, nullptr, nullptr, 0.f);
-            else SB_BUILD_LAUNCH(0, 4, size_t, nullptr, nullptr, 0.f);
-        }
-#undef SB_BUILD_LAUNCH
+        if (fp16)
+            thth_build_launch<2>(g, d_etas, e0, nb, ld, d_idx, d_nred, d_M, d_Mb, d_absmax, span, st);
+        else
+            thth_build_launch<0>(g, d_etas, e0, nb, ld, d_idx, d_nred, d_M, nullptr, nullptr, 0.f, st);
         prof_end(PROF_THTH_BUILD, st);
         SB_LAUNCH_CHECK();
         prof_begin(PROF_THTH_EIG, st);
-        // experimental solvers, each enabled by its own environment variable
-        int rc = mixed ? eig_half_launch(d_M, d_Mb, ld, d_nred, e0, nb, d_eigs, d_status,
-                                         d_iters, tol, 2e-7, max_iter, tensor, st)
-                       : 0;
-        if (rc == 0)
-            rc = eig_cluster_launch(d_M, ld, g.n, d_nred, e0, nb, d_eigs, d_status, d_iters,
-                                    tol, 2e-7, max_iter, st);
-        if (rc < 0) return rc;
-        if (rc > 0) {
-            // handled by eig_half.cu / eig_cluster.cu
-        } else if (use_tma && persist > 0)
-            thth_eig_kernel<TT, true, PS, true><<<persist < nb ? persist : nb, TT, smem_p, st>>>(
-                d_M, ld, d_nred, e0, d_eigs, d_status, d_iters, tol, 2e-7, max_iter, nb);
-        else if (use_tma)
-            thth_eig_kernel<TT, true, TS><<<nb, TT, smem, st>>>(
-                d_M, ld, d_nred, e0, d_eigs, d_status, d_iters, tol, 2e-7, max_iter, nb);
-        else
-            thth_eig_kernel<DT, false, 1><<<nb, DT, smem, st>>>(
-                d_M, ld, d_nred, e0, d_eigs, d_status, d_iters, tol, 2e-7, max_iter, nb);
+        if (fp16) {
+            rc = eig_half_launch(d_M, d_Mb, ld, d_nred, e0, nb, d_eigs, d_status, d_iters, tol,
+                                 2e-7, max_iter, st);
+            if (rc) return rc;
+        } else {
+            thth_eig_kernel<<<nb, EIG_THREADS, smem, st>>>(d_M, ld, d_nred, e0, d_eigs, d_status,
+                                                           d_iters, tol, 2e-7, max_iter);
+        }
         prof_end(PROF_THTH_EIG, st);
         SB_LAUNCH_CHECK();
     }

@@ -1,5 +1,5 @@
 // CPU run of the device code of sb::chisq_sweep up to the inverse FFT, under the
-// SIMT emulator: thth_prep_kernel and thth_build_kernel<0, 4> (csrc/thth.cu),
+// SIMT emulator: thth_prep_kernel and thth_build_kernel<0> (csrc/thth.cu),
 // herm_eigvec_batch_kernel, rev_scatter_rank1_kernel and rev_finalise_batch_kernel
 // (csrc/retrieval.cu), sources unchanged, launch geometry as in sb::chisq_sweep.
 // The transforms are not emulated.  TEST INFRASTRUCTURE (tests/test_chisq_cpu.py).
@@ -49,9 +49,9 @@ extern "C" int emu_chisq_stages(const float* cs, long long ntau, long long nfd, 
         for (unsigned by = 0; by < (unsigned)npairs; ++by)
             emu::run_block(emu::Dim3{32, 8, 1}, emu::Dim3{bx, by, 0},
                            emu::Dim3{gx, (unsigned)npairs, 1}, [&]() {
-                               thth_build_kernel<0, 4, unsigned>(g, etas, 0, neta, ld, idx.data(),
-                                                                 nred, M.data(), nullptr, nullptr,
-                                                                 0.f);
+                               thth_build_kernel<0, unsigned>(g, etas, 0, neta, ld, idx.data(),
+                                                              nred, M.data(), nullptr, nullptr,
+                                                              0.f);
                            });
     std::vector<float2> Q((size_t)neta * (max_iter + 1) * ld);
     float2* V = reinterpret_cast<float2*>(V_out);

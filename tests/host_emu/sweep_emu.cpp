@@ -1,18 +1,16 @@
-// CPU run of the DEFAULT curvature-sweep device code of csrc/thth.cu under the
-// SIMT emulator: thth_prep_kernel (crop mask + compaction), thth_indexerr_kernel,
-// thth_build_kernel (gather into the strict upper triangle) and
-// thth_eig_kernel<256, TMA, 2> (bulk-copy ring + Lanczos), sources unchanged,
-// launch geometry as in sb::eta_sweep.  mixed != 0: the default solver
-// csrc/eig_half.cu (bf16 iteration + fp32 Rayleigh quotient) instead of the fp32
-// thth_eig_kernel; -DSB_EB_SLOTS=3 exercises its fp32 restart.
+// CPU run of the curvature-sweep device code of csrc/thth.cu under the SIMT
+// emulator: thth_prep_kernel (crop mask + compaction), thth_indexerr_kernel,
+// thth_build_kernel (gather into the strict upper triangle) and the fp32
+// thth_eig_kernel (SB_EIG_FP32=1), sources unchanged, launch geometry as in
+// sb::eta_sweep.  mixed != 0: the default solver csrc/eig_half.cu (fp16 tensor-core
+// iteration + fp32 Rayleigh quotient) instead of thth_eig_kernel; mixed == 2 forces
+// its fp32 continuation (rtol_r = 0); -DSB_EB_SLOTS=3 exercises its fp32 restart.
 // TEST INFRASTRUCTURE (tests/test_host_emulation.py).
 #define SB_HOST_EMU 1
 #include "simt.h"
 
 #include <float.h>
 #include <limits.h>
-
-#include <type_traits>
 
 namespace sb {
 alignas(128) unsigned char smem_raw[256 * 1024];
@@ -70,57 +68,46 @@ extern "C" int emu_eta_sweep(const float* cs, long long ntau, long long nfd, lon
     const unsigned gx = (unsigned)((neta + SB_BUILD_EB - 1) / SB_BUILD_EB);
     for (unsigned bx = 0; bx < gx; ++bx)
         for (unsigned by = 0; by < (unsigned)npairs; ++by)
-            // mixed >= 3: the geometry sb::eta_sweep launches by default (4 rows per thread,
-            // 32 x 8 threads); the other paths run the 8-row variant (fewer fibers)
-            emu::run_block(emu::Dim3{32, (unsigned)(mixed >= 3 ? 8 : 4), 1}, emu::Dim3{bx, by, 0},
+            emu::run_block(emu::Dim3{32, 8, 1}, emu::Dim3{bx, by, 0},
                            emu::Dim3{gx, (unsigned)npairs, 1},
                            [&]() {
-                               if (mixed >= 3)
-                                   thth_build_kernel<2, 4, unsigned>(g, etas, 0, neta, ld, idx.data(), nred,
-                                                           M.data(), Mb.data(), &absmax_bits, span);
-                               else if (mixed)
-                                   thth_build_kernel<1, 8, unsigned>(g, etas, 0, neta, ld, idx.data(), nred,
-                                                           M.data(), Mb.data(), &absmax_bits, span);
+                               if (mixed)
+                                   thth_build_kernel<2, unsigned>(g, etas, 0, neta, ld, idx.data(), nred,
+                                                                  M.data(), Mb.data(), &absmax_bits, span);
                                else
-                                   thth_build_kernel<0, 8, size_t>(g, etas, 0, neta, ld, idx.data(), nred,
-                                                            M.data(), nullptr, nullptr, 0.f);
+                                   thth_build_kernel<0, size_t>(g, etas, 0, neta, ld, idx.data(), nred,
+                                                                M.data(), nullptr, nullptr, 0.f);
                            });
     if (M_out) std::memcpy(M_out, M.data(), M.size() * sizeof(float2));   // [neta][ld][ld] triangle
     if (max_iter <= 0 || max_iter > SB_LANCZOS_MAXIT) max_iter = SB_LANCZOS_MAXIT;
     if (mixed) {
-        // mixed = 1: packed-FMA mat-vec, default thresholds; 2: residual threshold 0 -> every
-        // curvature takes the fp32 continuation from the Ritz vector; 3: tensor-core mat-vec
-        // on the block layout (the default on the GPU)
+        // mixed = 2: residual threshold 0 -> every curvature takes the fp32 continuation
+        // from the Ritz vector
         std::vector<float2> gbasis((size_t)neta * EB_SLOTS * ld);
         for (int e = 0; e < neta; ++e) {
             std::memset(smem_raw, 0xa5, sizeof(smem_raw));     // garbage, like real shared memory
-            emu::run_block(emu::Dim3{(unsigned)(mixed >= 3 ? EB_THREADS + 32 : EB_THREADS), 1, 1}, emu::Dim3{(unsigned)e, 0, 0},
+            emu::run_block(emu::Dim3{EB_THREADS + 32, 1, 1}, emu::Dim3{(unsigned)e, 0, 0},
                            emu::Dim3{(unsigned)neta, 1, 1}, [&]() {
-                               if (mixed == 3)
-                                   thth_eig_half_kernel<EB_MODE_TC>(M.data(), Mb.data(), ld, nred, 0, eigs,
-                                                    status, iters, tol, 2e-7, 1e-6, 1e-3, max_iter,
-                                                    gbasis.data());
-                               else
-                                   thth_eig_half_kernel<EB_MODE_CPA>(M.data(), Mb.data(), ld, nred, 0, eigs,
-                                                    status, iters, tol, 2e-7, 1e-6, mixed == 2 ? 0.0 : 1e-3,
+                               thth_eig_half_kernel(M.data(), Mb.data(), ld, nred, 0, eigs, status,
+                                                    iters, tol, 2e-7, 1e-6, mixed == 2 ? 0.0 : 1e-3,
                                                     max_iter, gbasis.data());
                            });
         }
     } else {
         for (int e = 0; e < neta; ++e)
-            emu::run_block(emu::Dim3{256, 1, 1}, emu::Dim3{(unsigned)e, 0, 0},
+            emu::run_block(emu::Dim3{EIG_THREADS, 1, 1}, emu::Dim3{(unsigned)e, 0, 0},
                            emu::Dim3{(unsigned)neta, 1, 1}, [&]() {
-                               thth_eig_kernel<256, true, 2>(M.data(), ld, nred, 0, eigs, status,
-                                                             iters, tol, 2e-7, max_iter, neta);
+                               thth_eig_kernel(M.data(), ld, nred, 0, eigs, status, iters, tol,
+                                               2e-7, max_iter);
                            });
     }
     return 0;
 }
 
 // Eigen solvers on PRE-BUILT triangles M [nb][ld][ld] (strict upper triangle valid,
-// diagonal / columns >= n zero): mixed == 0 -> thth_eig_kernel<256, TMA, 2>,
-// else thth_eig_half_kernel on an fp16 copy packed here with the same rule as the
-// build kernel (power-of-two scale from the largest element).
+// diagonal / columns >= n zero): mixed == 0 -> thth_eig_kernel, else
+// thth_eig_half_kernel on an fp16 copy packed here in the block layout with the same
+// rule as the build kernel (power-of-two scale from the largest element).
 extern "C" int emu_eig_triangles(const float* Mf, int ld, const int* nred, int nb, int mixed,
                                  double tol, int max_iter, double* eigs, int* status, int* iters) {
     using namespace sb;
@@ -146,35 +133,29 @@ extern "C" int emu_eig_triangles(const float* Mf, int ld, const int* nred, int n
                     float2 q = M[((size_t)e * ld + a) * ld + c];
                     if (c >= n || c == a) q = make_float2(0.f, 0.f);
                     const unsigned h = pack_f16x2(make_float2(q.x * sc, q.y * sc));
-                    if (mixed >= 3) {       // block layout (zeros elsewhere: Mb starts as zeros)
-                        unsigned short* Mh = reinterpret_cast<unsigned short*>(Mb.data() + (size_t)e * ld * ld);
-                        const size_t ob = ((size_t)(a >> 4) * (ld >> 3) + (c >> 3)) * 256 + (a & 15) * 16 + (c & 7);
-                        const int sw = (((a & 15) >> 2) & 1) * 8;      // halves swapped in rows 4-7, 12-15
-                        Mh[ob + sw] = (unsigned short)(h & 0xffffu);
-                        Mh[ob + (8 - sw)] = (unsigned short)(h >> 16);
-                    } else {
-                        Mb[((size_t)e * ld + a) * ld + c] = h;
-                    }
+                    // block layout (zeros elsewhere: Mb starts as zeros)
+                    unsigned short* Mh = reinterpret_cast<unsigned short*>(Mb.data() + (size_t)e * ld * ld);
+                    const size_t ob = ((size_t)(a >> 4) * (ld >> 3) + (c >> 3)) * 256 + (a & 15) * 16 + (c & 7);
+                    const int sw = (((a & 15) >> 2) & 1) * 8;      // halves swapped in rows 4-7, 12-15
+                    Mh[ob + sw] = (unsigned short)(h & 0xffffu);
+                    Mh[ob + (8 - sw)] = (unsigned short)(h >> 16);
                 }
         }
     }
     for (int e = 0; e < nb; ++e) {
         std::memset(smem_raw, 0xa5, sizeof(smem_raw));
         if (mixed)
-            emu::run_block(emu::Dim3{(unsigned)(mixed >= 3 ? EB_THREADS + 32 : EB_THREADS), 1, 1}, emu::Dim3{(unsigned)e, 0, 0},
+            emu::run_block(emu::Dim3{EB_THREADS + 32, 1, 1}, emu::Dim3{(unsigned)e, 0, 0},
                            emu::Dim3{(unsigned)nb, 1, 1}, [&]() {
-                               if (mixed == 3)
-                                   thth_eig_half_kernel<EB_MODE_TC>(M, Mb.data(), ld, nred, 0, eigs, status,
-                                                          iters, tol, 2e-7, 1e-6, 1e-3, max_iter, gbasis.data());
-                               else
-                                   thth_eig_half_kernel<EB_MODE_CPA>(M, Mb.data(), ld, nred, 0, eigs, status,
-                                                          iters, tol, 2e-7, 1e-6, 1e-3, max_iter, gbasis.data());
+                               thth_eig_half_kernel(M, Mb.data(), ld, nred, 0, eigs, status, iters, tol,
+                                                    2e-7, 1e-6, mixed == 2 ? 0.0 : 1e-3, max_iter,
+                                                    gbasis.data());
                            });
         else
-            emu::run_block(emu::Dim3{256, 1, 1}, emu::Dim3{(unsigned)e, 0, 0},
+            emu::run_block(emu::Dim3{EIG_THREADS, 1, 1}, emu::Dim3{(unsigned)e, 0, 0},
                            emu::Dim3{(unsigned)nb, 1, 1}, [&]() {
-                               thth_eig_kernel<256, true, 2>(M, ld, nred, 0, eigs, status, iters, tol,
-                                                             2e-7, max_iter, nb);
+                               thth_eig_kernel(M, ld, nred, 0, eigs, status, iters, tol, 2e-7,
+                                               max_iter);
                            });
     }
     return 0;

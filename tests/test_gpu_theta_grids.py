@@ -5,9 +5,9 @@ Besides the spectrum size, the theta-theta code is dispatched on the number of
 theta centres N, padded to ld = 32 ceil(N / 32):
   sweep      eta_sweep / Eval_calc / single_search (thth.cu::eta_sweep):
              ld <= 512: the fp16 tensor-core solver (eig_half.cu), or with
-             SB_EIG_FP32=1 the fp32 TMA kernel; ld 544 .. 4096: the direct-load
-             thth_eig_kernel<512, false, 1>, which walks the cropped matrix in
-             column chunks of 512 (nchunk = ceil(nred / 512) = 1 .. 8);
+             SB_EIG_FP32=1 the fp32 direct-load thth_eig_kernel; ld 544 .. 4096:
+             thth_eig_kernel, which walks the cropped matrix in column chunks
+             of 512 (nchunk = ceil(nred / 512) = 1 .. 8);
              ld > 4096 is refused before any launch.
   thin       thin_sweep / singularvalue_calc (thin.cu): columns in chunks of 512
              (nchunk = ceil(n1 / 512) = 1 .. 8), rows of any count; 4096 on
@@ -141,7 +141,7 @@ def sweep_regimes(c):
     out = []
     for eta in c.etas:
         if ld <= 512:
-            out.append("fp32 tma" if dict(c.extra).get("fp32") else "fp16")
+            out.append("fp32 direct ld<=512" if dict(c.extra).get("fp32") else "fp16")
         else:
             out.append("direct nchunk=%d" % math.ceil(nred(c.n, eta) / 512))
     return out
@@ -154,7 +154,7 @@ def thin_regime(c):
 def missing_coverage():
     miss = []
     sweep = {r for c in SWEEP_CASES for r in sweep_regimes(c)}
-    for want in ["fp16", "fp32 tma"] + ["direct nchunk=%d" % k for k in range(1, 9)]:
+    for want in ["fp16", "fp32 direct ld<=512"] + ["direct nchunk=%d" % k for k in range(1, 9)]:
         if want not in sweep:
             miss.append("sweep " + want)
     lds = {32 * math.ceil(c.n / 32) for c in SWEEP_CASES}

@@ -58,32 +58,6 @@ def test_scale_dyn_kernels_on_host(golden_dir, flip):
     assert np.abs(out - ref).max() < 1e-5 * np.abs(ref).max()
 
 
-def test_bf16_pack_kernel_on_host():
-    """csrc/bf16_pack.cuh: round-to-nearest-even bf16 of (re, im), no overflow to
-    inf, compared with torch.bfloat16."""
-    import torch
-    src = os.path.join(EMU, "bf16_pack_emu.cpp")
-    out = os.path.join(EMU, "_build", "bf16_pack_emu.so")
-    os.makedirs(os.path.dirname(out), exist_ok=True)
-    subprocess.run(["g++", "-O2", "-std=c++17", "-shared", "-fPIC", "-x", "c++", src, "-o", out],
-                   check=True)
-    lib = ctypes.CDLL(out)
-    rng = np.random.default_rng(0)
-    n = 5000
-    x = (rng.normal(size=2 * n) * 10.0 ** rng.uniform(-20, 20, 2 * n)).astype(np.float32)
-    x[:8] = [0.0, -0.0, 1.0, -1.0, 3.3895314e38, -3.3895314e38, 1.0039062, 1.0117188]  # near max, ties
-    xb = np.ascontiguousarray(x)
-    packed = np.zeros(n, np.uint32)
-    lib.emu_pack_bf16.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_long]
-    lib.emu_pack_bf16(xb.ctypes.data_as(ctypes.c_void_p), packed.ctypes.data_as(ctypes.c_void_p), n)
-    re = ((packed & 0xffff).astype(np.uint32) << 16).view(np.float32)
-    im = (packed & 0xffff0000).view(np.float32)
-    ref = torch.from_numpy(xb).to(torch.bfloat16).to(torch.float32).numpy()
-    ref = np.where(np.isinf(ref), np.sign(ref) * np.float32(3.3895314e38), ref)   # we clamp, torch overflows
-    assert np.array_equal(re, ref[0::2])
-    assert np.array_equal(im, ref[1::2])
-
-
 @pytest.mark.parametrize("n0,n1,c0,c1", [(12, 10, 0, 0), (9, 20, 5, 7), (16, 15, 16, 4)])
 def test_chirp_ifft2_functors_on_host(n0, n1, c0, c1):
     """The chirp-z any-size inverse FFT (dynspec.cu::ifft2_c2c_any): tables and
@@ -156,16 +130,15 @@ def _sweep_emu_lib(slots=0):
     return ctypes.CDLL(out)
 
 
-@pytest.mark.parametrize("mixed,slots", [(0, 0), (1, 0), (2, 0), (1, 3), (3, 0), (3, 3)])
+@pytest.mark.parametrize("mixed,slots", [(0, 0), (2, 0), (3, 0), (3, 3)])
 def test_default_sweep_kernels_on_host(golden_dir, mixed, slots):
     """The device code of the curvature sweep (csrc/thth.cu: thth_prep_kernel,
     thth_indexerr_kernel, thth_build_kernel; csrc/eig_half.cu) under the SIMT
     emulator, launch geometry as in sb::eta_sweep, against the reference: cropped
-    sizes bit-exact, eigenvalues to 1e-5.  mixed=0: the fp32 streaming solver
-    thth_eig_kernel<256, TMA, 2> (SB_EIG_FP32=1); mixed=1: the default solver
-    with the FMA mat-vec (fp16 iteration + fp32 Rayleigh quotient); mixed=2: its
-    fp32 continuation forced on every curvature; mixed=3: the tensor-core mat-vec on the
-    block layout of the fp16 copy (ldmatrix / mma.sync emulated lane-exactly);
+    sizes bit-exact, eigenvalues to 1e-5.  mixed=0: the fp32 solver thth_eig_kernel
+    (SB_EIG_FP32=1); mixed=3: the default solver (fp16 tensor-core iteration on the
+    block layout of the fp16 copy, ldmatrix / mma.sync emulated lane-exactly, + fp32
+    Rayleigh quotient); mixed=2: its fp32 continuation forced on every curvature;
     slots=3: the fp32 restart (basis slots exhausted)."""
     from oracle import thth_oracle as TO
     lib = _sweep_emu_lib(slots)
@@ -272,7 +245,7 @@ def test_thin_three_column_chunks_on_host(golden_dir):
 
 
 @pytest.mark.parametrize("nedge,half,coherent,mixed", [(42, 0, 1, 0), (72, 1, 1, 0), (34, 0, 0, 0),
-                                                      (66, 1, 1, 1), (50, 1, 1, 2), (66, 1, 1, 3),
+                                                      (50, 1, 1, 2), (66, 1, 1, 3),
                                                       (42, 0, 1, 3), (34, 0, 0, 3)])
 def test_default_sweep_kernels_on_host_random(nedge, half, coherent, mixed):
     """Random small spectra through the emulated sweep kernels: full and
@@ -373,7 +346,7 @@ def test_retrieval_kernels_on_host(golden_dir):
     assert np.abs(V * (z / abs(z)) - Vr).max() < 3e-5 * np.abs(Vr).max()
 
 
-@pytest.mark.parametrize("mixed", [0, 1, 3])
+@pytest.mark.parametrize("mixed", [0, 3])
 def test_slowly_converging_curvature_on_host(golden_dir, mixed):
     """Regression for the round-1 stopping bug (lanczos.cuh: the residual estimate
     collapsed to 0 at the first range rescaling of the Sturm sequence, step ~21 for
