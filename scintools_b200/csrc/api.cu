@@ -11,8 +11,8 @@
 namespace sb {
 
 static thread_local char g_err[512] = "";
-static void* g_ws[8] = {nullptr};
-static size_t g_ws_bytes[8] = {0};
+static void* g_ws[9] = {nullptr};
+static size_t g_ws_bytes[9] = {0};
 static int g_sms = 132;
 
 void set_error(const char* fmt, ...) {
@@ -57,7 +57,7 @@ void prof_end(int id, cudaStream_t st) {
 }
 
 void* workspace(int slot, size_t bytes) {
-    if (slot < 0 || slot >= 8) return nullptr;
+    if (slot < 0 || slot >= 9) return nullptr;
     if (bytes <= g_ws_bytes[slot] && g_ws[slot]) return g_ws[slot];
     if (g_ws[slot]) {
         cudaDeviceSynchronize();
@@ -81,7 +81,7 @@ void* workspace(int slot, size_t bytes) {
 
 void workspace_release() {
     cudaDeviceSynchronize();
-    for (int i = 0; i < 8; ++i) {
+    for (int i = 0; i < 9; ++i) {
         if (g_ws[i]) cudaFree(g_ws[i]);
         g_ws[i] = nullptr;
         g_ws_bytes[i] = 0;

@@ -772,8 +772,11 @@ __global__ void chisq_finish_kernel(const double* __restrict__ part, int e0, int
 // thth.cu / dynspec.cu
 int thth_prep(const ThthGeom& g, const double* th_host, const double* d_etas, int neta, int ld,
               int* d_idx, int* d_nred, int* d_status, cudaStream_t st);
-int thth_build_f32(const ThthGeom& g, const double* d_etas, int e0, int nb, int ld,
-                   const int* d_idx, const int* d_nred, float2* d_M, cudaStream_t st);
+int thth_gather_source(const ThthGeom& g, const double* th_host, int neta, ThthCopy* copy,
+                       cudaStream_t st);
+int thth_gather_check(const ThthCopy& copy, cudaStream_t st);
+int thth_build_f32(const ThthGeom& g, const ThthCopy& copy, const double* d_etas, int e0, int nb,
+                   int ld, const int* d_idx, const int* d_nred, float2* d_M, cudaStream_t st);
 unsigned long long sweep_slab_bytes();
 int ifft2_any_residual(const float2* in, int n0, int n1, const ResidualSink& sink,
                        cudaStream_t st);
@@ -813,6 +816,9 @@ int chisq_sweep(const ThthGeom& g, const double* th_host, const double* d_etas, 
     if (!d_idx) return SB_ERR_NOMEM;
     int rc = thth_prep(g, th_host, d_etas, neta, ld, d_idx, d_nred, d_status, st);
     if (rc) return rc;
+    ThthCopy copy;
+    rc = thth_gather_source(g, th_host, neta, &copy, st);
+    if (rc) return rc;
     // per curvature: matrix, Lanczos basis, eigenvector, bin sums, partial sums, counts
     // (+ the row-transformed spectrum on the radix path), all under the sweep's slab budget
     const size_t bins = (size_t)n0 * n1;
@@ -850,7 +856,7 @@ int chisq_sweep(const ThthGeom& g, const double* th_host, const double* d_etas, 
     const float scale = (float)(1.0 / ((double)n0 * (double)n1));
     for (int e0 = 0; e0 < neta; e0 += batch) {
         const int nb = neta - e0 < batch ? neta - e0 : batch;
-        rc = thth_build_f32(g, d_etas, e0, nb, ld, d_idx, d_nred, M, st);
+        rc = thth_build_f32(g, copy, d_etas, e0, nb, ld, d_idx, d_nred, M, st);
         if (rc) return rc;
         herm_eigvec_batch_kernel<<<nb, EV_THREADS, smem, st>>>(M, ld, d_nred, e0, Q, max_iter, tol,
                                                               d_w, V, d_status, d_iters);
@@ -887,7 +893,7 @@ int chisq_sweep(const ThthGeom& g, const double* th_host, const double* d_etas, 
         chisq_finish_kernel<<<(nb + 127) / 128, 128, 0, st>>>(part, e0, nb, d_status, d_ssq);
         SB_LAUNCH_CHECK();
     }
-    return SB_OK;
+    return thth_gather_check(copy, st);
 }
 
 // --------------------------------------------------------------------------

@@ -10,6 +10,9 @@
 #include <limits.h>
 #include <math.h>
 #include <stdlib.h>
+#include <string.h>
+
+#include <vector>
 
 #include "lanczos.cuh"
 #include "thth.cuh"
@@ -163,30 +166,38 @@ __global__ void cs_absmax_kernel(const float2* __restrict__ cs, long long rows, 
 // Jacobian remain.  The cached pair is re-derived whenever the crop of the next
 // curvature moves the pair (idx differs).
 // ROWS = 4 rows of the tile per thread (block = 32 x 8 threads).  Per curvature the
-// body runs in three phases -- (1) tau_inv and the CS offset of every row, (2) ALL the
+// body runs in three phases -- (1) tau_inv and the offset of every row, (2) ALL the
 // gathers back to back, (3) Jacobian, clean-up, stores -- so that ROWS independent
-// L2 / DRAM gathers are in flight per thread: the kernel is bound by the latency of
-// these random 8-byte loads (long-scoreboard stalls dominate with one load in flight),
-// not by its instruction count.
+// gathers are in flight per thread.
+// COPY: the gathers read the compact copy of the spectrum columns the grid reaches
+// (ThthCopy, thth.cuh), delay axis contiguous, where neighbouring curvatures of a pair fall
+// in the same or the next 32-byte sector and the whole copy is re-read from L2
+// (thth_build_copy_kernel); otherwise the spectrum itself, where every gather costs a DRAM
+// sector of its own (thth_build_kernel).  thth_gather_source chooses.
 // PACK == 0: the fp32 triangle only.  PACK == 2: also the fp16 copy in the block layout
 // of eig_half.cu's tensor-core mat-vec: 512-byte blocks of 16 rows x 8 columns, block
 // (I, G) at ((I * ld / 8 + G) * 512) bytes, a block row = [re x 8 | im x 8] (the halves
 // swapped in rows 4-7, 12-15); the part of a diagonal block on / below the diagonal is
 // written as zeros (the MMA has no masks).
-// Three CTAs per SM (80 registers).  ptxas still spills at 80 registers, but
-// less: 40-48 bytes of stores and 56-68 bytes of loads per thread in the PACK == 2
-// instances on sm_90, against ~200 / ~150 bytes at four CTAs (64 registers), where the
-// gather runs ~15 % slower on the headline sweep (H100 SXM, 400 W power limit: 2.8-2.9 ms
-// instead of 2.4 ms per 1024-eta launch).
-template <int PACK, typename OFF>
-__global__ void __launch_bounds__(256, 3)
-thth_build_kernel(ThthGeom g, const double* __restrict__ etas, int eta0, int nbatch,
-                  int ld, const int* __restrict__ idx,
-                  const int* __restrict__ nred, float2* __restrict__ M,
-                  unsigned* __restrict__ Mb, const unsigned* __restrict__ absmax, float span) {
+// Three CTAs per SM (80 registers; spill stores per thread in the PACK == 2 instances on
+// sm_90: 40-44 bytes reading the spectrum, 12-20 bytes reading the copy).  Measured on the
+// headline sweep from the compact copy (H100 SXM, 700 W power limit, thth_build per
+// 1024-eta launch, copy included), variants built from one source and alternated in one
+// run: 1.76 ms as is; 1.78 ms with streaming (__stcs) stores of the triangles, alone or with
+// an L2 evict-last policy on the gathers; 1.84 ms with the tile pairs ordered by diagonal;
+// 1.78 ms with four CTAs per SM (64 registers, ~170 bytes of spills), which also slows the
+// gather from the spectrum itself (2.41 against 2.23 ms on an irregular grid).  None of
+// them is kept.
+template <int PACK, typename OFF, bool COPY>
+__device__ __forceinline__ void
+thth_build_body(const ThthGeom& g, const double* __restrict__ etas, int eta0, int nbatch,
+                int ld, const int* __restrict__ idx,
+                const int* __restrict__ nred, float2* __restrict__ M,
+                unsigned* __restrict__ Mb, const unsigned* __restrict__ absmax, float span,
+                const ThthCopy& copy) {
     // eta is the FAST grid index: CTAs resident at the same time work on the
     // same 32x32 tile for neighbouring curvatures, whose gathers fall on
-    // the same / adjacent CS rows for small |theta1^2 - theta2^2| (L2 reuse)
+    // the same / adjacent delay bins for small |theta1^2 - theta2^2| (L2 reuse)
     // pair index -> (ta <= tb)
     constexpr int ROWS = 4, TY = 32 / ROWS;
     int p = blockIdx.y, ta = 0;
@@ -196,13 +207,12 @@ thth_build_kernel(ThthGeom g, const double* __restrict__ etas, int eta0, int nba
     const int tx = threadIdx.x, ty = threadIdx.y;
     const int b = tb * 32 + tx;
     const double ntau_d = (double)g.ntau;
-    const long long hfd = g.nfd / 2;
     // cached eta-independent state of this thread's column and its ROWS rows
     int cj = -2;
     double thj = 0.0;
     int ci[ROWS];
     double dk[ROWS];
-    int col[ROWS];          // CS column to gather; < 0: never a valid point
+    int col[ROWS];          // CS column (COPY: slot of the copy) to gather; < 0: never a valid point
     unsigned conj = 0u;     // bit k: the point lies in the mirrored (fd < 0) half
     float wk[ROWS];
 #pragma unroll
@@ -252,7 +262,7 @@ thth_build_kernel(ThthGeom g, const double* __restrict__ etas, int eta0, int nba
         // power of two: |element| * hscale < 2^15
         const float hscale = PACK != 0 ? s_hscale[e - blockIdx.x * SB_BUILD_EB] : 1.f;
         // ---- phase 1: offsets
-        OFF off[ROWS];          // element offset into the CS (OFF = unsigned when it fits)
+        OFF off[ROWS];          // element offset into the CS / the copy (OFF = unsigned when it fits)
         unsigned hit = 0u;
 #pragma unroll
         for (int k = 0; k < ROWS; ++k) {
@@ -271,17 +281,17 @@ thth_build_kernel(ThthGeom g, const double* __restrict__ etas, int eta0, int nba
                     // th1 = theta of the column, th2 = theta of the row (ththmod.py:86-87)
                     const double th1 = thj, th2 = g.th[i];
                     dk[k] = __dsub_rn(__dmul_rn(th1, th1), __dmul_rn(th2, th2));
-                    const double bb = __dadd_rn(__dsub_rn(__dsub_rn(th1, th2), g.fd0), g.half_dfd);
-                    const double fqd = floor_div_fast(bb, g.dfd, g.inv_dfd);
-                    const long long fq = (fqd == fqd && fabs(fqd) < 9.0e18) ? (long long)fqd : LLONG_MIN;
                     wk[k] = sqrtf((float)fabs(th2 - th1));
-                    if (fq < g.nfd && !(fq < -g.nfd)) {     // pnts mask / IndexError (thth_point)
-                        const long long fi = fq < 0 ? fq + g.nfd : fq;
-                        if (!g.cs_half) col[k] = (int)fi;
-                        else if (fi >= hfd) col[k] = (int)(fi - hfd);
-                        else if (fi == 0) col[k] = (int)hfd;
-                        else { col[k] = (int)(hfd - fi); conj |= 1u << k; }   // CS[-tau,-fd] = conj(CS[tau,fd])
+                    bool mirrored;
+                    int c = thth_pair_column(g, th1, th2, &mirrored);
+                    if (COPY && c >= 0) {
+                        c = copy.slot_of_col[c];
+                        // a column the copy does not hold: the element stays zero, no
+                        // address is formed from it
+                        if (c < 0) atomicOr(copy.err, 1);
                     }
+                    col[k] = c;
+                    if (mirrored) conj |= 1u << k;
                 }
             }
             if (col[k] >= 0) {
@@ -290,15 +300,17 @@ thth_build_kernel(ThthGeom g, const double* __restrict__ etas, int eta0, int nba
                 if (tqd > 0.0 && tqd < ntau_d) {            // tau_inv > 0 and < ntau (ththmod.py:100)
                     const int tq = (int)tqd;
                     const int r = (conj >> k) & 1u ? (int)g.ntau - tq : tq;
-                    off[k] = (OFF)r * (OFF)g.cs_pitch + (OFF)col[k];
+                    off[k] = COPY ? (OFF)col[k] * (OFF)copy.tau_pitch + (OFF)r
+                                  : (OFF)r * (OFF)g.cs_pitch + (OFF)col[k];
                     hit |= 1u << k;
                 }
             }
         }
-        // ---- phase 2: the gathers, all in flight together (a miss reads CS[0], ignored)
+        // ---- phase 2: the gathers, all in flight together (a miss reads element 0, ignored)
         float2 val[ROWS];
+        const float2* __restrict__ from = COPY ? copy.base : g.cs;
 #pragma unroll
-        for (int k = 0; k < ROWS; ++k) val[k] = __ldg(g.cs + off[k]);
+        for (int k = 0; k < ROWS; ++k) val[k] = __ldg(from + off[k]);
         // ---- phase 3
 #pragma unroll
         for (int k = 0; k < ROWS; ++k) {
@@ -347,6 +359,106 @@ thth_build_kernel(ThthGeom g, const double* __restrict__ etas, int eta0, int nba
                 }
             }
         }
+    }
+}
+
+template <int PACK, typename OFF>
+__global__ void __launch_bounds__(256, 3)
+thth_build_kernel(ThthGeom g, const double* __restrict__ etas, int eta0, int nbatch,
+                  int ld, const int* __restrict__ idx,
+                  const int* __restrict__ nred, float2* __restrict__ M,
+                  unsigned* __restrict__ Mb, const unsigned* __restrict__ absmax, float span) {
+    thth_build_body<PACK, OFF, false>(g, etas, eta0, nbatch, ld, idx, nred, M, Mb, absmax, span,
+                                      ThthCopy{nullptr, 0, 0, nullptr, nullptr});
+}
+
+template <int PACK, typename OFF>
+__global__ void __launch_bounds__(256, 3)
+thth_build_copy_kernel(ThthGeom g, const double* __restrict__ etas, int eta0, int nbatch,
+                       int ld, const int* __restrict__ idx,
+                       const int* __restrict__ nred, float2* __restrict__ M,
+                       unsigned* __restrict__ Mb, const unsigned* __restrict__ absmax, float span,
+                       ThthCopy copy) {
+    thth_build_body<PACK, OFF, true>(g, etas, eta0, nbatch, ld, idx, nred, M, Mb, absmax, span,
+                                     copy);
+}
+
+// --------------------------------------------------------------------------
+// compact copy of the spectrum columns a theta grid reaches (ThthCopy, thth.cuh)
+// --------------------------------------------------------------------------
+// mark[c] = 1 for every stored column c that some pair (i, j), j > i, i + j != n - 1, of
+// ALL n centres maps to: a superset of what any curvature's cropped grid gathers, and
+// independent of the curvature.  mark: int [thth_ncols(g)], zeroed by the caller.
+__global__ void thth_colmark_kernel(ThthGeom g, int* __restrict__ mark) {
+    const long long total = (long long)g.n * g.n;
+    for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < total;
+         p += (long long)gridDim.x * blockDim.x) {
+        const int i = (int)(p / g.n), j = (int)(p % g.n);
+        if (!(j > i && i + j != g.n - 1)) continue;
+        bool mirrored;
+        const int c = thth_pair_column(g, g.th[j], g.th[i], &mirrored);
+        if (c >= 0) mark[c] = 1;
+    }
+}
+
+// One block: marks -> slot_of_col [ncols] (slots in column order, -1 = not reached),
+// col_of_slot [ncols] (first *nslots entries valid) and *nslots.  No slot >= cap is handed
+// out (cap = the slot count the copy was sized for): such a column stays unmapped and
+// *err is raised.
+constexpr int SLOT_THREADS = 256;
+__global__ void __launch_bounds__(SLOT_THREADS)
+thth_colslots_kernel(const int* __restrict__ mark, int ncols, int cap,
+                     int* __restrict__ slot_of_col, int* __restrict__ col_of_slot,
+                     int* __restrict__ nslots, int* __restrict__ err) {
+    SB_SHARED int s_cnt[SLOT_THREADS];
+    const int t = threadIdx.x;
+    const int per = (ncols + SLOT_THREADS - 1) / SLOT_THREADS;
+    const int c0 = min(t * per, ncols), c1 = min(c0 + per, ncols);
+    int cnt = 0;
+    for (int c = c0; c < c1; ++c) cnt += mark[c] != 0;
+    s_cnt[t] = cnt;
+    __syncthreads();
+    int s = 0, total = 0;
+    for (int k = 0; k < SLOT_THREADS; ++k) {
+        if (k < t) s += s_cnt[k];
+        total += s_cnt[k];
+    }
+    for (int c = c0; c < c1; ++c) {
+        int slot = -1;
+        if (mark[c] != 0) {
+            if (s < cap) { slot = s; col_of_slot[s] = c; }
+            else atomicOr(err, 1);
+            ++s;
+        }
+        slot_of_col[c] = slot;
+    }
+    if (t == 0) *nslots = total;
+}
+
+// C[slot][r] = CS[r][col_of_slot[slot]], C: float2 [nslots][tau_pitch].  32 x 32 tiles
+// through shared memory, so that the reads run along the columns (neighbouring slots are
+// neighbouring columns on a uniform grid) and the writes along the delay axis.
+// grid = (ceil(ntau / 32), ceil(nslots / 32)), block = 32 x 8.
+__global__ void __launch_bounds__(256)
+cs_compact_kernel(const float2* __restrict__ cs, long long ntau, long long cs_pitch,
+                  const int* __restrict__ col_of_slot, int nslots, long long tau_pitch,
+                  float2* __restrict__ C) {
+    SB_SHARED float2 tile[32][33];
+    const int tx = threadIdx.x, ty = threadIdx.y;
+    const long long r0 = (long long)blockIdx.x * 32;
+    const int s0 = blockIdx.y * 32;
+    const int c = s0 + tx < nslots ? col_of_slot[s0 + tx] : -1;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const long long r = r0 + ty + 8 * k;
+        if (c >= 0 && r < ntau) tile[ty + 8 * k][tx] = __ldg(cs + r * cs_pitch + c);
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const int s = s0 + ty + 8 * k;
+        const long long r = r0 + tx;
+        if (s < nslots && r < ntau) C[(long long)s * tau_pitch + r] = tile[tx][ty + 8 * k];
     }
 }
 
@@ -645,27 +757,156 @@ int thth_prep_table(const ThthGeom* geoms, const double* const* th_host, const T
     return SB_OK;
 }
 
-// gather of etas e0 .. e0 + nb - 1 into the fp32 strict upper triangles d_M [nb][ld][ld]
-// and, PACK == 2, the fp16 copy d_Mb; 32-bit CS offsets whenever the spectrum has fewer
-// than 2^32 elements
+// Where the gathers of one sweep call read (ThthCopy, thth.cuh), made once per call and
+// shared by its curvature batches.
+//
+// The table of reached columns is built on the device (thth_colmark_kernel,
+// thth_colslots_kernel) on every call; the host only needs the slot count, to size the
+// copy and to choose.  It is read back once per geometry (one stream synchronise) and kept:
+// the table depends on the theta centres and the fd axis only, and the kernels are
+// deterministic, so later calls with the same geometry get the same count without a
+// read-back, and hand it to thth_colslots_kernel as the cap no slot may reach.
+//
+// The copy is used when the 32-byte sectors the direct gather would read, one per
+// gathered element (neighbouring curvatures of a pair sit a whole CS row apart), are at
+// least twice the bytes of making the copy (a sector read + 8 bytes written per element):
+// few curvatures, or a grid whose pairs all fall on different columns, gather from the
+// spectrum itself.
+struct ColCache {
+    bool valid = false;
+    long long nfd = 0;
+    int cs_half = 0, n = 0;
+    double fd0 = 0, dfd = 0, half_dfd = 0, inv_dfd = 0;
+    std::vector<double> th;
+    int nslots = 0;
+    bool checked = false;   // the error word has been read back after a sweep from the copy
+};
+static ColCache g_colcache;
+
+int thth_gather_source(const ThthGeom& g, const double* th_host, int neta, ThthCopy* copy,
+                       cudaStream_t st) {
+    const int ncols = (int)(g.cs_half ? g.nfd / 2 + 1 : g.nfd);
+    const size_t tab_bytes = ((size_t)(3 * (size_t)ncols + 2) * sizeof(int) + 255) & ~(size_t)255;
+    ColCache& cc = g_colcache;
+    const bool hit = cc.valid && cc.nfd == g.nfd && cc.cs_half == g.cs_half && cc.n == g.n &&
+                     cc.fd0 == g.fd0 && cc.dfd == g.dfd && cc.half_dfd == g.half_dfd &&
+                     cc.inv_dfd == g.inv_dfd &&
+                     memcmp(cc.th.data(), th_host, (size_t)g.n * sizeof(double)) == 0;
+    // [mark | slot_of_col | col_of_slot | nslots, err] then the copy
+    auto build_table = [&](int* tab, int cap) -> int {
+        int* mark = tab;
+        int* slot_of_col = tab + ncols;
+        int* col_of_slot = tab + 2 * (size_t)ncols;
+        int* tail = tab + 3 * (size_t)ncols;
+        // zero: marks, the error word, and col_of_slot (an entry the scan does not write
+        // is column 0, inside the spectrum)
+        SB_CUDA(cudaMemsetAsync(tab, 0, tab_bytes, st));
+        const long long pairs = (long long)g.n * g.n;
+        int blocks = (int)((pairs + 255) / 256);
+        if (blocks > num_sms() * 16) blocks = num_sms() * 16;
+        thth_colmark_kernel<<<blocks, 256, 0, st>>>(g, mark);
+        SB_LAUNCH_CHECK();
+        thth_colslots_kernel<<<1, SLOT_THREADS, 0, st>>>(mark, ncols, cap, slot_of_col,
+                                                         col_of_slot, tail, tail + 1);
+        SB_LAUNCH_CHECK();
+        return SB_OK;
+    };
+    if (!hit) {
+        int* tab = (int*)workspace(8, tab_bytes);
+        if (!tab) return SB_ERR_NOMEM;
+        int rc = build_table(tab, INT_MAX);
+        if (rc) return rc;
+        int nslots = 0;
+        SB_CUDA(cudaMemcpyAsync(&nslots, tab + 3 * (size_t)ncols, sizeof(int),
+                                cudaMemcpyDeviceToHost, st));
+        SB_CUDA(cudaStreamSynchronize(st));
+        if (nslots < 0 || nslots > ncols) {
+            set_error("theta-theta column table: %d slots for %d columns", nslots, ncols);
+            return SB_ERR_CUDA;
+        }
+        cc.valid = true;
+        cc.nfd = g.nfd; cc.cs_half = g.cs_half; cc.n = g.n;
+        cc.fd0 = g.fd0; cc.dfd = g.dfd; cc.half_dfd = g.half_dfd; cc.inv_dfd = g.inv_dfd;
+        cc.th.assign(th_host, th_host + g.n);
+        cc.nslots = nslots;
+        cc.checked = false;
+    }
+    const int nslots = cc.nslots;
+    const long long tau_pitch = (g.ntau + 3) / 4 * 4;
+    const double pairs = 0.5 * (double)g.n * (double)(g.n - 1);
+    const double direct_bytes = 32.0 * (double)neta * pairs;
+    const double copy_bytes = 40.0 * (double)nslots * (double)g.ntau;
+    if (nslots == 0 || direct_bytes < 2.0 * copy_bytes) {
+        *copy = ThthCopy{nullptr, 0, 0, nullptr, nullptr};
+        return SB_OK;
+    }
+    unsigned char* ws = (unsigned char*)workspace(
+        8, tab_bytes + (size_t)nslots * (size_t)tau_pitch * sizeof(float2));
+    if (!ws) return SB_ERR_NOMEM;
+    int* tab = (int*)ws;
+    float2* C = (float2*)(ws + tab_bytes);
+    prof_begin(PROF_THTH_BUILD, st);
+    int rc = build_table(tab, nslots);
+    if (!rc) {
+        const dim3 grid((unsigned)((g.ntau + 31) / 32), (unsigned)((nslots + 31) / 32));
+        cs_compact_kernel<<<grid, dim3(32, 8), 0, st>>>(g.cs, g.ntau, g.cs_pitch,
+                                                        tab + 2 * (size_t)ncols, nslots,
+                                                        tau_pitch, C);
+    }
+    prof_end(PROF_THTH_BUILD, st);
+    if (rc) return rc;
+    SB_LAUNCH_CHECK();
+    *copy = ThthCopy{C, tau_pitch, nslots, tab + ncols, tab + 3 * (size_t)ncols + 1};
+    return SB_OK;
+}
+
+// After the gathers of a sweep: the first sweep of a geometry that read the copy waits for
+// them and reports a raised error word (a pair whose column the table did not hold: its
+// element was left zero).  Later sweeps of the same geometry do not wait.
+int thth_gather_check(const ThthCopy& copy, cudaStream_t st) {
+    if (!copy.base || g_colcache.checked) return SB_OK;
+    int err = 0;
+    SB_CUDA(cudaMemcpyAsync(&err, copy.err, sizeof(int), cudaMemcpyDeviceToHost, st));
+    SB_CUDA(cudaStreamSynchronize(st));
+    if (err) {
+        set_error("theta-theta gather: a pair of the grid maps to a spectrum column that the "
+                  "table of reached columns does not hold");
+        return SB_ERR_CUDA;
+    }
+    g_colcache.checked = true;
+    return SB_OK;
+}
+
+// gather of etas e0 .. e0 + nb - 1, from the copy if there is one and from the spectrum
+// otherwise, into the fp32 strict upper triangles d_M [nb][ld][ld] and, PACK == 2, the fp16
+// copy d_Mb; 32-bit offsets whenever what is gathered from has fewer than 2^32 elements
 template <int PACK>
-static void thth_build_launch(const ThthGeom& g, const double* d_etas, int e0, int nb, int ld,
-                              const int* d_idx, const int* d_nred, float2* d_M, unsigned* d_Mb,
-                              const unsigned* d_absmax, float span, cudaStream_t st) {
+static void thth_build_launch(const ThthGeom& g, const ThthCopy& copy, const double* d_etas,
+                              int e0, int nb, int ld, const int* d_idx, const int* d_nred,
+                              float2* d_M, unsigned* d_Mb, const unsigned* d_absmax, float span,
+                              cudaStream_t st) {
     const int T = ld / 32;
     const dim3 grid((nb + SB_BUILD_EB - 1) / SB_BUILD_EB, T * (T + 1) / 2), block(32, 8);
-    if ((unsigned long long)g.ntau * (unsigned long long)g.cs_pitch < (1ull << 32))
+    if (copy.base) {
+        if ((unsigned long long)copy.nslots * (unsigned long long)copy.tau_pitch < (1ull << 32))
+            thth_build_copy_kernel<PACK, unsigned><<<grid, block, 0, st>>>(
+                g, d_etas, e0, nb, ld, d_idx, d_nred, d_M, d_Mb, d_absmax, span, copy);
+        else
+            thth_build_copy_kernel<PACK, size_t><<<grid, block, 0, st>>>(
+                g, d_etas, e0, nb, ld, d_idx, d_nred, d_M, d_Mb, d_absmax, span, copy);
+    } else if ((unsigned long long)g.ntau * (unsigned long long)g.cs_pitch < (1ull << 32)) {
         thth_build_kernel<PACK, unsigned><<<grid, block, 0, st>>>(g, d_etas, e0, nb, ld, d_idx,
                                                                   d_nred, d_M, d_Mb, d_absmax, span);
-    else
+    } else {
         thth_build_kernel<PACK, size_t><<<grid, block, 0, st>>>(g, d_etas, e0, nb, ld, d_idx,
                                                                 d_nred, d_M, d_Mb, d_absmax, span);
+    }
 }
 
 // fp32 strict upper triangles [nb][ld][ld] of etas e0 .. e0 + nb - 1 (no fp16 copy)
-int thth_build_f32(const ThthGeom& g, const double* d_etas, int e0, int nb, int ld,
-                   const int* d_idx, const int* d_nred, float2* d_M, cudaStream_t st) {
-    thth_build_launch<0>(g, d_etas, e0, nb, ld, d_idx, d_nred, d_M, nullptr, nullptr, 0.f, st);
+int thth_build_f32(const ThthGeom& g, const ThthCopy& copy, const double* d_etas, int e0, int nb,
+                   int ld, const int* d_idx, const int* d_nred, float2* d_M, cudaStream_t st) {
+    thth_build_launch<0>(g, copy, d_etas, e0, nb, ld, d_idx, d_nred, d_M, nullptr, nullptr, 0.f, st);
     SB_LAUNCH_CHECK();
     return SB_OK;
 }
@@ -683,6 +924,9 @@ int eta_sweep(const ThthGeom& g, const double* th_host, const double* d_etas,
     int* d_idx = (int*)workspace(1, (size_t)neta * ld * sizeof(int));
     if (!d_idx) return SB_ERR_NOMEM;
     int rc = thth_prep(g, th_host, d_etas, neta, ld, d_idx, d_nred, d_status, st);
+    if (rc) return rc;
+    ThthCopy copy;
+    rc = thth_gather_source(g, th_host, neta, &copy, st);
     if (rc) return rc;
     // batch so that the matrix slab stays <= ~3 GiB
     const size_t per = (size_t)ld * ld * sizeof(float2);
@@ -731,9 +975,10 @@ int eta_sweep(const ThthGeom& g, const double* th_host, const double* d_etas,
         const int nb = neta - e0 < batch ? neta - e0 : batch;
         prof_begin(PROF_THTH_BUILD, st);
         if (fp16)
-            thth_build_launch<2>(g, d_etas, e0, nb, ld, d_idx, d_nred, d_M, d_Mb, d_absmax, span, st);
+            thth_build_launch<2>(g, copy, d_etas, e0, nb, ld, d_idx, d_nred, d_M, d_Mb, d_absmax, span, st);
         else
-            thth_build_launch<0>(g, d_etas, e0, nb, ld, d_idx, d_nred, d_M, nullptr, nullptr, 0.f, st);
+            thth_build_launch<0>(g, copy, d_etas, e0, nb, ld, d_idx, d_nred, d_M, nullptr, nullptr, 0.f,
+                                 st);
         prof_end(PROF_THTH_BUILD, st);
         SB_LAUNCH_CHECK();
         prof_begin(PROF_THTH_EIG, st);
@@ -748,7 +993,7 @@ int eta_sweep(const ThthGeom& g, const double* th_host, const double* d_etas,
         prof_end(PROF_THTH_EIG, st);
         SB_LAUNCH_CHECK();
     }
-    return SB_OK;
+    return thth_gather_check(copy, st);
 }
 
 __global__ void thth_mask_kernel(ThthGeom g, double eta,

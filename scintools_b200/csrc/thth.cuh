@@ -1,5 +1,7 @@
 // theta-theta geometry shared by the gather / eigen kernels.
 #pragma once
+#include <limits.h>
+
 #include "common.cuh"
 
 namespace sb {
@@ -45,6 +47,47 @@ __device__ __forceinline__ ThthPoint thth_point(const ThthGeom& g, double eta,
     p.index_error = p.pnt && (p.fq < -g.nfd);
     return p;
 }
+
+// Stored CS columns a gather can address: every column of the full layout, the fd >= 0
+// half (k = 0..nfd/2, all inside cs_pitch) of the half layout.
+__device__ __forceinline__ int thth_ncols(const ThthGeom& g) {
+    return (int)(g.cs_half ? g.nfd / 2 + 1 : g.nfd);
+}
+
+// Stored CS column of the pair (th1 = theta of the column, th2 = theta of the row): the fd
+// bin of thth_point with python's wrap of a negative index, then, in the half layout, the
+// stored column of that bin; *mirrored is set when the bin lies in the fd < 0 half
+// (CS[-tau, -fd] = conj(CS[tau, fd]): the row is mirrored and the value conjugated).
+// Returns -1 where the pnts mask / IndexError rule out the point for every curvature,
+// otherwise a column in [0, thth_ncols(g)).  The curvature-sweep gather and the table of
+// reached columns (thth_colmark_kernel) both call this, so they cannot disagree.
+__device__ __forceinline__ int thth_pair_column(const ThthGeom& g, double th1, double th2,
+                                                bool* mirrored) {
+    *mirrored = false;
+    const double bb = __dadd_rn(__dsub_rn(__dsub_rn(th1, th2), g.fd0), g.half_dfd);
+    const double fqd = floor_div_fast(bb, g.dfd, g.inv_dfd);
+    const long long fq = (fqd == fqd && fabs(fqd) < 9.0e18) ? (long long)fqd : LLONG_MIN;
+    if (!(fq < g.nfd && !(fq < -g.nfd))) return -1;     // pnts mask / IndexError (thth_point)
+    const long long fi = fq < 0 ? fq + g.nfd : fq;
+    if (!g.cs_half) return (int)fi;
+    const long long hfd = g.nfd / 2;
+    if (fi >= hfd) return (int)(fi - hfd);
+    if (fi == 0) return (int)hfd;
+    *mirrored = true;
+    return (int)(hfd - fi);
+}
+
+// Compact copy of the spectrum columns a theta grid reaches, delay axis contiguous:
+// element (row r, stored column c) of the spectrum is base[slot_of_col[c] * tau_pitch + r];
+// slot_of_col[c] < 0 marks a column the copy does not hold.  base == null: no copy was
+// made, the sweep gathers from the spectrum itself (thth_gather_source, thth.cu).
+struct ThthCopy {
+    const float2* base;
+    long long tau_pitch;
+    int nslots;
+    const int* slot_of_col;
+    int* err;              // device word, set non-zero by a gather that meets slot < 0
+};
 
 // Gathered, Jacobian-weighted value before the Hermitian fill
 // (ththmod.py:104,107).  Negative fd_inv wraps like python indexing.
