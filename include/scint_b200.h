@@ -48,7 +48,8 @@ int sb_release(void);
 
 /* Per-kernel timing with CUDA events recorded on the launching stream.
  * Slots: 0 cs_rows 1 cs_colA 2 cs_colB 3 thth_prep 4 thth_build 5 thth_eig
- * 6 sspec 7 acf 8 sim_screen 9 sim_freq.  sb_profile_collect synchronises the
+ * 6 sspec 7 acf 8 sim_screen 9 sim_freq 10 mosaic_tile 11 mosaic_reduce.
+ * sb_profile_collect synchronises the
  * device, writes accumulated milliseconds and launch counts (host arrays of
  * at least 16 entries) and resets the accumulators. */
 /* number of kernels this library has launched so far in this process */
@@ -378,6 +379,55 @@ int sb_vlbi_retrieval(const sb_thth_geom* geom, const void* const* cs_list_host,
 int sb_asymmetry_batch(const sb_thth_geom* geoms_host, int32_t nchunk, const double* etas,
                        double tol, int32_t max_iter, double* asym, double* w, int32_t* status,
                        int32_t* nred, int32_t* iters, void* v, void* stream);
+
+/* ---- wavefield mosaic ---------------------------------------------------- */
+
+/* ththmod.rotMos / rotFit / rotDer / rotInit and fullMos / fullMosFit /
+ * fullMosGrad / fullMosHess (:1708-2310) for ncf x nct half-overlapping chunks
+ * of cwf x cwt: chunks float2 [ncf*nct][cwf][cwt], chunk k = cf*nct + ct covers
+ * mosaic rows cf*(cwf/2) .. +cwf and columns ct*(cwt/2) .. +cwt, weighted by the
+ * separable sin^2 ramps of mask_func.  The mosaic is nF x nT =
+ * ((ncf-1)*(cwf/2)+cwf) x ((nct-1)*(cwt/2)+cwt).  phi: device float64 [P]
+ * phases per chunk (phi[0] is the first chunk's, 0 in the reference); amp:
+ * device float64 [P] amplitudes or NULL (ones, sb_mosaic_build only).  e^{i phi}
+ * is formed in float64 per chunk; pixels are float32 arithmetic, every sum is
+ * accumulated in float64 in a fixed order (results are deterministic).
+ * Limits, checked before any workspace is allocated: an axis with more than one
+ * chunk needs an even width (SB_ERR_ARG); half-tile extents (cwf/2, or cwf for a
+ * single chunk; the same in time) <= 2048, mosaic sides < 2^31 and fewer than
+ * 2^28 chunks (SB_ERR_UNSUPPORTED). */
+
+/* wavefield float2 [nF][nT] = sum_k amp_k e^{i phi_k} mask_k chunk_k */
+int sb_mosaic_build(const void* chunks, int32_t ncf, int32_t nct, int32_t cwf, int32_t cwt,
+                    const double* phi, const double* amp, void* wavefield, void* stream);
+/* from the wavefield sb_mosaic_build made with the same phi and amp = NULL:
+ * power float64 [1] = sum |W|^2 (rotFit = -power), der float64 [P] with
+ * der[k] = 2 sum Im(conj(W) e^{i phi_k} mask_k chunk_k) (rotDer[k-1] = der[k]).
+ * NaN propagates. */
+int sb_mosaic_rot(const void* chunks, int32_t ncf, int32_t nct, int32_t cwf, int32_t cwt,
+                  const double* phi, const void* wavefield, double* power, double* der,
+                  void* stream);
+/* overlap float64 complex [P][4]: overlap[k][e] = sum over the overlap of
+ * mask_j chunk_j conj(mask_k chunk_k) with the earlier neighbour j of chunk
+ * (cf, ct) at e = 0 (cf-1, ct-1), 1 (cf-1, ct), 2 (cf-1, ct+1), 3 (cf, ct-1);
+ * 0 where there is none.  rotInit is then rot_k = angle(sum_e e^{i rot_j} overlap[k][e]). */
+int sb_mosaic_overlap(const void* chunks, int32_t ncf, int32_t nct, int32_t cwf, int32_t cwt,
+                      double* overlap, void* stream);
+/* from the wavefield sb_mosaic_build made with the same phi and amp, dspec and
+ * noise float32 [nF][nT]: fit float64 [1] = sum ((|W|^2 - dspec) / noise)^2 and
+ * grad float64 [P][2] = (d fit / d amp_k, d fit / d phi_k), NaN terms skipped
+ * (numpy nansum; a complex gradient term is skipped if either part is NaN). */
+int sb_mosaic_fit(const void* chunks, int32_t ncf, int32_t nct, int32_t cwf, int32_t cwt,
+                  const double* phi, const double* amp, const void* wavefield, const float* dspec,
+                  const float* noise, double* fit, double* grad, void* stream);
+/* Hessian of that fit as COO triplets, 8 per (chunk, forward neighbour) slot,
+ * rows / cols int64 and vals float64 of 40 P entries each.  Parameter index
+ * of phi_k is k-1 (k >= 1), of amp_k is k+P-1 (fullMosHess's p layout); every
+ * (row, col) appears at most once; unused slots have row = col = -1.  Sums
+ * over each pair's overlap; NaN propagates (numpy sum). */
+int sb_mosaic_hess(const void* chunks, int32_t ncf, int32_t nct, int32_t cwf, int32_t cwt,
+                   const double* phi, const double* amp, const void* wavefield, const float* dspec,
+                   const float* noise, int64_t* rows, int64_t* cols, double* vals, void* stream);
 
 /* ---- scint_sim.Simulation ------------------------------------------------ */
 

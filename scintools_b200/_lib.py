@@ -87,6 +87,12 @@ _SIGS = {
                                   c_int, c_int, c_dbl, c_int, vp, vp, vp, vp, vp]),
     "sb_asymmetry_batch": (c_int, [ctypes.POINTER(ThthGeom), c_int, vp, c_dbl, c_int, vp, vp, vp,
                                    vp, vp, vp, vp]),
+    "sb_mosaic_build": (c_int, [vp, c_int, c_int, c_int, c_int, vp, vp, vp, vp]),
+    "sb_mosaic_rot": (c_int, [vp, c_int, c_int, c_int, c_int, vp, vp, vp, vp, vp]),
+    "sb_mosaic_overlap": (c_int, [vp, c_int, c_int, c_int, c_int, vp, vp]),
+    "sb_mosaic_fit": (c_int, [vp, c_int, c_int, c_int, c_int, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "sb_mosaic_hess": (c_int, [vp, c_int, c_int, c_int, c_int, vp, vp, vp, vp, vp, vp, vp, vp,
+                               vp]),
     "sb_sim_weights": (c_int, [ctypes.POINTER(SimParams), vp, vp]),
     "sb_sim_screen": (c_int, [c_int, c_int, vp, vp, vp, ctypes.c_uint64, vp, vp]),
     "sb_sim_intensity": (c_int, [c_int, c_int, c_int, vp, vp, c_dbl, c_dbl, vp,

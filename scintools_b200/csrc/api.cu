@@ -161,6 +161,19 @@ int asymmetry_batch(const ThthGeom* geoms, const double* const* th_host, int nch
                     const double* d_etas, double tol, int max_iter, double* d_asym, double* d_w,
                     int* d_status, int* d_nred, int* d_iters, float2* d_v, cudaStream_t st);
 
+int mosaic_build(const float2* chunks, int ncf, int nct, int cwf, int cwt, const double* phi,
+                 const double* amp, float2* W, cudaStream_t st);
+int mosaic_rot(const float2* chunks, int ncf, int nct, int cwf, int cwt, const double* phi,
+               const float2* W, double* power, double* der, cudaStream_t st);
+int mosaic_overlap(const float2* chunks, int ncf, int nct, int cwf, int cwt, double* C,
+                   cudaStream_t st);
+int mosaic_fit(const float2* chunks, int ncf, int nct, int cwf, int cwt, const double* phi,
+               const double* amp, const float2* W, const float* dspec, const float* noise,
+               double* fit, double* grad, cudaStream_t st);
+int mosaic_hess(const float2* chunks, int ncf, int nct, int cwf, int cwt, const double* phi,
+                const double* amp, const float2* W, const float* dspec, const float* noise,
+                long long* rows, long long* cols, double* vals, cudaStream_t st);
+
 int gerchberg_saxton(float2* W, const float* amp, const unsigned char* rowmask, int n0, int n1,
                      int niter, cudaStream_t st);
 
@@ -208,7 +221,7 @@ static int to_geom(const sb_thth_geom* in, ThthGeom* g) {
 
 extern "C" {
 
-int sb_abi_version(void) { return 5; }
+int sb_abi_version(void) { return 6; }
 const char* sb_last_error(void) { return sb::last_error(); }
 
 int sb_init(int device) {
@@ -460,6 +473,45 @@ int sb_asymmetry_batch(const sb_thth_geom* geoms_host, int32_t nchunk, const dou
     }
     return sb::asymmetry_batch(g.data(), th.data(), nchunk, etas, tol, max_iter, asym, w, status,
                                nred, iters, (float2*)v, (cudaStream_t)stream);
+}
+
+int sb_mosaic_build(const void* chunks, int32_t ncf, int32_t nct, int32_t cwf, int32_t cwt,
+                    const double* phi, const double* amp, void* wavefield, void* stream) {
+    SB_ARG(chunks && phi && wavefield);
+    return sb::mosaic_build((const float2*)chunks, ncf, nct, cwf, cwt, phi, amp,
+                            (float2*)wavefield, (cudaStream_t)stream);
+}
+
+int sb_mosaic_rot(const void* chunks, int32_t ncf, int32_t nct, int32_t cwf, int32_t cwt,
+                  const double* phi, const void* wavefield, double* power, double* der,
+                  void* stream) {
+    SB_ARG(chunks && phi && wavefield && power && der);
+    return sb::mosaic_rot((const float2*)chunks, ncf, nct, cwf, cwt, phi, (const float2*)wavefield,
+                          power, der, (cudaStream_t)stream);
+}
+
+int sb_mosaic_overlap(const void* chunks, int32_t ncf, int32_t nct, int32_t cwf, int32_t cwt,
+                      double* overlap, void* stream) {
+    SB_ARG(chunks && overlap);
+    return sb::mosaic_overlap((const float2*)chunks, ncf, nct, cwf, cwt, overlap,
+                              (cudaStream_t)stream);
+}
+
+int sb_mosaic_fit(const void* chunks, int32_t ncf, int32_t nct, int32_t cwf, int32_t cwt,
+                  const double* phi, const double* amp, const void* wavefield, const float* dspec,
+                  const float* noise, double* fit, double* grad, void* stream) {
+    SB_ARG(chunks && phi && amp && wavefield && dspec && noise && fit && grad);
+    return sb::mosaic_fit((const float2*)chunks, ncf, nct, cwf, cwt, phi, amp,
+                          (const float2*)wavefield, dspec, noise, fit, grad, (cudaStream_t)stream);
+}
+
+int sb_mosaic_hess(const void* chunks, int32_t ncf, int32_t nct, int32_t cwf, int32_t cwt,
+                   const double* phi, const double* amp, const void* wavefield, const float* dspec,
+                   const float* noise, int64_t* rows, int64_t* cols, double* vals, void* stream) {
+    SB_ARG(chunks && phi && amp && wavefield && dspec && noise && rows && cols && vals);
+    return sb::mosaic_hess((const float2*)chunks, ncf, nct, cwf, cwt, phi, amp,
+                           (const float2*)wavefield, dspec, noise, (long long*)rows,
+                           (long long*)cols, vals, (cudaStream_t)stream);
 }
 
 int sb_sim_weights(const sb_sim_params* p, double* w, void* stream) {

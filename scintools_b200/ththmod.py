@@ -16,6 +16,9 @@ Same function names, argument order and failure behaviour as the reference
                  sb_vlbi_retrieval (host: rev_map centres, input checks)
   calc_asymmetry ththmod.py:2385-2463 -> sb_cs_f32 + sb_asymmetry_batch (one chunk)
   asymmetry_batch the chunk loop of Dynspec.calc_asymmetry (batched per padded shape)
+  rotInit, rotMos, rotFit, rotDer, fullMos, fullMosFit, fullMosGrad, fullMosHess
+                 ththmod.py:1708-2310 -> sb_mosaic_* (MosaicModel keeps the chunks
+                 resident; rotInit's scalar recurrence runs on the host)
   min_edges      ththmod.py:1671-1705 (host)
   chi_par        ththmod.py:38-53     (host)
 
@@ -1183,3 +1186,286 @@ def min_edges(fd_lim, fd, tau, eta, factor=2):
     return U.wrap(np.linspace(-fd_lim_v, fd_lim_v, int(npoints)), "mHz",
                   like=fd_lim)
 
+
+
+class MosaicModel:
+    """The chunks [ncf][nct][cwf][cwt] uploaded once (complex64) for the mosaic fit of
+    ththmod.py:1708-2310, on the device (sb_mosaic_*).
+
+    ``rot_init()``, ``rot_mos(x)``, ``rot_fit(x)``, ``rot_der(x)`` take the phase of every
+    chunk after the first; ``full_mos(p)``, ``fit(p)``, ``grad(p)``, ``hess(p, sparse=False)``
+    take p = (those phases, then one amplitude per chunk).  Entries past them are ignored
+    (their gradient and Hessian rows are zero); a shorter vector raises IndexError.  The
+    last wavefield and the last fit / gradient are cached per parameter vector, so ``fit``,
+    ``grad`` and ``hess`` at one p (as scipy.optimize.minimize calls them) build the
+    mosaic once.  ``dspec`` and ``N`` (noise standard deviation) are cropped to the mosaic
+    shape and must be at least that large.  fit and grad skip NaN terms (nansum);
+    rot_fit, rot_der and hess let NaN propagate.  Pixels are float32 arithmetic with
+    float64 sums; ``hess(sparse=True)`` gives a scipy.sparse.csr_matrix."""
+
+    def __init__(self, chunks, dspec=None, N=None):
+        ch = np.asarray(chunks)
+        if ch.ndim != 4:
+            raise ValueError("chunks must be 4-D [ncf][nct][cwf][cwt], got shape %r" % (ch.shape,))
+        ncf, nct, cwf, cwt = (int(n) for n in ch.shape)
+        _check_widths(ch.shape)
+        hf, ht = (cwf // 2 if ncf > 1 else cwf), (cwt // 2 if nct > 1 else cwt)
+        if min(ncf, nct, cwf, cwt) < 1 or hf > 2048 or ht > 2048 or ncf * nct >= 2 ** 28:
+            raise _lib.SbError("mosaic: %d x %d chunks of %d x %d outside the supported "
+                               "geometry (half-chunk extent <= 2048, fewer than 2^28 chunks)"
+                               % (ncf, nct, cwf, cwt))
+        self.dims = (ncf, nct, cwf, cwt)
+        self.P = ncf * nct
+        self.shape = ((ncf - 1) * (cwf // 2) + cwf, (nct - 1) * (cwt // 2) + cwt)
+        if dspec is not None or N is not None:
+            dspec, N = self._crop(dspec, "dspec"), self._crop(N, "N")
+        self._ch = D.upload(ch.astype(np.complex64, copy=False))
+        self._D = None if dspec is None else D.upload(dspec)
+        self._N = None if N is None else D.upload(N)
+        import torch
+        self._W = D.empty(self.shape + (2,), torch.float32)
+        self._wkey = None
+        self._fkey = self._rkey = None
+
+    def _crop(self, a, name):
+        if a is None:
+            raise ValueError("MosaicModel: dspec and N are needed together")
+        a = np.asarray(a)
+        nF, nT = self.shape
+        if a.ndim != 2 or a.shape[0] < nF or a.shape[1] < nT:
+            raise ValueError("%s of shape %r is smaller than the mosaic %r" % (name, a.shape, self.shape))
+        return np.ascontiguousarray(a[:nF, :nT], dtype=np.float32)
+
+    def _params(self, p, with_amp):
+        p = np.asarray(p, dtype=np.float64)
+        need = 2 * self.P - 1 if with_amp else self.P - 1
+        if p.ndim != 1 or p.shape[0] < need:
+            raise IndexError("parameter vector of length %d; %d chunks need %d"
+                             % (p.shape[0] if p.ndim else 0, self.P, need))
+        phi = np.concatenate([[0.0], p[:self.P - 1]])
+        amp = p[self.P - 1:2 * self.P - 1].copy() if with_amp else None
+        return p, phi, amp
+
+    def _build(self, phi, amp):
+        key = (phi.tobytes(), None if amp is None else amp.tobytes())
+        if key != self._wkey:
+            self._dphi = D.upload(phi)
+            self._damp = None if amp is None else D.upload(amp)
+            ncf, nct, cwf, cwt = self.dims
+            _lib.check(_lib.lib.sb_mosaic_build(self._ch.data_ptr(), ncf, nct, cwf, cwt,
+                                                self._dphi.data_ptr(), D.ptr(self._damp),
+                                                self._W.data_ptr(), D.stream_ptr()))
+            self._wkey = key
+            self._fkey = self._rkey = None
+
+    def _wave(self):
+        a = self._W.cpu().numpy()
+        return (a[..., 0] + 1j * a[..., 1]).astype(np.complex128)
+
+    def rot_init(self):
+        """Phase of every chunk after the first that stacks it coherently onto the chunks
+        before it (ththmod.py:1791-1856).  The device sums each chunk's overlap with its
+        (at most four) earlier neighbours; the recurrence rot_k = angle(sum_j e^{i rot_j}
+        C_kj) runs on the host in float64.  A chunk whose sum is exactly zero (an all-zero
+        chunk) gets 0, where the reference returns the angle of a signed zero (0 or +-pi);
+        such a chunk adds nothing to the mosaic either way."""
+        import cmath
+        import torch
+        ncf, nct, cwf, cwt = self.dims
+        C = D.empty((self.P, 4, 2), torch.float64)
+        _lib.check(_lib.lib.sb_mosaic_overlap(self._ch.data_ptr(), ncf, nct, cwf, cwt,
+                                              C.data_ptr(), D.stream_ptr()))
+        c = C.cpu().numpy()
+        c = (c[..., 0] + 1j * c[..., 1]).tolist()
+        rot = [0.0] * self.P
+        for k in range(1, self.P):
+            cf, ct = divmod(k, nct)
+            s = 0j
+            for e, (jf, jt) in enumerate(((cf - 1, ct - 1), (cf - 1, ct), (cf - 1, ct + 1),
+                                          (cf, ct - 1))):
+                if jf >= 0 and 0 <= jt < nct:
+                    s += cmath.exp(1j * rot[jf * nct + jt]) * c[k][e]
+            rot[k] = cmath.phase(s) if s != 0 else 0.0
+        return np.array(rot[1:])
+
+    def rot_mos(self, x):
+        """ththmod.rotMos (:1708-1770): complex128 mosaic with phases x."""
+        _, phi, _ = self._params(x, False)
+        self._build(phi, None)
+        return self._wave()
+
+    def _rot(self, x):
+        import torch
+        x, phi, _ = self._params(x, False)
+        self._build(phi, None)
+        if self._rkey is None:
+            ncf, nct, cwf, cwt = self.dims
+            out = D.empty((self.P + 1,), torch.float64)
+            _lib.check(_lib.lib.sb_mosaic_rot(self._ch.data_ptr(), ncf, nct, cwf, cwt,
+                                              self._dphi.data_ptr(), self._W.data_ptr(),
+                                              out.data_ptr(), out.data_ptr() + 8,
+                                              D.stream_ptr()))
+            self._rkey = out.cpu().numpy()
+        return x, self._rkey
+
+    def rot_fit(self, x):
+        """ththmod.rotFit (:1773-1788): -sum |rotMos(x)|^2 (NaN propagates)."""
+        return float(-self._rot(x)[1][0])
+
+    def rot_der(self, x):
+        """ththmod.rotDer (:1859-1919): d rotFit / d x, shaped like x."""
+        x, r = self._rot(x)
+        out = np.zeros(x.shape)
+        out[:self.P - 1] = r[2:]
+        return out
+
+    def full_mos(self, p):
+        """ththmod.fullMos (:1922-1987): complex128 mosaic with phases and amplitudes p."""
+        _, phi, amp = self._params(p, True)
+        self._build(phi, amp)
+        return self._wave()
+
+    def _need_data(self):
+        if self._D is None:
+            raise ValueError("MosaicModel: fit / grad / hess need dspec and N")
+
+    def _fit(self, p):
+        import torch
+        p, phi, amp = self._params(p, True)
+        self._need_data()
+        self._build(phi, amp)
+        if self._fkey is None:
+            ncf, nct, cwf, cwt = self.dims
+            out = D.empty((2 * self.P + 1,), torch.float64)
+            _lib.check(_lib.lib.sb_mosaic_fit(self._ch.data_ptr(), ncf, nct, cwf, cwt,
+                                              self._dphi.data_ptr(), self._damp.data_ptr(),
+                                              self._W.data_ptr(), self._D.data_ptr(),
+                                              self._N.data_ptr(), out.data_ptr(),
+                                              out.data_ptr() + 8, D.stream_ptr()))
+            self._fkey = out.cpu().numpy()
+        return p, self._fkey
+
+    def fit(self, p):
+        """ththmod.fullMosFit (:1990-2016): nansum(((|W|^2 - dspec) / N)^2)."""
+        return float(self._fit(p)[1][0])
+
+    def grad(self, p):
+        """ththmod.fullMosGrad (:2019-2102): gradient of fit, length len(p)."""
+        p, r = self._fit(p)
+        g = r[1:].reshape(self.P, 2)
+        out = np.zeros(p.shape[0])
+        out[self.P - 1:2 * self.P - 1] = g[:, 0]
+        out[:self.P - 1] = g[1:, 1]
+        return out
+
+    def hess(self, p, sparse=False):
+        """ththmod.fullMosHess (:2105-2310): Hessian of fit, (len(p), len(p)); from the
+        sums over each pair of neighbouring chunks.  NaN propagates."""
+        import torch
+        p, phi, amp = self._params(p, True)
+        self._need_data()
+        self._build(phi, amp)
+        ncf, nct, cwf, cwt = self.dims
+        n = 40 * self.P
+        rows, cols = D.empty((n,), torch.int64), D.empty((n,), torch.int64)
+        vals = D.empty((n,), torch.float64)
+        _lib.check(_lib.lib.sb_mosaic_hess(self._ch.data_ptr(), ncf, nct, cwf, cwt,
+                                           self._dphi.data_ptr(), self._damp.data_ptr(),
+                                           self._W.data_ptr(), self._D.data_ptr(),
+                                           self._N.data_ptr(), rows.data_ptr(), cols.data_ptr(),
+                                           vals.data_ptr(), D.stream_ptr()))
+        r, c, v = rows.cpu().numpy(), cols.cpu().numpy(), vals.cpu().numpy()
+        keep = r >= 0
+        r, c, v = r[keep], c[keep], v[keep]
+        m = p.shape[0]
+        if sparse:
+            from scipy.sparse import csr_matrix
+            return csr_matrix((v, (r, c)), shape=(m, m))
+        H = np.zeros((m, m))
+        H[r, c] = v
+        return H
+
+
+def _check_widths(shape):
+    """The reference's ramps broadcast only onto even halves: an axis with more than one
+    chunk needs an even width (ValueError otherwise, as in the reference)."""
+    ncf, nct, cwf, cwt = shape
+    if (ncf > 1 and cwf % 2) or (nct > 1 and cwt % 2):
+        raise ValueError("chunk width %d x %d: an axis with more than one chunk needs an "
+                         "even width" % (cwf, cwt))
+
+
+def _grad_data(chunks, dspec, N):
+    """fullMosGrad / fullMosHess index dspec with the mosaic's shape exactly and N by
+    slices of it: dspec must be the mosaic's shape, N at least that."""
+    ch = np.asarray(chunks)
+    if ch.ndim == 4:
+        _check_widths(ch.shape)
+        ncf, nct, cwf, cwt = ch.shape
+        shape = ((ncf - 1) * (cwf // 2) + cwf, (nct - 1) * (cwt // 2) + cwt)
+        if np.shape(dspec) != shape:
+            raise ValueError("dspec of shape %r does not match the mosaic %r"
+                             % (np.shape(dspec), shape))
+        if np.ndim(N) != 2 or np.shape(N)[0] < shape[0] or np.shape(N)[1] < shape[1]:
+            raise ValueError("N of shape %r is smaller than the mosaic %r" % (np.shape(N), shape))
+
+
+def _check_p(chunks, p, with_amp):
+    ch = np.asarray(chunks)
+    P = ch.shape[0] * ch.shape[1] if ch.ndim == 4 else 0
+    need = 2 * P - 1 if with_amp else P - 1
+    if np.ndim(p) != 1 or np.shape(p)[0] < need:
+        raise IndexError("parameter vector of length %d; %d chunks need %d"
+                         % (np.size(p), P, need))
+
+
+def rotInit(chunks):
+    """ththmod.rotInit (ththmod.py:1791-1856) on the device; see MosaicModel.rot_init."""
+    return MosaicModel(chunks).rot_init()
+
+
+def rotMos(chunks, x):
+    """ththmod.rotMos (ththmod.py:1708-1770) on the device."""
+    _check_p(chunks, x, False)
+    return MosaicModel(chunks).rot_mos(x)
+
+
+def rotFit(x, chunks):
+    """ththmod.rotFit (ththmod.py:1773-1788) on the device."""
+    _check_p(chunks, x, False)
+    return MosaicModel(chunks).rot_fit(x)
+
+
+def rotDer(x, chunks):
+    """ththmod.rotDer (ththmod.py:1859-1919) on the device."""
+    _check_p(chunks, x, False)
+    return MosaicModel(chunks).rot_der(x)
+
+
+def fullMos(chunks, p):
+    """ththmod.fullMos (ththmod.py:1922-1987) on the device."""
+    _check_p(chunks, p, True)
+    return MosaicModel(chunks).full_mos(p)
+
+
+def fullMosFit(p, chunks, dspec, N):
+    """ththmod.fullMosFit (ththmod.py:1990-2016) on the device; dspec and N are cropped
+    to the mosaic."""
+    _check_p(chunks, p, True)
+    return MosaicModel(chunks, dspec, N).fit(p)
+
+
+def fullMosGrad(p, chunks, dspec, N):
+    """ththmod.fullMosGrad (ththmod.py:2019-2102) on the device; dspec must have the
+    mosaic's shape and N at least that."""
+    _check_p(chunks, p, True)
+    _grad_data(chunks, dspec, N)
+    return MosaicModel(chunks, dspec, N).grad(p)
+
+
+def fullMosHess(p, chunks, dspec, N):
+    """ththmod.fullMosHess (ththmod.py:2105-2310) on the device, dense (len(p), len(p));
+    dspec must have the mosaic's shape and N at least that."""
+    _check_p(chunks, p, True)
+    _grad_data(chunks, dspec, N)
+    return MosaicModel(chunks, dspec, N).hess(p)
