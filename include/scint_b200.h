@@ -48,7 +48,8 @@ int sb_release(void);
 
 /* Per-kernel timing with CUDA events recorded on the launching stream.
  * Slots: 0 cs_rows 1 cs_colA 2 cs_colB 3 thth_prep 4 thth_build 5 thth_eig
- * 6 sspec 7 acf 8 sim_screen 9 sim_freq 10 mosaic_tile 11 mosaic_reduce.
+ * 6 sspec 7 acf 8 sim_screen 9 sim_freq 10 mosaic_tile 11 mosaic_reduce
+ * 12 svd_gram (one A^T A pass of sb_svd_topk) 13 svd_apply.
  * sb_profile_collect synchronises the
  * device, writes accumulated milliseconds and launch counts (host arrays of
  * at least 16 entries) and resets the accumulators. */
@@ -428,6 +429,39 @@ int sb_mosaic_fit(const void* chunks, int32_t ncf, int32_t nct, int32_t cwf, int
 int sb_mosaic_hess(const void* chunks, int32_t ncf, int32_t nct, int32_t cwf, int32_t cwt,
                    const double* phi, const double* amp, const void* wavefield, const float* dspec,
                    const float* noise, int64_t* rows, int64_t* cols, double* vals, void* stream);
+
+/* ---- flux-variation correction ------------------------------------------ */
+
+/* Dynspec.correct_dyn (dynspec.py:3325-3410) and svd_model (scint_utils.py:705-729,
+ * ththmod.py:18-35).  A: device float32 [nf][nt], NaN read as 0.  Shapes: 1 <= nf <=
+ * 32768, 1 <= nt <= 16384, else SB_ERR_UNSUPPORTED; 1 <= k <= 32, else SB_ERR_ARG.
+ * Every sum is float64 in a fixed order: repeated calls are bit-identical. */
+
+/* Top-k right singular vectors of A: Lanczos on A^T A in float64 with full
+ * re-orthogonalisation, one read of A per step, then one more read per mode for the true
+ * residual (stopping rule in csrc/svd.cu).  Synchronous.  V: device float64 [k][nt]
+ * (orthonormal; rows past the numerical rank are zero).  s_host [k]: singular values,
+ * descending; res_host [k]: ||A^T A v_j - s_j^2 v_j||_2; gap_host [1]: the lower bound
+ * theta_k - theta_{k+1} - r_{k+1} on the eigenvalue gap of A^T A the rule used (0 when the
+ * iteration ended with at most k Ritz values); info_host int32 [4]: Lanczos steps,
+ * converged (0/1), tie at the truncation boundary (0/1), exact breakdown (0/1). */
+int sb_svd_topk(const float* A, int32_t nf, int32_t nt, int32_t k, double* V, double* s_host,
+                double* res_host, double* gap_host, int32_t* info_host, void* stream);
+/* Final pass, one read of A: model_ij = sum_j (a_i . v_j) v_j and out_ij = a_ij / |model_ij|
+ * (float64, rounded once; 0/0 -> NaN, a/0 -> inf).  out or model may be NULL (not both). */
+int sb_svd_apply(const float* A, int32_t nf, int32_t nt, int32_t k, const double* V, float* out,
+                 float* model, void* stream);
+/* svd=False passes.  A value is NaN if zero_as_nan and it is 0 (the host decides, from
+ * whether the array is Dynspec.dyn itself); means skip NaN (numpy nanmean, NaN when no
+ * value is left).  rows: mean float64 [nf] over each row.  cols: mean float64 [nt] over
+ * each column of value / rowdiv[i] (rowdiv float64 [nf] or NULL).  divide: out float32
+ * [nf][nt] = (value / rowdiv[i]) / coldiv[j] in float64 (either NULL: skipped). */
+int sb_bandpass_rows(const float* A, int32_t nf, int32_t nt, int32_t zero_as_nan, double* mean,
+                     void* stream);
+int sb_bandpass_cols(const float* A, int32_t nf, int32_t nt, int32_t zero_as_nan,
+                     const double* rowdiv, double* mean, void* stream);
+int sb_bandpass_divide(const float* A, int32_t nf, int32_t nt, int32_t zero_as_nan,
+                       const double* rowdiv, const double* coldiv, float* out, void* stream);
 
 /* ---- scint_sim.Simulation ------------------------------------------------ */
 

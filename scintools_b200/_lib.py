@@ -93,6 +93,11 @@ _SIGS = {
     "sb_mosaic_fit": (c_int, [vp, c_int, c_int, c_int, c_int, vp, vp, vp, vp, vp, vp, vp, vp]),
     "sb_mosaic_hess": (c_int, [vp, c_int, c_int, c_int, c_int, vp, vp, vp, vp, vp, vp, vp, vp,
                                vp]),
+    "sb_svd_topk": (c_int, [vp, c_int, c_int, c_int, vp, vp, vp, vp, vp, vp]),
+    "sb_svd_apply": (c_int, [vp, c_int, c_int, c_int, vp, vp, vp, vp]),
+    "sb_bandpass_rows": (c_int, [vp, c_int, c_int, c_int, vp, vp]),
+    "sb_bandpass_cols": (c_int, [vp, c_int, c_int, c_int, vp, vp, vp]),
+    "sb_bandpass_divide": (c_int, [vp, c_int, c_int, c_int, vp, vp, vp, vp]),
     "sb_sim_weights": (c_int, [ctypes.POINTER(SimParams), vp, vp]),
     "sb_sim_screen": (c_int, [c_int, c_int, vp, vp, vp, ctypes.c_uint64, vp, vp]),
     "sb_sim_intensity": (c_int, [c_int, c_int, c_int, vp, vp, c_dbl, c_dbl, vp,

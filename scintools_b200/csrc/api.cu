@@ -174,6 +174,16 @@ int mosaic_hess(const float2* chunks, int ncf, int nct, int cwf, int cwt, const 
                 const double* amp, const float2* W, const float* dspec, const float* noise,
                 long long* rows, long long* cols, double* vals, cudaStream_t st);
 
+int svd_topk(const float* A, int nf, int nt, int k, double* Y, double* s_host, double* res_host,
+             double* gap_host, int* info_host, cudaStream_t st);
+int svd_apply(const float* A, int nf, int nt, int k, const double* Y, float* out, float* model,
+              cudaStream_t st);
+int bandpass_rows(const float* A, int nf, int nt, int zero_as_nan, double* mean, cudaStream_t st);
+int bandpass_cols(const float* A, int nf, int nt, int zero_as_nan, const double* rowdiv,
+                  double* mean, cudaStream_t st);
+int bandpass_divide(const float* A, int nf, int nt, int zero_as_nan, const double* rowdiv,
+                    const double* coldiv, float* out, cudaStream_t st);
+
 int gerchberg_saxton(float2* W, const float* amp, const unsigned char* rowmask, int n0, int n1,
                      int niter, cudaStream_t st);
 
@@ -221,7 +231,7 @@ static int to_geom(const sb_thth_geom* in, ThthGeom* g) {
 
 extern "C" {
 
-int sb_abi_version(void) { return 6; }
+int sb_abi_version(void) { return 7; }
 const char* sb_last_error(void) { return sb::last_error(); }
 
 int sb_init(int device) {
@@ -532,6 +542,32 @@ int sb_sim_intensity(int32_t nx, int32_t ny, int32_t nf, const double* xyp,
     SB_ARG(xyp && scales_host && spe_t && nf >= 1);
     return sb::sim_intensity(nx, ny, nf, xyp, scales_host, ffconx, ffcony,
                              (float2*)spe_t, xyi, (cudaStream_t)stream);
+}
+
+int sb_svd_topk(const float* A, int32_t nf, int32_t nt, int32_t k, double* V, double* s_host,
+                double* res_host, double* gap_host, int32_t* info_host, void* stream) {
+    return sb::svd_topk(A, nf, nt, k, V, s_host, res_host, gap_host, info_host,
+                        (cudaStream_t)stream);
+}
+
+int sb_svd_apply(const float* A, int32_t nf, int32_t nt, int32_t k, const double* V, float* out,
+                 float* model, void* stream) {
+    return sb::svd_apply(A, nf, nt, k, V, out, model, (cudaStream_t)stream);
+}
+
+int sb_bandpass_rows(const float* A, int32_t nf, int32_t nt, int32_t zero_as_nan, double* mean,
+                     void* stream) {
+    return sb::bandpass_rows(A, nf, nt, zero_as_nan, mean, (cudaStream_t)stream);
+}
+
+int sb_bandpass_cols(const float* A, int32_t nf, int32_t nt, int32_t zero_as_nan,
+                     const double* rowdiv, double* mean, void* stream) {
+    return sb::bandpass_cols(A, nf, nt, zero_as_nan, rowdiv, mean, (cudaStream_t)stream);
+}
+
+int sb_bandpass_divide(const float* A, int32_t nf, int32_t nt, int32_t zero_as_nan,
+                       const double* rowdiv, const double* coldiv, float* out, void* stream) {
+    return sb::bandpass_divide(A, nf, nt, zero_as_nan, rowdiv, coldiv, out, (cudaStream_t)stream);
 }
 
 int sb_convert_f64_f32(const double* src, float* dst, int64_t n, void* stream) {

@@ -14,7 +14,8 @@ lmfit models) is deliberately not here: use the reference for those and hand
 the arrays over with ``BasicDyn`` exactly as the reference's tutorials do.
 Units: times in s, freqs in MHz, eta in s^3, edges in mHz, tau in us.
 
-Also here: scale_dyn('lambda') (dynspec.py:3926-3957 -> sb_scale_dyn_lambda_f32),
+Also here: correct_dyn (dynspec.py:3325-3410 -> sb_svd_topk + sb_svd_apply, or the
+sb_bandpass_* passes), scale_dyn('lambda') (dynspec.py:3926-3957 -> sb_scale_dyn_lambda_f32),
 thetatheta_chunks / calc_wavefield / gerchberg_saxton (:1765-1896), and, through
 ``arcfit.ArcFitMixin``, norm_sspec / fit_arc (:1920-2183, :970-1346).
 
@@ -125,6 +126,93 @@ class Dynspec(ArcFitMixin):
             self.calc_sspec(lamsteps=lamsteps)
         if verbose:
             print("LOADED DYNSPEC OBJECT {0}".format(self.name))
+
+    # ------------------------------------------------------------------
+    # flux-variation correction (csrc/svd.cu)
+    # ------------------------------------------------------------------
+    def correct_dyn(self, svd=True, nmodes=1, frequency=True, time=True,
+                    lamsteps=False, nsmooth=None, velocity=False, dtype=np.float64):
+        """Correct for flux variations in time and frequency (reference
+        dynspec.py:3325-3410), with the reference's side effects:
+
+        - the array is self.dyn, self.lamdyn (lamsteps; made by scale_dyn if
+          missing), self.vdyn or self.vlamdyn (velocity; ValueError if missing);
+          its NaN pixels are set to 0 in place and the result replaces it;
+        - svd=True: self.svd_model is the rank-nmodes model M (complex, zero
+          imaginary part) and the array becomes array / |M| (inf / NaN where M is 0);
+          frequency, time and nsmooth are ignored;
+        - svd=False: self.bandpass = nanmean over time (zeros replaced by its
+          mean), divided out (savgol_filter(., nsmooth, 1) first if nsmooth), then
+          the same over frequency on the quotient.  Zeros of self.dyn count as
+          NaN in both passes, so when the array is self.dyn every zero or NaN
+          pixel comes out NaN; NaN pixels of self.dyn are set to 0.
+
+        dtype=np.float64 returns float64 / complex128 like the reference;
+        np.float32 skips the widening.  nmodes must be in 1..32 and the array
+        at most 32768 x 16384 (ValueError before any device work).  A solver
+        that does not converge, or a tie between singular values nmodes and
+        nmodes+1, raises a RuntimeWarning; the result is still stored."""
+        import torch
+        from scipy.signal import savgol_filter
+        if svd:
+            thth._svd_check_modes(nmodes)
+        if hasattr(self, 'svd_model'):
+            print('Warning: An svd_model exists. Check before applying twice')
+        if lamsteps:
+            if velocity:
+                if not hasattr(self, 'vlamdyn'):
+                    raise ValueError('Need to run scale_dyn with a model')
+                attr = 'vlamdyn'
+            else:
+                if not hasattr(self, 'lamdyn'):
+                    self.scale_dyn(lamsteps=lamsteps)
+                attr = 'lamdyn'
+        elif velocity:
+            if not hasattr(self, 'vdyn'):
+                raise ValueError('Need to run scale_dyn with a model')
+            attr = 'vdyn'
+        else:
+            attr = 'dyn'
+        dyn = getattr(self, attr)
+        thth._svd_check(dyn, nmodes if svd else 1)
+        dyn[np.isnan(dyn)] = 0
+        cdt = np.complex64 if np.dtype(dtype) == np.float32 else np.complex128
+        if svd:
+            out, model, _ = thth._svd_run(dyn, int(nmodes))
+            self.svd_model = D.download(model).astype(cdt)
+        else:
+            nf, nt = dyn.shape
+            # the reference sets zeros of self.dyn to NaN before each pass: they are
+            # the selected array's zeros only when that array is self.dyn
+            zero_nan = 1 if (dyn is self.dyn and (frequency or time)) else 0
+            d = D.upload_f32(dyn)
+            rowdiv = coldiv = None
+            if frequency:
+                m = D.empty((nf,), torch.float64)
+                _lib.check(_lib.lib.sb_bandpass_rows(d.data_ptr(), nf, nt, zero_nan,
+                                                     m.data_ptr(), D.stream_ptr()))
+                bandpass = m.cpu().numpy()
+                bandpass[bandpass == 0] = np.mean(bandpass)
+                self.bandpass = bandpass.astype(dtype)
+                if nsmooth is not None:
+                    bandpass = savgol_filter(bandpass, nsmooth, 1)
+                rowdiv = D.upload(np.ascontiguousarray(bandpass, dtype=np.float64))
+            if time:
+                m = D.empty((nt,), torch.float64)
+                _lib.check(_lib.lib.sb_bandpass_cols(d.data_ptr(), nf, nt, zero_nan,
+                                                     D.ptr(rowdiv), m.data_ptr(),
+                                                     D.stream_ptr()))
+                timestructure = m.cpu().numpy()
+                timestructure[timestructure == 0] = np.mean(timestructure)
+                if nsmooth is not None:
+                    timestructure = savgol_filter(timestructure, nsmooth, 1)
+                coldiv = D.upload(np.ascontiguousarray(timestructure, dtype=np.float64))
+            out = D.empty((nf, nt), torch.float32)
+            _lib.check(_lib.lib.sb_bandpass_divide(d.data_ptr(), nf, nt, zero_nan,
+                                                   D.ptr(rowdiv), D.ptr(coldiv),
+                                                   out.data_ptr(), D.stream_ptr()))
+            self.dyn[np.isnan(self.dyn)] = 0
+        setattr(self, attr, D.download(out, np.dtype(dtype)))
 
     # ------------------------------------------------------------------
     # secondary spectrum

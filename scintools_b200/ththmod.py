@@ -19,6 +19,9 @@ Same function names, argument order and failure behaviour as the reference
   rotInit, rotMos, rotFit, rotDer, fullMos, fullMosFit, fullMosGrad, fullMosHess
                  ththmod.py:1708-2310 -> sb_mosaic_* (MosaicModel keeps the chunks
                  resident; rotInit's scalar recurrence runs on the host)
+  svd_model      ththmod.py:18-35 / scint_utils.py:705-729 -> sb_svd_topk +
+                 sb_svd_apply (the top nmodes triplets only; Dynspec.correct_dyn
+                 uses the same driver)
   min_edges      ththmod.py:1671-1705 (host)
   chi_par        ththmod.py:38-53     (host)
 
@@ -1469,3 +1472,84 @@ def fullMosHess(p, chunks, dspec, N):
     _check_p(chunks, p, True)
     _grad_data(chunks, dspec, N)
     return MosaicModel(chunks, dspec, N).hess(p)
+
+
+# ---- rank-k SVD model (Dynspec.correct_dyn) ------------------------------------------
+
+SVD_MAX_MODES = 32
+SVD_MAX_NF, SVD_MAX_NT = 32768, 16384
+
+
+def _svd_check(arr, nmodes):
+    """Argument checks of svd_model / Dynspec.correct_dyn, raised before any device call:
+    a real 2-D array of at most SVD_MAX_NF x SVD_MAX_NT and 1 <= nmodes <= SVD_MAX_MODES."""
+    a = np.asarray(arr)
+    if np.iscomplexobj(a):
+        raise TypeError("svd_model takes a real array, not %s" % a.dtype)
+    if a.ndim != 2:
+        raise ValueError("svd_model takes a 2-D array, got shape %s" % (a.shape,))
+    _svd_check_modes(nmodes)
+    nf, nt = a.shape
+    if not (1 <= nf <= SVD_MAX_NF and 1 <= nt <= SVD_MAX_NT):
+        raise ValueError("svd_model: shape %d x %d is outside 1..%d x 1..%d"
+                         % (nf, nt, SVD_MAX_NF, SVD_MAX_NT))
+    return a
+
+
+def _svd_check_modes(nmodes):
+    if not isinstance(nmodes, (int, np.integer)) or isinstance(nmodes, bool):
+        raise TypeError("nmodes must be an integer, got %r" % (nmodes,))
+    if not 1 <= nmodes <= SVD_MAX_MODES:
+        raise ValueError("nmodes must be in 1..%d, got %d" % (SVD_MAX_MODES, nmodes))
+
+
+def _svd_run(arr, nmodes, want_out=True, want_model=True):
+    """Device driver of svd_model and Dynspec.correct_dyn(svd=True) for a checked array:
+    the top-nmodes right singular vectors (sb_svd_topk), then one pass that writes
+    arr / |model| and the model (sb_svd_apply).  NaN pixels are read as 0.  Returns
+    (out, model, info): float32 device tensors (or None) and the solver's info dict.
+    Warns (RuntimeWarning) when the solver did not converge or the truncation boundary
+    is a tie."""
+    import torch
+    nf, nt = arr.shape
+    d = D.upload_f32(arr)
+    V = D.empty((nmodes, nt), torch.float64)
+    s = np.zeros(nmodes)
+    res = np.zeros(nmodes)
+    gap = np.zeros(1)
+    st = np.zeros(4, np.int32)
+    _lib.check(_lib.lib.sb_svd_topk(d.data_ptr(), nf, nt, nmodes, V.data_ptr(),
+                                    s.ctypes.data, res.ctypes.data, gap.ctypes.data,
+                                    st.ctypes.data, D.stream_ptr()))
+    out = D.empty((nf, nt), torch.float32) if want_out else None
+    model = D.empty((nf, nt), torch.float32) if want_model else None
+    _lib.check(_lib.lib.sb_svd_apply(d.data_ptr(), nf, nt, nmodes, V.data_ptr(), D.ptr(out),
+                                     D.ptr(model), D.stream_ptr()))
+    info = dict(s=s, residuals=res, steps=int(st[0]), converged=bool(st[1]), tie=bool(st[2]),
+                breakdown=bool(st[3]), gap=float(gap[0]))
+    if info["tie"]:
+        warnings.warn("svd_model: singular values %d and %d are equal to float32 precision; "
+                      "the rank-%d model is not defined by the data" % (nmodes, nmodes + 1, nmodes),
+                      RuntimeWarning, stacklevel=3)
+    elif not info["converged"]:
+        warnings.warn("svd_model: the rank-%d model did not converge (%d Lanczos steps)"
+                      % (nmodes, info["steps"]), RuntimeWarning, stacklevel=3)
+    return out, model, info
+
+
+def svd_model(arr, nmodes=1, return_info=False):
+    """ththmod.svd_model (ththmod.py:18-35): the rank-nmodes model of a real 2-D array,
+    complex128 with zero imaginary part like the reference's.  Only the top nmodes
+    singular triplets are computed (csrc/svd.cu); NaN pixels are read as 0.
+    nmodes >= min(arr.shape) gives the whole matrix, as in the reference.
+
+    ``return_info`` adds a dict: ``s`` (the nmodes singular values, descending),
+    ``residuals`` (||A^T A v_j - s_j^2 v_j||_2 from a final pass), ``steps`` (Lanczos
+    steps), ``converged``, ``tie`` (s_nmodes = s_nmodes+1 to float32 precision),
+    ``breakdown`` (the Krylov space became invariant: the model is exact) and ``gap``
+    (the lower bound on the eigenvalue gap of A^T A at the truncation the stopping rule
+    used).  Non-convergence and ties also raise a RuntimeWarning."""
+    a = _svd_check(arr, nmodes)
+    _, model, info = _svd_run(a, int(nmodes), want_out=False)
+    m = D.download(model).astype(np.complex128)
+    return (m, info) if return_info else m
