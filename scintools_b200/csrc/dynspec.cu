@@ -13,7 +13,6 @@
 #include <stdlib.h>
 
 #include "fft_kernels.cuh"
-#include "chirp.cuh"
 #include "chisq.cuh"
 
 namespace sb {
@@ -204,35 +203,6 @@ struct HalfStore {   // X[k] -> H[row][k], only the first kmax bins are kept
     }
 };
 
-// ------------------------------------------------------ column pass functors
-struct ColALoad {    // y = r2, i = r1: row r1*R2 + r2, zero beyond the live rows
-    const float2* H;
-    long pitch;
-    int R2, live;
-    __device__ __forceinline__ float2 operator()(int y, int i, int c) const {
-        const int row = i * R2 + y;
-        return row < live ? H[(size_t)row * pitch + c] : make_float2(0.f, 0.f);
-    }
-};
-struct ColAStore {   // multiply by W_R^(dir r2 k1), write row k1*R2 + r2
-    float2* A;
-    long pitch;
-    int R2, R;
-    const float2* wR;
-    __device__ __forceinline__ void operator()(int y, int k, int c, float2 v) const {
-        const float2 w = wR[(y * k) & (R - 1)];
-        A[(size_t)(k * R2 + y) * pitch + c] = cmul(v, w);
-    }
-};
-struct ColBLoad {    // y = k1, i = r2
-    const float2* A;
-    long pitch;
-    int R2;
-    __device__ __forceinline__ float2 operator()(int y, int i, int c) const {
-        return A[(size_t)(y * R2 + i) * pitch + c];
-    }
-};
-
 // conjugate spectrum epilogue: fftshift both axes, Hermitian expansion to the
 // full plane, tau row mask, DC correction for a non-zero pad constant
 struct CsStore {
@@ -348,22 +318,6 @@ acf_mid_kernel(const float2* __restrict__ A, float2* __restrict__ G, long pitch,
     }
 }
 
-struct AcfInvLoad {   // y = n2, i = k1
-    const float2* G;
-    long pitch;
-    int R2;
-    __device__ __forceinline__ float2 operator()(int y, int i, int c) const {
-        return G[(size_t)(i * R2 + y) * pitch + c];
-    }
-};
-struct AcfInvStore {  // n = n2 + R2 n1
-    float2* Q;
-    long pitch;
-    int R2;
-    __device__ __forceinline__ void operator()(int y, int k, int c, float2 v) const {
-        Q[(size_t)(y + R2 * k) * pitch + c] = v;
-    }
-};
 struct AcfRowLoad {   // output row i <- circular row (i - nf) mod PF
     const float2* Q;
     long pitch;
@@ -444,11 +398,16 @@ static TmaEncodeFn tma_encoder() {
     return fn;
 }
 
+// The tensor map of a column pass that fetches its tiles by the TMA, or false
+// when the pass must use plain loads (tile_fft_kernel) instead: SB_FFT_NO_TMA
+// is set, the driver has no encoder, or the live rows are not whole r2-groups.
 // float2 matrix [rows][pitch] seen as float32; tiles of L rows x W complex.
-// r2 > 0: rank-3 view (col, y < r2, i) of the row i * r2 + y with `nlive / r2`
-// valid i (rows >= nlive read as zeros); r2 == 0: plain rank-2 (col, row).
+// r2 > 0: rank-3 view (col, y < r2, i) of the row i * r2 + y with `nrows / r2`
+// valid i (rows past them read as zeros); r2 == 0: plain rank-2 (col, row).
 static bool make_tile_map(CUtensorMap* m, const float2* base, long pitch, int ncols, long nrows,
                           int r2, int L, int W) {
+    static const bool no_tma = getenv("SB_FFT_NO_TMA") != nullptr;
+    if (no_tma || (r2 > 0 && (nrows % r2 != 0 || nrows < r2))) return false;
     TmaEncodeFn enc = tma_encoder();
     if (!enc) return false;
     cuuint64_t gdim[3], gstr[2];
@@ -477,11 +436,7 @@ static bool make_tile_map(CUtensorMap* m, const float2* base, long pitch, int nc
 
 // Column transform of length NF (four-step split R1 x R2, two tile passes) over the
 // half spectra H[live][pitch] -> epilogue stb.  Tiles are fetched by the TMA
-// (cp.async.bulk.tensor, zero fill for the padded rows) whenever the live rows are
-// whole r2-groups; SB_FFT_NO_TMA=1 forces the LDG path.  SB_COL_CHUNK_MB=N walks the
-// columns in chunks of N MB of the intermediate A[NF][chunk] (an experiment: pass B
-// re-reads each chunk from DRAM anyway -- L2 hit rate 12 % at 48 MB chunks -- and the
-// smaller grids cost more than they save, so the default is one chunk).
+// (cp.async.bulk.tensor, zero fill for the padded rows) when make_tile_map allows it.
 template <class StoreB>
 static int cols_forward(const float2* H, float2* A, long pitch, int NF, int live,
                         int ncols, StoreB stb, cudaStream_t st, int profA = -1,
@@ -490,42 +445,28 @@ static int cols_forward(const float2* H, float2* A, long pitch, int NF, int live
     split_len(NF, &R1, &R2);
     const float2* wR = twiddle_table<float>(NF, -1, st);
     if (!wR) return SB_ERR_NOMEM;
-    ColALoad la{H, pitch, R2, live};
-    ColAStore sa{A, pitch, R2, NF, wR};
-    ColBLoad lb{A, pitch, R2};
-    static const bool no_tma = getenv("SB_FFT_NO_TMA") != nullptr;
+    ZeroPadALoad<float2> la{H, pitch, R2, live};
+    TwiddleAStore<float2> sa{A, pitch, R2, NF, wR};
+    BlockBLoad<float2> lb{A, pitch, R2};
     CUtensorMap mapA, mapB;
-    const bool tma = !no_tma && live % R2 == 0 && live >= R2 && R1 <= 256 && R2 <= 256 &&
-                     make_tile_map(&mapA, H, pitch, ncols, live, R2, R1, 32) &&
+    const bool tma = make_tile_map(&mapA, H, pitch, ncols, live, R2, R1, 32) &&
                      make_tile_map(&mapB, A, pitch, ncols, NF, 0, R2, 64);
-    long chunk_mb = 0;
-    if (const char* ev = getenv("SB_COL_CHUNK_MB")) chunk_mb = atol(ev);
-    int cw = ncols;
-    if (chunk_mb > 0) {
-        const long c = (chunk_mb << 20) / ((long)NF * (long)sizeof(float2));
-        cw = (int)((c / 64) * 64);
-        if (cw < 256) cw = 256;
-        if (cw > ncols) cw = ncols;
-    }
     int rc = SB_OK;
-    for (int cb = 0; cb < ncols && rc == SB_OK; cb += cw) {
-        const int ce = cb + cw < ncols ? cb + cw : ncols;
-        if (profA >= 0) prof_begin(profA, st);
-        if (tma) {
-            SB_TILE_DISPATCH(R1, rc = (launch_tile_fft_tma<LL, 32, -1, 3>(mapA, sa, ncols, R2, st, cb, ce)));
-        } else {
-            SB_TILE_DISPATCH(R1, rc = (launch_tile_fft<float, LL, 32, -1>(la, sa, ncols, R2, st, cb, ce)));
-        }
-        if (profA >= 0) prof_end(profA, st);
-        if (rc) return rc;
-        if (profB >= 0) prof_begin(profB, st);
-        if (tma) {
-            SB_TILE_DISPATCH(R2, rc = (launch_tile_fft_tma<LL, 64, -1, 2>(mapB, stb, ncols, R1, st, cb, ce)));
-        } else {
-            SB_TILE_DISPATCH(R2, rc = (launch_tile_fft<float, LL, 64, -1>(lb, stb, ncols, R1, st, cb, ce)));
-        }
-        if (profB >= 0) prof_end(profB, st);
+    if (profA >= 0) prof_begin(profA, st);
+    if (tma) {
+        SB_TILE_DISPATCH(R1, rc = (launch_tile_fft_tma<LL, 32, -1, 3>(mapA, sa, ncols, R2, st)));
+    } else {
+        SB_TILE_DISPATCH(R1, rc = (launch_tile_fft<float, LL, 32, -1>(la, sa, ncols, R2, st)));
     }
+    if (profA >= 0) prof_end(profA, st);
+    if (rc) return rc;
+    if (profB >= 0) prof_begin(profB, st);
+    if (tma) {
+        SB_TILE_DISPATCH(R2, rc = (launch_tile_fft_tma<LL, 64, -1, 2>(mapB, stb, ncols, R1, st)));
+    } else {
+        SB_TILE_DISPATCH(R2, rc = (launch_tile_fft<float, LL, 64, -1>(lb, stb, ncols, R1, st)));
+    }
+    if (profB >= 0) prof_end(profB, st);
     return rc;
 }
 
@@ -568,39 +509,6 @@ struct DynRowLoadD {
         return make_double2(get((int)row, 2 * n), get((int)row, 2 * n + 1));
     }
 };
-struct HalfStoreD {
-    double2* H;
-    long pitch;
-    __device__ __forceinline__ void operator()(long row, int k, double2 v) const {
-        H[row * pitch + k] = v;
-    }
-};
-struct ColALoadD {
-    const double2* H;
-    long pitch;
-    int R2, live;
-    __device__ __forceinline__ double2 operator()(int y, int i, int c) const {
-        const int row = i * R2 + y;
-        return row < live ? H[(size_t)row * pitch + c] : make_double2(0.0, 0.0);
-    }
-};
-struct ColAStoreD {
-    double2* A;
-    long pitch;
-    int R2, R;
-    const double2* wR;
-    __device__ __forceinline__ void operator()(int y, int k, int c, double2 v) const {
-        A[(size_t)(k * R2 + y) * pitch + c] = cmul(v, wR[(y * k) & (R - 1)]);
-    }
-};
-struct ColBLoadD {
-    const double2* A;
-    long pitch;
-    int R2;
-    __device__ __forceinline__ double2 operator()(int y, int i, int c) const {
-        return A[(size_t)(y * R2 + i) * pitch + c];
-    }
-};
 struct SspecStoreD {     // halved frame only (prewhite requires halve)
     float* sec;
     int NF, NT, R1, db;
@@ -636,24 +544,16 @@ static int sspec_prewhite_f64(const float* dyn, int nf, int nt, const float* wt,
     double2* A = (double2*)workspace(4, (size_t)NF * pitch * sizeof(double2));
     if (!H || !A) return SB_ERR_NOMEM;
     DynRowLoadD ld{dyn, nf, nt, wt, wf, stats};
-    HalfStoreD hs{H, pitch};
+    PlainRowStore<double2> hs{H, pitch};
     int rc = SB_OK;
     const int N = NT / 2;
     SB_ROW_DISPATCH(N, rc = (launch_row_r2c<double, N1, N2>(ld, hs, live, st)));
     if (rc) return rc;
     int R1, R2;
     split_len(NF, &R1, &R2);
-    const double2* wR = twiddle_table<double>(NF, -1, st);
-    if (!wR) return SB_ERR_NOMEM;
-    ColALoadD la{H, pitch, R2, live};
-    ColAStoreD sa{A, pitch, R2, NF, wR};
-    const int ncols = NT / 2 + 1;
-    SB_TILE_DISPATCH(R1, rc = (launch_tile_fft<double, LL, 16, -1>(la, sa, ncols, R2, st)));
-    if (rc) return rc;
-    ColBLoadD lb{A, pitch, R2};
+    ZeroPadALoad<double2> la{H, pitch, R2, live};
     SspecStoreD ss{sec, NF, NT, R1, db};
-    SB_TILE_DISPATCH(R2, rc = (launch_tile_fft<double, LL, 16, -1>(lb, ss, ncols, R1, st)));
-    return rc;
+    return cols_generic<double, -1>(la, A, pitch, NF, NT / 2 + 1, ss, st);
 }
 
 // Dynspec.calc_sspec (dynspec.py:3664-3721)
@@ -685,11 +585,6 @@ int sspec(const float* dyn, int nf, int nt, const float* wt, const float* wf,
     SspecStore ss{sec, NF, NT, R1, halve, db, prewhite ? pd1 : nullptr, pd2, noshift};
     return cols_forward(H, A, pitch, NF, live, NT / 2 + 1, ss, st);
 }
-
-static int conj_spectrum_bluestein(const float* dyn, int nf, int nt, int NF, int NT,
-                                   float pad_value, const double* stats,
-                                   const unsigned char* rowmask, float2* CS,
-                                   cudaStream_t st);
 
 // sum |dyn - c| (c = stats[4], the mean, when use_mean; else the constant sub)
 __global__ void dyn_l1_kernel(const float* __restrict__ dyn, long total, const double* __restrict__ stats,
@@ -735,6 +630,92 @@ int conj_spectrum_bound(const float* dyn, int nf, int nt, int npad, float pad_va
     return SB_OK;
 }
 
+// ------------------------------------------------------------------------
+// 2-D transforms of sizes that are NOT powers of two (e.g. the reference
+// tutorial's 64 x 150 chunk -> 256 x 600 conjugate spectrum, and its inverse in
+// phase retrieval): Bluestein / chirp-z on both axes on top of the power-of-two
+// engine.
+//   X[k] = w[k] * sum_n (x[n] w[n]) conj(w)[k - n],  w[n] = exp(-i pi n^2 / N)
+// = w[k] * IFFT_M( FFT_M(x w) * FFT_M(b) )[k],  M = 2^p >= 2N - 1.
+// Full plane output (no Hermitian shortcut), generic fftshift (odd N too).
+// Chirp tables and the load / store functors of these passes: fft_functors.cuh
+// ------------------------------------------------------------------------
+// chirp w[N] and the transformed kernel B = FFT_M(b)
+static int bluestein_tables(int N, int M, float2* w, float2* B, float2* scratch,
+                            cudaStream_t st) {
+    chirp_fill_kernel<<<(M + 255) / 256, 256, 0, st>>>(w, B, N, M);
+    SB_LAUNCH_CHECK();
+    if (M <= 16384) {
+        SB_CUDA(cudaMemcpyAsync(scratch, B, (size_t)M * sizeof(float2),
+                                cudaMemcpyDeviceToDevice, st));
+        VecLoad ld{scratch};
+        VecStore vs{B};
+        int rc = SB_OK;
+        SB_ROW_DISPATCH(M, rc = (launch_row_c2c<float, N1, N2, -1>(ld, vs, 1, st)));
+        return rc;
+    }
+    int R1, R2;
+    split_len(M, &R1, &R2);
+    SB_CUDA(cudaMemcpyAsync(scratch, B, (size_t)M * sizeof(float2),
+                            cudaMemcpyDeviceToDevice, st));
+    ColVecLoad la{scratch, R2};
+    ColVecStore sb_{B, R1};
+    return cols_generic<float, -1>(la, scratch + M, 1, M, 1, sb_, st);
+}
+
+// Forward chirp-z transform of an n0 x n1 plane whose first `live` rows are read by
+// ld (ChirpRowLoad or ChirpRowLoadC; its chirp w is set here) and whose other rows
+// are zero.  The final column pass stores through mk(R1, wF, MF) (wF: chirp of the
+// column axis, MF: its padded length); columns >= ncols are never stored.  `what`
+// begins the error message of a size outside the limits.
+template <class RowLoad, class MakeStore>
+static int chirp_fft2(RowLoad ld, int n0, int n1, int live, int ncols, MakeStore mk,
+                      const char* what, cudaStream_t st) {
+    const int MT = next_pow2(2L * n1 - 1), MF = next_pow2(2L * n0 - 1);
+    // M >= 8 on both axes: bluestein_tables transforms the kernel with a row FFT (>= 8 points)
+    if (MT < 8 || MT > 16384 || MF < 8 || MF > 65536) {
+        set_error("%s %d x %d outside 3..32768 x 3..8192 (rows 3..32768, cols 3..8192)", what,
+                  n0, n1);
+        return SB_ERR_UNSUPPORTED;
+    }
+    const long pt = ((long)n1 + 15) & ~15L;
+    float2* tabs = (float2*)workspace(6, (size_t)(n1 + 3L * MT + n0 + 3L * MF + 64) * sizeof(float2));
+    float2* R1buf = (float2*)workspace(3, (size_t)live * MT * sizeof(float2));
+    float2* Ybuf = (float2*)workspace(4, (size_t)live * pt * sizeof(float2));
+    float2* C0 = (float2*)workspace(5, (size_t)MF * pt * sizeof(float2));
+    float2* C1 = (float2*)workspace(7, (size_t)MF * pt * sizeof(float2));
+    if (!tabs || !R1buf || !Ybuf || !C0 || !C1) return SB_ERR_NOMEM;
+    float2* wT = tabs;
+    float2* BT = wT + n1;
+    float2* wF = BT + MT;
+    float2* BF = wF + n0;
+    float2* scratch = BF + MF;      // 2*max(MT, MF)
+    int rc = bluestein_tables(n1, MT, wT, BT, scratch, st);
+    if (rc) return rc;
+    rc = bluestein_tables(n0, MF, wF, BF, scratch, st);
+    if (rc) return rc;
+    // rows: chirp, FFT, multiply, inverse FFT, chirp
+    {
+        ld.w = wT;
+        MulVecRowStore ms{R1buf, MT, BT};
+        SB_ROW_DISPATCH(MT, rc = (launch_row_c2c<float, N1, N2, -1>(ld, ms, live, st)));
+        if (rc) return rc;
+        PitchRowLoad<float2> pl{R1buf, MT};
+        ChirpOutRowStore os{Ybuf, pt, wT, n1, 1.0f / (float)MT};
+        SB_ROW_DISPATCH(MT, rc = (launch_row_c2c<float, N1, N2, +1>(pl, os, live, st)));
+        if (rc) return rc;
+    }
+    // columns
+    int R1, R2;
+    split_len(MF, &R1, &R2);
+    ChirpColALoad la{Ybuf, pt, R2, live, wF};
+    MulVecColStore mc{C1, pt, R1, BF};
+    rc = cols_generic<float, -1>(la, C0, pt, MF, ncols, mc, st);
+    if (rc) return rc;
+    StrideALoad<float2> pa{C1, pt, R2};
+    return cols_generic<float, +1>(pa, C0, pt, MF, ncols, mk(R1, wF, MF), st);
+}
+
 // conjugate spectrum of a zero(/constant)-padded chunk
 // (ththmod.py:777-787, dynspec.py:1572-1579)
 int conj_spectrum(const float* dyn, int nf, int nt, int npad, float pad_value,
@@ -756,8 +737,12 @@ int conj_spectrum(const float* dyn, int nf, int nt, int npad, float pad_value,
             if (rc0) return rc0;
             pad_value = 0.f;
         }
-        return conj_spectrum_bluestein(dyn, nf, nt, (int)NFl, (int)NTl, pad_value,
-                                       bstats, rowmask, CS, st);
+        const int NF = (int)NFl, NT = (int)NTl;
+        return chirp_fft2(ChirpRowLoad{dyn, nt, nullptr, bstats, pad_value}, NF, NT, nf, NT,
+                          [&](int R1, const float2* wF, int MF) {
+                              return ChirpCsStore{CS, NF, NT, R1, wF, 1.0f / (float)MF, rowmask,
+                                                  pad_value * (float)NF * (float)NT, bstats};
+                          }, "conjugate spectrum (chirp-z): padded size", st);
     }
     if (NTl / 2 > 16384 || NFl > 65536) {
         set_error("conjugate spectrum: padded size %ldx%ld too large "
@@ -798,171 +783,21 @@ int conj_spectrum(const float* dyn, int nf, int nt, int npad, float pad_value,
 }
 
 
-// ------------------------------------------------------------------------
-// Conjugate spectrum for padded sizes that are NOT powers of two (e.g. the
-// reference tutorial's 64 x 150 chunk -> 256 x 600): Bluestein / chirp-z on
-// both axes on top of the power-of-two engine.
-//   X[k] = w[k] * sum_n (x[n] w[n]) conj(w)[k - n],  w[n] = exp(-i pi n^2 / N)
-// = w[k] * IFFT_M( FFT_M(x w) * FFT_M(b) )[k],  M = 2^p >= 2N - 1.
-// Full plane output (no Hermitian shortcut), generic fftshift (odd N too).
-// ------------------------------------------------------------------------
-// chirp tables and the load / store functors of the chirp-z passes: chirp.cuh
-template <int DIR, class LoadA, class StoreB>
-static int cols_generic_f(LoadA la, float2* tmp, long pitch, int R, int ncols,
-                          StoreB sb, cudaStream_t st) {
-    int R1, R2;
-    split_len(R, &R1, &R2);
-    const float2* wR = twiddle_table<float>(R, DIR, st);
-    if (!wR) return SB_ERR_NOMEM;
-    ColAStore sa{tmp, pitch, R2, R, wR};
-    int rc = SB_OK;
-    SB_TILE_DISPATCH(R1, rc = (launch_tile_fft<float, LL, 32, DIR>(la, sa, ncols, R2, st)));
-    if (rc) return rc;
-    ColBLoad lb{tmp, pitch, R2};
-    SB_TILE_DISPATCH(R2, rc = (launch_tile_fft<float, LL, 32, DIR>(lb, sb, ncols, R1, st)));
-    return rc;
-}
-
-// chirp w[N] and the transformed kernel B = FFT_M(b)
-static int bluestein_tables(int N, int M, float2* w, float2* B, float2* scratch,
-                            cudaStream_t st) {
-    chirp_fill_kernel<<<(M + 255) / 256, 256, 0, st>>>(w, B, N, M);
-    SB_LAUNCH_CHECK();
-    if (M <= 16384) {
-        SB_CUDA(cudaMemcpyAsync(scratch, B, (size_t)M * sizeof(float2),
-                                cudaMemcpyDeviceToDevice, st));
-        VecLoad ld{scratch};
-        VecStore vs{B};
-        int rc = SB_OK;
-        SB_ROW_DISPATCH(M, rc = (launch_row_c2c<float, N1, N2, -1>(ld, vs, 1, st)));
-        return rc;
-    }
-    int R1, R2;
-    split_len(M, &R1, &R2);
-    SB_CUDA(cudaMemcpyAsync(scratch, B, (size_t)M * sizeof(float2),
-                            cudaMemcpyDeviceToDevice, st));
-    ColVecLoad la{scratch, R2};
-    ColVecStore sb_{B, R1};
-    return cols_generic_f<-1>(la, scratch + M, 1, M, 1, sb_, st);
-}
-
-static int conj_spectrum_bluestein(const float* dyn, int nf, int nt, int NF, int NT,
-                                   float pad_value, const double* stats,
-                                   const unsigned char* rowmask, float2* CS,
-                                   cudaStream_t st) {
-    const int MT = next_pow2(2L * NT - 1), MF = next_pow2(2L * NF - 1);
-    // M >= 8 on both axes: bluestein_tables transforms the kernel with a row FFT (>= 8 points)
-    if (MT < 8 || MT > 16384 || MF < 8 || MF > 65536) {
-        set_error("conjugate spectrum (Bluestein): padded size %dx%d unsupported "
-                  "(rows 3..32768, cols 3..8192 for non power-of-two sizes)", NF, NT);
-        return SB_ERR_UNSUPPORTED;
-    }
-    const long pt = ((long)NT + 15) & ~15L;
-    float2* tabs = (float2*)workspace(6, (size_t)(NT + 3L * MT + NF + 3L * MF + 64) * sizeof(float2));
-    float2* R1buf = (float2*)workspace(3, (size_t)nf * MT * sizeof(float2));
-    float2* Ybuf = (float2*)workspace(4, (size_t)nf * pt * sizeof(float2));
-    float2* C0 = (float2*)workspace(5, (size_t)MF * pt * sizeof(float2));
-    float2* C1 = (float2*)workspace(7, (size_t)MF * pt * sizeof(float2));
-    if (!tabs || !R1buf || !Ybuf || !C0 || !C1) return SB_ERR_NOMEM;
-    float2* wT = tabs;
-    float2* BT = wT + NT;
-    float2* wF = BT + MT;
-    float2* BF = wF + NF;
-    float2* scratch = BF + MF;      // 2*max(MT, MF)
-    int rc = bluestein_tables(NT, MT, wT, BT, scratch, st);
-    if (rc) return rc;
-    rc = bluestein_tables(NF, MF, wF, BF, scratch, st);
-    if (rc) return rc;
-    // rows: chirp, FFT, multiply, inverse FFT, chirp
-    {
-        ChirpRowLoad ld{dyn, nt, wT, stats, pad_value};
-        MulVecRowStore ms{R1buf, MT, BT};
-        SB_ROW_DISPATCH(MT, rc = (launch_row_c2c<float, N1, N2, -1>(ld, ms, nf, st)));
-        if (rc) return rc;
-        PitchRowLoad pl{R1buf, MT};
-        ChirpOutRowStore os{Ybuf, pt, wT, NT, 1.0f / (float)MT};
-        SB_ROW_DISPATCH(MT, rc = (launch_row_c2c<float, N1, N2, +1>(pl, os, nf, st)));
-        if (rc) return rc;
-    }
-    // columns
-    int R1, R2;
-    split_len(MF, &R1, &R2);
-    ChirpColALoad la{Ybuf, pt, R2, nf, wF};
-    MulVecColStore mc{C1, pt, R1, BF};
-    rc = cols_generic_f<-1>(la, C0, pt, MF, NT, mc, st);
-    if (rc) return rc;
-    PlainColALoad pa{C1, pt, R2};
-    ChirpCsStore cs{CS, NF, NT, R1, wF, 1.0f / (float)MF, rowmask,
-                    pad_value * (float)NF * (float)NT, stats};
-    return cols_generic_f<+1>(pa, C0, pt, MF, NT, cs, st);
-}
-
-// ------------------------------------------------------------------------
-// out[:crop0, :crop1] = scale * ifft2(ifftshift(in)) for ANY sizes (phase
-// retrieval on the tutorial's 256 x 600 conjugate spectrum), by the same
-// chirp-z machinery: ifft2(X) = conj(fft2(conj X)) / (N0 N1).
-// ------------------------------------------------------------------------
-// conj_in != 0: returns ifft2(conj(in)) = conj(fft2(in)) / (n0 n1) (used for the
-// forward transform of the Gerchberg-Saxton loop)
-// the chirp-z inverse of ifft2_c2c_any up to its final column pass, whose store is
-// mk(R1, wF, MF * n0 * n1) (wF: chirp of the column axis, the last argument the divisor
-// that normalises the transform); columns >= ncols are never stored
-template <class MakeStore>
-static int ifft2_any_core(const float2* in, int n0, int n1, int centred, int ncols, int conj_in,
-                          MakeStore mk, cudaStream_t st) {
-    const int MT = next_pow2(2L * n1 - 1), MF = next_pow2(2L * n0 - 1);
-    // M >= 8 on both axes: bluestein_tables transforms the kernel with a row FFT (>= 8 points)
-    if (MT < 8 || MT > 16384 || MF < 8 || MF > 65536) {
-        set_error("ifft2 (chirp-z): %d x %d outside 3..32768 x 3..8192", n0, n1);
-        return SB_ERR_UNSUPPORTED;
-    }
-    const long pt = ((long)n1 + 15) & ~15L;
-    float2* tabs = (float2*)workspace(6, (size_t)(n1 + 3L * MT + n0 + 3L * MF + 64) * sizeof(float2));
-    float2* R1buf = (float2*)workspace(3, (size_t)n0 * MT * sizeof(float2));
-    float2* Ybuf = (float2*)workspace(4, (size_t)n0 * pt * sizeof(float2));
-    float2* C0 = (float2*)workspace(5, (size_t)MF * pt * sizeof(float2));
-    float2* C1 = (float2*)workspace(7, (size_t)MF * pt * sizeof(float2));
-    if (!tabs || !R1buf || !Ybuf || !C0 || !C1) return SB_ERR_NOMEM;
-    float2* wT = tabs;
-    float2* BT = wT + n1;
-    float2* wF = BT + MT;
-    float2* BF = wF + n0;
-    float2* scratch = BF + MF;      // 2*max(MT, MF)
-    int rc = bluestein_tables(n1, MT, wT, BT, scratch, st);
-    if (rc) return rc;
-    rc = bluestein_tables(n0, MF, wF, BF, scratch, st);
-    if (rc) return rc;
-    {
-        ChirpRowLoadC ld{in, n0, n1, centred, conj_in, wT};
-        MulVecRowStore ms{R1buf, MT, BT};
-        SB_ROW_DISPATCH(MT, rc = (launch_row_c2c<float, N1, N2, -1>(ld, ms, n0, st)));
-        if (rc) return rc;
-        PitchRowLoad pl{R1buf, MT};
-        ChirpOutRowStore os{Ybuf, pt, wT, n1, 1.0f / (float)MT};
-        SB_ROW_DISPATCH(MT, rc = (launch_row_c2c<float, N1, N2, +1>(pl, os, n0, st)));
-        if (rc) return rc;
-    }
-    int R1, R2;
-    split_len(MF, &R1, &R2);
-    ChirpColALoad la{Ybuf, pt, R2, n0, wF};
-    MulVecColStore mc{C1, pt, R1, BF};
-    rc = cols_generic_f<-1>(la, C0, pt, MF, ncols, mc, st);
-    if (rc) return rc;
-    PlainColALoad pa{C1, pt, R2};
-    return cols_generic_f<+1>(pa, C0, pt, MF, ncols, mk(R1, wF, (double)MF * (double)n0 * (double)n1),
-                              st);
-}
-
+// out[:crop0, :crop1] = scale * ifft2(ifftshift(in)) for ANY sizes (phase retrieval
+// on the tutorial's 256 x 600 conjugate spectrum), by the chirp-z transform:
+// ifft2(X) = conj(fft2(conj X)) / (N0 N1).  conj_in != 0: returns ifft2(conj(in)) =
+// conj(fft2(in)) / (n0 n1) (the forward transform of the Gerchberg-Saxton loop)
 int ifft2_c2c_any(const float2* in, int n0, int n1, int centred, int crop0, int crop1,
                   double scale, int real_only, void* out, cudaStream_t st, int conj_in) {
     if (crop0 <= 0 || crop0 > n0) crop0 = n0;
     if (crop1 <= 0 || crop1 > n1) crop1 = n1;
-    return ifft2_any_core(in, n0, n1, centred, crop1, conj_in,
-                          [&](int R1, const float2* wF, double den) {
-                              return ChirpCropStore{real_only ? nullptr : (float2*)out,
-                                                    real_only ? (float*)out : nullptr, R1,
-                                                    crop0, crop1, wF, (float)(scale / den)};
-                          }, st);
+    return chirp_fft2(ChirpRowLoadC{in, n0, n1, centred, conj_in, nullptr}, n0, n1, n0, crop1,
+                      [&](int R1, const float2* wF, int MF) {
+                          const double den = (double)MF * (double)n0 * (double)n1;
+                          return ChirpCropStore{real_only ? nullptr : (float2*)out,
+                                                real_only ? (float*)out : nullptr, R1,
+                                                crop0, crop1, wF, (float)(scale / den)};
+                      }, "ifft2 (chirp-z):", st);
 }
 
 // chisq_sweep (retrieval.cu): sum over the mask of (real(ifft2(ifftshift(in)))[:nf, :nt] -
@@ -980,10 +815,11 @@ struct ChirpResidualStore {
 };
 int ifft2_any_residual(const float2* in, int n0, int n1, const ResidualSink& sink,
                        cudaStream_t st) {
-    return ifft2_any_core(in, n0, n1, 1, sink.nt, 0,
-                          [&](int R1, const float2* wF, double den) {
-                              return ChirpResidualStore{R1, wF, (float)(1.0 / den), sink};
-                          }, st);
+    return chirp_fft2(ChirpRowLoadC{in, n0, n1, 1, 0, nullptr}, n0, n1, n0, sink.nt,
+                      [&](int R1, const float2* wF, int MF) {
+                          const double den = (double)MF * (double)n0 * (double)n1;
+                          return ChirpResidualStore{R1, wF, (float)(1.0 / den), sink};
+                      }, "ifft2 (chirp-z):", st);
 }
 
 // Dynspec.calc_acf(method='direct') (dynspec.py:3780-3797)
@@ -1014,11 +850,10 @@ int acf(const float* dyn, int nf, int nt, int subtract_mean, int normalise,
     {
         const float2* wR = twiddle_table<float>(PF, -1, st);
         if (!wR) return SB_ERR_NOMEM;
-        ColALoad la{H, pitch, R2, nf};
-        ColAStore sa{A, pitch, R2, PF, wR};
+        ZeroPadALoad<float2> la{H, pitch, R2, nf};
+        TwiddleAStore<float2> sa{A, pitch, R2, PF, wR};
         CUtensorMap mapA;
-        if (!getenv("SB_FFT_NO_TMA") && nf % R2 == 0 && nf >= R2 && R1 <= 256 &&
-            make_tile_map(&mapA, H, pitch, ncols, nf, R2, R1, 32)) {
+        if (make_tile_map(&mapA, H, pitch, ncols, nf, R2, R1, 32)) {
             SB_TILE_DISPATCH(R1, rc = (launch_tile_fft_tma<LL, 32, -1, 3>(mapA, sa, ncols, R2, st)));
         } else {
             SB_TILE_DISPATCH(R1, rc = (launch_tile_fft<float, LL, 32, -1>(la, sa, ncols, R2, st)));
@@ -1044,11 +879,10 @@ int acf(const float* dyn, int nf, int nt, int subtract_mean, int normalise,
     }
     // inverse over k1 -> Q (reuse A)
     {
-        AcfInvLoad li{G, pitch, R2};
-        AcfInvStore si{A, pitch, R2};
+        StrideALoad<float2> li{G, pitch, R2};      // y = n2, i = k1
+        NaturalBStore<float2> si{A, pitch, R2};    // n = n2 + R2 n1
         CUtensorMap mapG;
-        if (!getenv("SB_FFT_NO_TMA") && R1 <= 256 &&
-            make_tile_map(&mapG, G, pitch, ncols, PF, R2, R1, 32)) {
+        if (make_tile_map(&mapG, G, pitch, ncols, PF, R2, R1, 32)) {
             SB_TILE_DISPATCH(R1, rc = (launch_tile_fft_tma<LL, 32, +1, 3>(mapG, si, ncols, R2, st)));
         } else {
             SB_TILE_DISPATCH(R1, rc = (launch_tile_fft<float, LL, 32, +1>(li, si, ncols, R2, st)));

@@ -14,9 +14,9 @@
 //                    complex->complex, real->half-spectrum, half-spectrum->real.
 #pragma once
 #include <cuda.h>      // CUtensorMap (type only; the encoder is fetched through the runtime)
-#include <stdlib.h>
 
 #include "fft_core.cuh"
+#include "fft_functors.cuh"
 #include "tma.cuh"
 
 namespace sb {
@@ -34,14 +34,14 @@ template <> struct ILog2<1> { static constexpr int value = 0; };
 // --------------------------------------------------------------------------
 template <typename T, int L, int W, int DIR, class Load, class Store>
 __global__ void __launch_bounds__(256)
-tile_fft_kernel(Load ld, Store st, const cx<T>* __restrict__ twL, int ncols, int col_base) {
+tile_fft_kernel(Load ld, Store st, const cx<T>* __restrict__ twL, int ncols) {
     using C = cx<T>;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     C* s = reinterpret_cast<C*>(smem_raw);
     C* tw = s + L * W;
     const int tid = threadIdx.x;
     constexpr int NT = 256;
-    const int c0 = col_base + blockIdx.x * W;
+    const int c0 = blockIdx.x * W;
     const int y = blockIdx.y;
     for (int i = tid; i < L; i += NT) tw[i] = twL[i];
     for (int idx = tid; idx < L * W; idx += NT) {
@@ -56,18 +56,15 @@ tile_fft_kernel(Load ld, Store st, const cx<T>* __restrict__ twL, int ncols, int
     }
 }
 
-// columns [col_base, col_end) of the problem (col_end <= ncols_total is the store limit)
 template <typename T, int L, int W, int DIR, class Load, class Store>
-int launch_tile_fft(Load ld, Store st, int ncols, int ny, cudaStream_t stream,
-                    int col_base = 0, int col_end = -1) {
+int launch_tile_fft(Load ld, Store st, int ncols, int ny, cudaStream_t stream) {
     const cx<T>* tw = twiddle_table<T>(L, DIR, stream);
     if (!tw) return SB_ERR_NOMEM;
-    if (col_end < 0 || col_end > ncols) col_end = ncols;
     auto kern = tile_fft_kernel<T, L, W, DIR, Load, Store>;
     const size_t smem = (size_t)(L * W + L) * sizeof(cx<T>);
     SB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    dim3 grid((col_end - col_base + W - 1) / W, ny);
-    kern<<<grid, 256, smem, stream>>>(ld, st, tw, col_end, col_base);
+    dim3 grid((ncols + W - 1) / W, ny);
+    kern<<<grid, 256, smem, stream>>>(ld, st, tw, ncols);
     SB_LAUNCH_CHECK();
     return SB_OK;
 }
@@ -101,14 +98,14 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, i
 template <int L, int W, int DIR, int RANK, class Store>
 __global__ void __launch_bounds__(256)
 tile_fft_tma_kernel(const __grid_constant__ CUtensorMap tmap, Store st,
-                    const float2* __restrict__ twL, int ncols, int col_base) {
+                    const float2* __restrict__ twL, int ncols) {
     extern __shared__ __align__(128) unsigned char smem_tma[];
     float2* s = reinterpret_cast<float2*>(smem_tma);
     float2* tw = s + L * W;
     unsigned long long* bar = reinterpret_cast<unsigned long long*>(tw + L);
     const int tid = threadIdx.x;
     constexpr int NT = 256;
-    const int c0 = col_base + blockIdx.x * W;
+    const int c0 = blockIdx.x * W;
     const int y = blockIdx.y;
     if (tid == 0) {
         mbar_init(bar, 1);
@@ -128,16 +125,14 @@ tile_fft_tma_kernel(const __grid_constant__ CUtensorMap tmap, Store st,
 }
 
 template <int L, int W, int DIR, int RANK, class Store>
-int launch_tile_fft_tma(const CUtensorMap& map, Store st, int ncols, int ny, cudaStream_t stream,
-                        int col_base = 0, int col_end = -1) {
+int launch_tile_fft_tma(const CUtensorMap& map, Store st, int ncols, int ny, cudaStream_t stream) {
     const float2* tw = twiddle_table<float>(L, DIR, stream);
     if (!tw) return SB_ERR_NOMEM;
-    if (col_end < 0 || col_end > ncols) col_end = ncols;
     auto kern = tile_fft_tma_kernel<L, W, DIR, RANK, Store>;
     const size_t smem = (size_t)(L * W + L) * sizeof(float2) + 16;
     SB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    dim3 grid((col_end - col_base + W - 1) / W, ny);
-    kern<<<grid, 256, smem, stream>>>(map, st, tw, col_end, col_base);
+    dim3 grid((ncols + W - 1) / W, ny);
+    kern<<<grid, 256, smem, stream>>>(map, st, tw, ncols);
     SB_LAUNCH_CHECK();
     return SB_OK;
 }
@@ -298,9 +293,8 @@ __global__ void __launch_bounds__(sizeof(T) == 4 ? 1024 : 512) row_fft_c2r_kerne
 inline int row_threads(int N, int elem_bytes = 8) {
     // N / 16 threads: one radix-16 butterfly per thread and pass, and two CTAs share an SM for
     // rows up to 8192 points, overlapping their load / transform / store phases (16384-point
-    // rows keep 1024 threads either way).  SB_ROW_DIV=8: the round-1 geometry (N / 8 threads)
-    static const int div = (getenv("SB_ROW_DIV") && atoi(getenv("SB_ROW_DIV")) == 8) ? 8 : 16;
-    int t = N / div;
+    // rows keep 1024 threads either way)
+    int t = N / 16;
     if (t < 32) t = 32;
     const int cap = elem_bytes <= 8 ? 1024 : 512;   // fp32 rows: 32 warps hide latency
     if (t > cap) t = cap;
@@ -393,5 +387,25 @@ inline void split_len(int R, int* R1, int* R2) {
     *R2 = R / *R1;
 }
 inline bool is_pow2(long v) { return v > 0 && (v & (v - 1)) == 0; }
+
+// generic strided-axis transform of a [R][pitch] complex array with plain-load
+// tile passes, functor on the final store: storeB(y=k1, k=k2, c, v)
+template <typename T, int DIR, class LoadA, class StoreB>
+static inline int cols_generic(LoadA la, cx<T>* tmp, long pitch, int R, int ncols,
+                        StoreB sb, cudaStream_t st) {
+    using C = cx<T>;
+    constexpr int W = 256 / sizeof(C);
+    int R1, R2;
+    split_len(R, &R1, &R2);
+    const C* wR = twiddle_table<T>(R, DIR, st);
+    if (!wR) return SB_ERR_NOMEM;
+    TwiddleAStore<C> sa{tmp, pitch, R2, R, wR};
+    int rc = SB_OK;
+    SB_TILE_DISPATCH(R1, rc = (launch_tile_fft<T, LL, W, DIR>(la, sa, ncols, R2, st)));
+    if (rc) return rc;
+    BlockBLoad<C> lb{tmp, pitch, R2};
+    SB_TILE_DISPATCH(R2, rc = (launch_tile_fft<T, LL, W, DIR>(lb, sb, ncols, R1, st)));
+    return rc;
+}
 
 }  // namespace sb

@@ -16,7 +16,7 @@
 
 #ifndef SB_HOST_EMU            // tests/host_emu runs the scatter / eigenpair kernels on the CPU
 #include "chisq.cuh"
-#include "fft_generic.cuh"
+#include "fft_kernels.cuh"
 #endif
 #include "lanczos.cuh"
 #include "thth.cuh"
@@ -903,13 +903,6 @@ int chisq_sweep(const ThthGeom& g, const double* th_host, const double* d_etas, 
 // the causality mask is applied to the unshifted rows; mask and amplitude are
 // fused into the final stores of the two column passes.
 // --------------------------------------------------------------------------
-template <typename C> struct PitchRowLoadC {
-    const C* in;
-    long pitch;
-    __device__ __forceinline__ C operator()(long row, int n) const {
-        return in[(size_t)row * pitch + n];
-    }
-};
 template <typename C> struct RowMaskStore {     // out[k][c] = rowmask[k] ? 0 : v,  k = k1 + R1 k2
     C* out;
     long pitch;
@@ -1004,7 +997,7 @@ static int gs_pow2(cx<T>* W, const float* amp, const unsigned char* rowmask, int
     split_len(n0, &R1, &R2);
     for (int it = 0; it < niter; ++it) {
         int rc = SB_OK;
-        PitchRowLoadC<C> l0{W, n1};
+        PitchRowLoad<C> l0{W, n1};
         PlainRowStore<C> s1{B[0], n1};
         SB_ROW_DISPATCH(n1, rc = (launch_row_c2c<T, N1, N2, -1>(l0, s1, n0, st)));
         if (rc) return rc;
@@ -1012,7 +1005,7 @@ static int gs_pow2(cx<T>* W, const float* amp, const unsigned char* rowmask, int
         RowMaskStore<C> ms{B[2], n1, R1, rowmask};
         rc = cols_generic<T, -1>(la, B[1], n1, n0, n1, ms, st);
         if (rc) return rc;
-        PitchRowLoadC<C> l3{B[2], n1};
+        PitchRowLoad<C> l3{B[2], n1};
         SB_ROW_DISPATCH(n1, rc = (launch_row_c2c<T, N1, N2, +1>(l3, s1, n0, st)));
         if (rc) return rc;
         AmplitudeStore<T> as{W, n1, R1, amp, (T)(1.0 / ((double)n0 * (double)n1))};
@@ -1147,7 +1140,7 @@ int conj_spectrum_c2c(const float2* in, int nf, int nt, int npad, float pad_re, 
         float2* B2 = (float2*)workspace(4, count * sizeof(float2));
         if (!B1 || !B2) return SB_ERR_NOMEM;
         int rc = SB_OK;
-        PitchRowLoadC<float2> lr{P, NT};
+        PitchRowLoad<float2> lr{P, NT};
         PlainRowStore<float2> rs{B1, NT};
         SB_ROW_DISPATCH(NT, rc = (launch_row_c2c<float, N1, N2, -1>(lr, rs, NF, st)));
         if (rc) return rc;

@@ -16,7 +16,6 @@
 #include <math.h>
 
 #include "fft_kernels.cuh"
-#include "fft_generic.cuh"
 
 namespace sb {
 
@@ -175,14 +174,6 @@ struct FieldALoad {   // exp(i * xyp * scale), x-axis pass A: y = r2, i = r1
         return make_float2(cc, s);
     }
 };
-struct NaturalBStore {   // out[k1 + R1 k2][c] = v
-    float2* out;
-    long pitch;
-    int R1;
-    __device__ __forceinline__ void operator()(int y, int k, int c, float2 v) const {
-        out[(size_t)(y + R1 * k) * pitch + c] = v;
-    }
-};
 
 // Fresnel filter tables for one frequency (frfilt3 :294-311):
 //   fx[kx] = exp(-i s ffconx kx'^2), kx' = min(kx, nx - kx)
@@ -262,13 +253,6 @@ struct SpeRowStore {   // spe_t[f][x] = z / (nx ny)
         spe[(size_t)row * nx + k] = make_float2(v.x * scale, v.y * scale);
     }
 };
-struct FullRowLoad {
-    const float2* in;
-    long pitch;
-    __device__ __forceinline__ float2 operator()(long row, int n) const {
-        return in[row * pitch + n];
-    }
-};
 struct PowerBStore {     // xyi[k][c] = |v|^2 * scale^2
     float* out;
     long pitch;
@@ -311,7 +295,7 @@ int sim_intensity(int nx, int ny, int nf, const double* xyp, const double* scale
         SB_LAUNCH_CHECK();
         // x axis (strided): exp(i phi s) fused into the first load
         FieldALoad la{xyp, ny, R2, scale};
-        NaturalBStore nb{B2, ny, R1};
+        NaturalBStore<float2> nb{B2, ny, R1};
         int rc = cols_generic<float, -1>(la, B1, ny, nx, ny, nb, st);
         if (rc) return rc;
         // y axis (contiguous) + filtered reduction over ky
@@ -325,7 +309,7 @@ int sim_intensity(int nx, int ny, int nf, const double* xyp, const double* scale
         SB_LAUNCH_CHECK();
         if (last) {
             // full inverse of the filtered spectrum (in B1): rows then columns
-            FullRowLoad fl{B1, ny};
+            PitchRowLoad<float2> fl{B1, ny};
             PlainRowStore<float2> ps{B2, ny};
             SB_ROW_DISPATCH(ny, rc = (launch_row_c2c<float, N1, N2, +1>(fl, ps, nx, st)));
             if (rc) return rc;

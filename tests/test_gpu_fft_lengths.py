@@ -2,7 +2,7 @@
 DFTs, and every size limit of the entry points from both sides.
 
 Every product output goes through one set of FFT templates chosen by length
-(fft_core.cuh, fft_kernels.cuh, fft_generic.cuh, chirp.cuh):
+(fft_core.cuh, fft_kernels.cuh, fft_functors.cuh):
   rows     one CTA per row in shared memory, N = 8 .. 16384 (SB_ROW_DISPATCH),
            r2c / c2r / c2c, fp32 and fp64;
   columns  R = 4 .. 65536 split by split_len into two tile passes R1 x R2 with
@@ -103,7 +103,7 @@ def templates(case):
         r1, r2 = split_len(R)
         out.update({("col", tag, prec, R, load), ("tile", prec, r1), ("tile", prec, r2)})
 
-    def chirp(tag, n0, n1):       # conj_spectrum_bluestein / ifft2_c2c_any
+    def chirp(tag, n0, n1):       # chirp_fft2 (conj_spectrum / ifft2_c2c_any)
         mt, mf = next_pow2(2 * n1 - 1), next_pow2(2 * n0 - 1)
         out.add(("row", tag, "c2c", "f32", mt))
         cols(tag, "f32", mf, "plain")
@@ -865,7 +865,7 @@ def test_size_limit(what, bad, words, ok):
     run_case(min((c for c in CASES if c.entry == bad.entry), key=case_size))
 
 
-# TMA-eligible shapes: the fetch path and the row-thread layout must not change a bit
+# TMA-eligible shapes: the fetch path must not change a bit
 BITWISE_CASES = [
     _c("sspec", nf=64, nt=4096, window=False, halve=1, prewhite=0),
     _c("sspec", nf=2048, nt=100, window=False, halve=0, prewhite=0),
@@ -879,13 +879,13 @@ BITWISE_CASES = [
 @pytest.mark.gpu
 def test_load_paths_bit_identical(tmp_path):
     """The fp32 transforms round every operation explicitly (fft_core.cuh), so the
-    TMA and plain-load column passes and the N/16 and N/8 row-thread layouts
-    compute the same bits.  Both switches are read once per process."""
+    TMA and plain-load column passes compute the same bits.  The switch is read
+    once per process."""
     for c in BITWISE_CASES:
         assert any(t[0] == "col" and t[-1] == "tma" for t in templates(c)), case_id(c)
     here = [run_device(c) for c in BITWISE_CASES]
     out = tmp_path / "alt.npz"
-    env = dict(os.environ, SB_FFT_NO_TMA="1", SB_ROW_DIV="8",
+    env = dict(os.environ, SB_FFT_NO_TMA="1",
                PYTHONPATH=ROOT + os.pathsep + os.environ.get("PYTHONPATH", ""))
     r = subprocess.run([sys.executable, os.path.abspath(__file__), "--device-outputs", str(out)],
                        env=env, cwd=ROOT, capture_output=True, text=True, timeout=600)
@@ -893,20 +893,6 @@ def test_load_paths_bit_identical(tmp_path):
     alt = np.load(out)
     for i, c in enumerate(BITWISE_CASES):
         assert np.array_equal(here[i], alt["arr_%d" % i]), case_id(c)
-
-
-@pytest.mark.gpu
-def test_column_chunks_bit_identical(monkeypatch):
-    """SB_COL_CHUNK_MB=1 at 512 x 1024: five column chunks, the last one column
-    wide, give the same bits as one pass."""
-    c = _c("sspec", nf=512, nt=1024, window=False, halve=1, prewhite=0)
-    x = sspec_inputs(c)
-    whole = sspec_device(c, x)
-    monkeypatch.setenv("SB_COL_CHUNK_MB", "1")
-    chunked = sspec_device(c, x)
-    monkeypatch.delenv("SB_COL_CHUNK_MB")
-    assert np.array_equal(whole, chunked)
-    sspec_check(c, x, chunked)
 
 
 if __name__ == "__main__":

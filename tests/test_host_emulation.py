@@ -58,24 +58,51 @@ def test_scale_dyn_kernels_on_host(golden_dir, flip):
     assert np.abs(out - ref).max() < 1e-5 * np.abs(ref).max()
 
 
-@pytest.mark.parametrize("n0,n1,c0,c1", [(12, 10, 0, 0), (9, 20, 5, 7), (16, 15, 16, 4)])
-def test_chirp_ifft2_functors_on_host(n0, n1, c0, c1):
-    """The chirp-z any-size inverse FFT (dynspec.cu::ifft2_c2c_any): tables and
-    load / store functors of csrc/chirp.cuh around a reference DFT reproduce
-    numpy's ifft2(ifftshift(x)) (and ifft2(conj x) for the Gerchberg-Saxton
-    forward step), crop and scale included."""
-    src = os.path.join(EMU, "chirp_ifft2_emu.cpp")
-    out = os.path.join(EMU, "_build", "chirp_ifft2_emu.so")
+CHIRP_CASES = [("ifft2", (12, 10, 0, 0)), ("ifft2", (9, 20, 5, 7)), ("ifft2", (16, 15, 16, 4)),
+               ("cs", (6, 5, 1, 0)), ("cs", (5, 12, 0, 1)), ("cs", (7, 9, 2, 1))]
+
+
+@pytest.mark.parametrize("entry,shape", CHIRP_CASES,
+                         ids=[e + "-" + "-".join(map(str, s)) for e, s in CHIRP_CASES])
+def test_chirp_fft2_functors_on_host(entry, shape):
+    """The chirp-z any-size 2-D FFT (dynspec.cu::chirp_fft2): tables and load /
+    store functors of csrc/fft_functors.cuh around a reference DFT reproduce
+      ifft2: numpy's ifft2(ifftshift(x)) (and ifft2(conj x) for the
+             Gerchberg-Saxton forward step), crop and scale included
+             (shape = n0, n1, crop0, crop1);
+      cs:    the conjugate spectrum of a constant-padded chunk, fftshift, DC
+             correction and tau row mask included (shape = nf, nt, npad, masked)."""
+    src = os.path.join(EMU, "chirp_fft2_emu.cpp")
+    out = os.path.join(EMU, "_build", "chirp_fft2_emu.so")
     os.makedirs(os.path.dirname(out), exist_ok=True)
     subprocess.run(["g++", "-O2", "-std=c++17", "-shared", "-fPIC", "-x", "c++", src, "-o", out],
                    check=True)
     lib = ctypes.CDLL(out)
+    P = lambda a: a.ctypes.data_as(ctypes.c_void_p)
+    if entry == "cs":
+        from oracle import thth_oracle as TO
+        nf, nt, npad, masked = shape
+        NF, NT = (npad + 1) * nf, (npad + 1) * nt
+        lib.emu_cs_any.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 4 + \
+            [ctypes.c_float, ctypes.c_void_p, ctypes.c_void_p]
+        rng = np.random.default_rng(nf * 100 + nt)
+        dyn = rng.normal(size=(nf, nt)).astype(np.float32)
+        pad = np.float32(0.375)
+        rowmask = np.zeros(NF, np.uint8)
+        if masked:
+            rowmask[NF // 2 - 1:NF // 2 + 2] = 1
+        got = np.zeros((NF, NT), np.complex64)
+        lib.emu_cs_any(P(dyn), nf, nt, NF, NT, pad, P(rowmask), P(got))
+        ref = TO.conjugate_spectrum(dyn, npad, float(pad))
+        ref[rowmask.astype(bool)] = 0
+        assert np.abs(got - ref).max() < 2e-5 * np.abs(ref).max()
+        return
+    n0, n1, c0, c1 = shape
     lib.emu_ifft2_any.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 5 + [ctypes.c_double] + \
         [ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
     rng = np.random.default_rng(n0 * 100 + n1)
     x = (rng.normal(size=(n0, n1)) + 1j * rng.normal(size=(n0, n1))).astype(np.complex64)
     cc0, cc1 = (c0 or n0), (c1 or n1)
-    P = lambda a: a.ctypes.data_as(ctypes.c_void_p)
     got = np.zeros((cc0, cc1), np.complex64)
     lib.emu_ifft2_any(P(x), n0, n1, 1, c0, c1, 3.0, 0, 0, P(got))
     ref = 3.0 * np.fft.ifft2(np.fft.ifftshift(x))[:cc0, :cc1]
