@@ -49,7 +49,8 @@ int sb_release(void);
 /* Per-kernel timing with CUDA events recorded on the launching stream.
  * Slots: 0 cs_rows 1 cs_colA 2 cs_colB 3 thth_prep 4 thth_build 5 thth_eig
  * 6 sspec 7 acf 8 sim_screen 9 sim_freq 10 mosaic_tile 11 mosaic_reduce
- * 12 svd_gram (one A^T A pass of sb_svd_topk) 13 svd_apply.
+ * 12 svd_gram (one A^T A pass of sb_svd_topk) 13 svd_apply 14 slow_ft_doppler (the three
+ * column transforms of sb_slow_ft_f32) 15 slow_ft_delay (its row transform).
  * sb_profile_collect synchronises the
  * device, writes accumulated milliseconds and launch counts (host arrays of
  * at least 16 entries) and resets the accumulators. */
@@ -462,6 +463,22 @@ int sb_bandpass_cols(const float* A, int32_t nf, int32_t nt, int32_t zero_as_nan
                      const double* rowdiv, double* mean, void* stream);
 int sb_bandpass_divide(const float* A, int32_t nf, int32_t nt, int32_t zero_as_nan,
                        const double* rowdiv, const double* coldiv, float* out, void* stream);
+
+/* ---- frequency-scaled Doppler transform ----------------------------------- */
+
+/* scint_utils.slow_FT (scint_utils.py:655-702, with its fftshift keyword read as axes=0).
+ * x: device float32 [ntime][nfreq] (time-major); fscale: device float64 [nfreq], f / fref;
+ * out: device float2 [ntime][nfreq].  With c = ntime / 2,
+ *   out[m][j] = sum_f sum_t x[t][f] exp(-2 pi i fscale[f] t (m - c) / ntime)
+ *                                   exp(-2 pi i f (j - nfreq/2) / nfreq).
+ * Shapes 1..32768 x 1..8192, else SB_ERR_UNSUPPORTED.  A non-finite x or fscale makes
+ * every output non-finite.  Asynchronous on `stream`; no atomics, so repeated calls are
+ * bit-identical.  Device memory: two grow-only workspace planes of M x nfreq complex64
+ * (M = 2^ceil(log2(2 ntime - 1)), at least 8), 8 GiB at 32768 x 8192; a nfreq that is not
+ * a power of two >= 8 adds ntime x MT complex64 (MT = 2^ceil(log2(2 nfreq - 1))), at most
+ * 4 GiB.  The workspace stays allocated until sb_release. */
+int sb_slow_ft_f32(const float* x, int32_t ntime, int32_t nfreq, const double* fscale, void* out,
+                   void* stream);
 
 /* ---- scint_sim.Simulation ------------------------------------------------ */
 

@@ -98,6 +98,7 @@ _SIGS = {
     "sb_bandpass_rows": (c_int, [vp, c_int, c_int, c_int, vp, vp]),
     "sb_bandpass_cols": (c_int, [vp, c_int, c_int, c_int, vp, vp, vp]),
     "sb_bandpass_divide": (c_int, [vp, c_int, c_int, c_int, vp, vp, vp, vp]),
+    "sb_slow_ft_f32": (c_int, [vp, c_int, c_int, vp, vp, vp]),
     "sb_sim_weights": (c_int, [ctypes.POINTER(SimParams), vp, vp]),
     "sb_sim_screen": (c_int, [c_int, c_int, vp, vp, vp, ctypes.c_uint64, vp, vp]),
     "sb_sim_intensity": (c_int, [c_int, c_int, c_int, vp, vp, c_dbl, c_dbl, vp,

@@ -184,6 +184,8 @@ int bandpass_cols(const float* A, int nf, int nt, int zero_as_nan, const double*
 int bandpass_divide(const float* A, int nf, int nt, int zero_as_nan, const double* rowdiv,
                     const double* coldiv, float* out, cudaStream_t st);
 
+int slow_ft(const float* x, int nt, int nf, const double* s, float2* out, cudaStream_t st);
+
 int gerchberg_saxton(float2* W, const float* amp, const unsigned char* rowmask, int n0, int n1,
                      int niter, cudaStream_t st);
 
@@ -231,7 +233,7 @@ static int to_geom(const sb_thth_geom* in, ThthGeom* g) {
 
 extern "C" {
 
-int sb_abi_version(void) { return 7; }
+int sb_abi_version(void) { return 8; }
 const char* sb_last_error(void) { return sb::last_error(); }
 
 int sb_init(int device) {
@@ -568,6 +570,12 @@ int sb_bandpass_cols(const float* A, int32_t nf, int32_t nt, int32_t zero_as_nan
 int sb_bandpass_divide(const float* A, int32_t nf, int32_t nt, int32_t zero_as_nan,
                        const double* rowdiv, const double* coldiv, float* out, void* stream) {
     return sb::bandpass_divide(A, nf, nt, zero_as_nan, rowdiv, coldiv, out, (cudaStream_t)stream);
+}
+
+int sb_slow_ft_f32(const float* x, int32_t ntime, int32_t nfreq, const double* fscale, void* out,
+                   void* stream) {
+    SB_ARG(x && fscale && out);
+    return sb::slow_ft(x, ntime, nfreq, fscale, (float2*)out, (cudaStream_t)stream);
 }
 
 int sb_convert_f64_f32(const double* src, float* dst, int64_t n, void* stream) {

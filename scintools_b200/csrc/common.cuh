@@ -23,7 +23,7 @@ int num_sms();
 enum ProfId { PROF_CS_ROWS = 0, PROF_CS_COLA, PROF_CS_COLB, PROF_THTH_PREP,
               PROF_THTH_BUILD, PROF_THTH_EIG, PROF_SSPEC, PROF_ACF, PROF_SIM_SCREEN,
               PROF_SIM_FREQ, PROF_MOSAIC_TILE, PROF_MOSAIC_REDUCE, PROF_SVD_GRAM,
-              PROF_SVD_APPLY, PROF_COUNT };
+              PROF_SVD_APPLY, PROF_SFT_DOPPLER, PROF_SFT_DELAY, PROF_COUNT };
 void prof_begin(int id, cudaStream_t st);
 void prof_end(int id, cudaStream_t st);
 struct ProfScope {

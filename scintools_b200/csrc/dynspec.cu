@@ -361,12 +361,6 @@ int stats_pass(const float* dyn, int nf, int nt, const float* wt, const float* w
                double swt, double swf, double* stats, cudaStream_t st);
 static long half_pitch(long NT) { return ((NT / 2 + 1) + 15) & ~15L; }
 
-static int next_pow2(long v) {
-    int p = 1;
-    while (p < v) p <<= 1;
-    return p;
-}
-
 // rows: real dyn [nf_live][*] -> H[nf_live][pitch] half spectra of length NT
 static int rows_r2c(const DynRowLoad& ld, float2* H, long pitch, int NT,
                     long nrows, cudaStream_t st, int kmax = 1 << 30) {
@@ -641,8 +635,7 @@ int conj_spectrum_bound(const float* dyn, int nf, int nt, int npad, float pad_va
 // Chirp tables and the load / store functors of these passes: fft_functors.cuh
 // ------------------------------------------------------------------------
 // chirp w[N] and the transformed kernel B = FFT_M(b)
-static int bluestein_tables(int N, int M, float2* w, float2* B, float2* scratch,
-                            cudaStream_t st) {
+int bluestein_tables(int N, int M, float2* w, float2* B, float2* scratch, cudaStream_t st) {
     chirp_fill_kernel<<<(M + 255) / 256, 256, 0, st>>>(w, B, N, M);
     SB_LAUNCH_CHECK();
     if (M <= 16384) {
@@ -695,16 +688,9 @@ static int chirp_fft2(RowLoad ld, int n0, int n1, int live, int ncols, MakeStore
     rc = bluestein_tables(n0, MF, wF, BF, scratch, st);
     if (rc) return rc;
     // rows: chirp, FFT, multiply, inverse FFT, chirp
-    {
-        ld.w = wT;
-        MulVecRowStore ms{R1buf, MT, BT};
-        SB_ROW_DISPATCH(MT, rc = (launch_row_c2c<float, N1, N2, -1>(ld, ms, live, st)));
-        if (rc) return rc;
-        PitchRowLoad<float2> pl{R1buf, MT};
-        ChirpOutRowStore os{Ybuf, pt, wT, n1, 1.0f / (float)MT};
-        SB_ROW_DISPATCH(MT, rc = (launch_row_c2c<float, N1, N2, +1>(pl, os, live, st)));
-        if (rc) return rc;
-    }
+    rc = chirp_rows(ld, ChirpOutRowStore{Ybuf, pt, wT, n1, 1.0f / (float)MT}, R1buf, MT, live,
+                    wT, BT, st);
+    if (rc) return rc;
     // columns
     int R1, R2;
     split_len(MF, &R1, &R2);

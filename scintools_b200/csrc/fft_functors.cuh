@@ -1,5 +1,5 @@
 // Load / store functors of the FFT passes, shared by every transform driver
-// (dynspec.cu, retrieval.cu, sim.cu), and the chirp-z (Bluestein) tables.
+// (dynspec.cu, retrieval.cu, sim.cu, slow_ft.cu), and the chirp-z (Bluestein) tables.
 // Row kernels: load(row, n), store(row, k, v).  Tile kernels (four-step column
 // pass): load(y, i, c), store(y, k, c, v).  Barrier-free, so tests/host_emu can
 // compile this header for the CPU (SB_HOST_EMU) and check the index /
@@ -205,6 +205,81 @@ struct ChirpCropStore {  // out[k][c] = conj(v * wF[k]) * scale, k < crop0, c < 
         const size_t o = (size_t)kf * crop1 + c;
         if (outr) outr[o] = r.x * scale;
         else outc[o] = make_float2(r.x * scale, -r.y * scale);
+    }
+};
+
+// ------------------------------------------- frequency-scaled chirp-z (slow_ft.cu)
+// Each column c (channel) has its own chirp rate s[c] / nt, not a multiple of 1 / nt, so
+// the chirps are generated here instead of read from tables.
+// exp(i pi s q / n) for an integer |q| < 2^31 (exact in float64): the phase is reduced mod
+// 2 in float64 (x - 2 floor(x / 2) is exact) before sincospi; at |x| ~ 4e4 a float32
+// phase would be off by ~0.03 rad.  A non-finite s gives NaN.
+__device__ __forceinline__ float2 chirp_pi(double s, long long q, int n) {
+    const double x = s * (double)q / (double)n;
+    double sn, cs;
+    sincospi(x - 2.0 * floor(0.5 * x), &sn, &cs);
+    return make_float2((float)cs, (float)sn);
+}
+struct SlowKernelColLoad {   // y = r2, i = r1: b_c[n] = exp(+i pi s[c] n^2 / nt), |n| < nt, mod M
+    int R2, M, nt;
+    const double* s;
+    __device__ __forceinline__ float2 operator()(int y, int i, int c) const {
+        const int n = i * R2 + y;
+        const int m = n < nt ? n : (M - n < nt ? M - n : -1);
+        if (m < 0) return make_float2(0.f, 0.f);
+        return chirp_pi(s[c], (long long)m * m, nt);
+    }
+};
+struct SlowChirpColLoad {    // y = r2, i = r1: x[t][c] exp(-i pi s[c] (t^2 - 2 (nt/2) t) / nt)
+    const float* x;          // [nt][nf]; rows t >= nt are the zero padding
+    int nf, nt, R2;
+    const double* s;
+    __device__ __forceinline__ float2 operator()(int y, int i, int c) const {
+        const int t = i * R2 + y;
+        if (t >= nt) return make_float2(0.f, 0.f);
+        const float v = x[(size_t)t * nf + c];
+        const float2 w = chirp_pi(-s[c], (long long)t * (t - 2 * (nt / 2)), nt);
+        return make_float2(v * w.x, v * w.y);
+    }
+};
+struct MulPlaneColStore {    // B[k][c] = v * B[k][c], k = k1 + R1 k2 (in place: one thread per element)
+    float2* B;
+    long pitch;
+    int R1;
+    __device__ __forceinline__ void operator()(int y, int k, int c, float2 v) const {
+        const size_t o = (size_t)(y + R1 * k) * pitch + c;
+        B[o] = cmul(v, B[o]);
+    }
+};
+struct SlowChirpOutColStore {   // out[m][c] = v exp(-i pi s[c] m^2 / nt) * scale, m < nt
+    float2* out;
+    int nf, nt, R1;
+    const double* s;
+    float scale;
+    __device__ __forceinline__ void operator()(int y, int k, int c, float2 v) const {
+        const int m = y + R1 * k;
+        if (m >= nt) return;
+        const float2 r = cmul(v, chirp_pi(-s[c], (long long)m * m, nt));
+        out[(size_t)m * nf + c] = make_float2(r.x * scale, r.y * scale);
+    }
+};
+struct ShiftRowStore {       // out[row][(k + N/2) % N] = v: the fftshift of a row
+    float2* out;
+    int N;
+    __device__ __forceinline__ void operator()(long row, int k, float2 v) const {
+        out[row * N + (k + N / 2) % N] = v;
+    }
+};
+struct ChirpShiftRowStore {  // out[row][(k + N/2) % N] = v * w[k] * scale, k < N
+    float2* out;
+    int N;
+    const float2* w;
+    float scale;
+    __device__ __forceinline__ void operator()(long row, int k, float2 v) const {
+        if (k < N) {
+            const float2 r = cmul(v, w[k]);
+            out[row * N + (k + N / 2) % N] = make_float2(r.x * scale, r.y * scale);
+        }
     }
 };
 

@@ -387,6 +387,11 @@ inline void split_len(int R, int* R1, int* R2) {
     *R2 = R / *R1;
 }
 inline bool is_pow2(long v) { return v > 0 && (v & (v - 1)) == 0; }
+inline int next_pow2(long v) {
+    int p = 1;
+    while (p < v) p <<= 1;
+    return p;
+}
 
 // generic strided-axis transform of a [R][pitch] complex array with plain-load
 // tile passes, functor on the final store: storeB(y=k1, k=k2, c, v)
@@ -405,6 +410,27 @@ static inline int cols_generic(LoadA la, cx<T>* tmp, long pitch, int R, int ncol
     if (rc) return rc;
     BlockBLoad<C> lb{tmp, pitch, R2};
     SB_TILE_DISPATCH(R2, rc = (launch_tile_fft<T, LL, W, DIR>(lb, sb, ncols, R1, st)));
+    return rc;
+}
+
+// chirp-z (Bluestein) tables of length N, padded length M (8 <= M <= 65536): the chirp
+// w[N] and the transformed kernel B = FFT_M(b); scratch holds 2 M points (dynspec.cu)
+int bluestein_tables(int N, int M, float2* w, float2* B, float2* scratch, cudaStream_t st);
+
+// Row half of a chirp-z transform: every one of nrows rows read by ld (its chirp w is set
+// here) is chirped, transformed at length MT, multiplied by BT, inverse transformed into
+// buf [nrows][MT] and back; os(row, k, v) receives bin k < MT of the unnormalised inverse,
+// before the output chirp w[k] and the 1 / MT.
+template <class RowLoad, class Store>
+static inline int chirp_rows(RowLoad ld, Store os, float2* buf, int MT, long nrows,
+                             const float2* wT, const float2* BT, cudaStream_t st) {
+    ld.w = wT;
+    MulVecRowStore ms{buf, MT, BT};
+    int rc = SB_OK;
+    SB_ROW_DISPATCH(MT, rc = (launch_row_c2c<float, N1, N2, -1>(ld, ms, nrows, st)));
+    if (rc) return rc;
+    PitchRowLoad<float2> pl{buf, MT};
+    SB_ROW_DISPATCH(MT, rc = (launch_row_c2c<float, N1, N2, +1>(pl, os, nrows, st)));
     return rc;
 }
 
