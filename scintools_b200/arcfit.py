@@ -57,12 +57,20 @@ def fit_log_parabola(x, y):
 def norm_rows_device(sspec, fdop, tdel, eta, maxnormfac, fdopnew, weights_fn, want_2d=True):
     """Resample + scrunch on the GPU.  ``weights_fn(power) -> weights [nr]`` runs on
     the host between the two kernels (the reference derives the weights from the
-    per-row power spectrum).  Returns (norm [nr][nq] float64 with NaN where masked
-    or None, power [nr], avg [nq] with NaN where fully masked)."""
+    per-row power spectrum); it may return ``(weights, rows)`` instead, a boolean
+    selection of the rows that enter the average (the others are left out, not given
+    a zero weight, which would turn a +-inf sample into NaN).  Returns (norm [nr][nq]
+    float64 with NaN where masked or None, power [nr], avg [nq] with NaN where the
+    weights sum to zero)."""
     import torch
     sspec = np.ascontiguousarray(sspec)
     nr, nc = sspec.shape
     nq = int(np.shape(fdopnew)[0])
+    # np.interp raises on a row with no selected sample (a NaN sqrt(tdel / eta), e.g. the
+    # delay-zero row at eta = 0); the kernel would return it fully masked instead
+    imax = maxnormfac * np.sqrt(np.asarray(tdel, dtype=np.float64) / eta)
+    if not np.all(np.min(np.abs(fdop)) <= imax):
+        raise ValueError("array of sample points is empty")
     d_s = D.upload_f32(sspec)
     d_fd = D.upload(np.ascontiguousarray(fdop, dtype=np.float64))
     d_td = D.upload(np.ascontiguousarray(tdel, dtype=np.float64))
@@ -74,14 +82,28 @@ def norm_rows_device(sspec, fdop, tdel, eta, maxnormfac, fdopnew, weights_fn, wa
                                           d_fn.data_ptr(), nq, d_out.data_ptr(),
                                           d_pow.data_ptr(), D.stream_ptr()))
     power = d_pow.cpu().numpy()
-    weights = np.ascontiguousarray(weights_fn(power), dtype=np.float64)
+    weights, rows = weights_fn(power), None
+    if isinstance(weights, tuple):
+        weights, rows = weights
+    weights = np.ascontiguousarray(weights, dtype=np.float64)
     if weights.shape != (nr,):
         raise ValueError("norm_sspec: weights must have one entry per delay row")
-    d_w = D.upload(weights)
-    d_avg = D.empty((nq,), torch.float64)
-    _lib.check(_lib.lib.sb_norm_sspec_avg_f32(d_out.data_ptr(), nr, nq, d_w.data_ptr(),
-                                              d_avg.data_ptr(), D.stream_ptr()))
-    avg = d_avg.cpu().numpy()
+    d_in = d_out
+    if rows is not None:
+        rows = np.asarray(rows, dtype=bool)
+        if not rows.all():          # the rows the average reads, gathered in order
+            d_in = d_out.index_select(0, torch.as_tensor(np.flatnonzero(rows),
+                                                         device=d_out.device))
+            weights = np.ascontiguousarray(weights[rows])
+    if d_in.shape[0] == 0:          # no row: every weight sum is zero
+        avg = np.full(nq, np.nan)
+    else:
+        d_w = D.upload(weights)
+        d_avg = D.empty((nq,), torch.float64)
+        _lib.check(_lib.lib.sb_norm_sspec_avg_f32(d_in.data_ptr(), d_in.shape[0], nq,
+                                                  d_w.data_ptr(), d_avg.data_ptr(),
+                                                  D.stream_ptr()))
+        avg = d_avg.cpu().numpy()
     norm = d_out.cpu().numpy().astype(np.float64) if want_2d else None
     return norm, power, avg
 
@@ -172,7 +194,14 @@ class ArcFitMixin:
             state["weights"] = w
             wdev = np.array(np.ma.filled(w, 0.0), dtype=np.float64)
             if powerspec_cut:       # np.ma.average over the rows with arc_spectrum > wn only
-                wdev = np.where(np.ma.filled(arc_spectrum > wn, False), wdev, 0.0)
+                keep = np.ma.filled(arc_spectrum > wn, False)
+                if np.count_nonzero(keep) == 1:
+                    # the reference squeezes the weights of a single row to a scalar, and
+                    # np.ma.average rejects them (dynspec.py:2172-2175)
+                    raise ValueError("Shape of weights must be consistent with shape of a "
+                                     "along specified axis.")
+                # np.ma.average(normSspec[indices, :]): the other rows are not read
+                return wdev, keep
             return wdev
 
         norm, power, avg = _norm_rows(sspec, fdop, tdel, eta, maxnormfac, fdopnew, weights_fn)
@@ -180,10 +209,13 @@ class ArcFitMixin:
         self.mask = mask
         self.powerspectrum = state["powerspectrum"]
         self.weights = state["weights"]
-        # np.ma.average leaves 0.0 under the mask of a fully masked column; fit_arc's
-        # np.array(masked) then sees that data (not NaN), so keep it identical
+        # np.ma.average divides with numpy.ma's safe division, which masks a quotient whose
+        # numerator is not small against its denominator: a zero weight sum (the device's
+        # NaN; 0.0 is left under the mask) and the +-inf sum of a column holding a +-inf
+        # sample (the infinity is left under the mask).  fit_arc's np.array(masked) then
+        # sees that data, so keep it identical
         gone = np.isnan(avg)
-        self.normsspecavg = np.ma.array(np.where(gone, 0.0, avg), mask=gone)
+        self.normsspecavg = np.ma.array(np.where(gone, 0.0, avg), mask=gone | np.isinf(avg))
         self.normsspec = np.ma.array(norm, mask=mask)
         self.normsspec_tdel = tdel
         self.normsspec_fdop = fdopnew

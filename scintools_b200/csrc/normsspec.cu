@@ -7,7 +7,7 @@
 //   row ii :  s = sqrt(tdel[ii] / eta);  sel = |fdop| <= maxnormfac * s
 //             normline = np.interp(fdopnew, fdop[sel] / s, sspec[ii, sel])
 //             mask     = |fdopnew| > max|fdop[sel] / s|   (or NaN result)
-//   powerspectrum[ii] = masked mean of 10^(normline / 10)            (:2120)
+//   powerspectrum[ii] = masked mean of 10^(normline / 10), finite samples only (:2127)
 //   normsspecavg[j]   = masked weighted average over the rows         (:2166)
 //
 // All axis arithmetic is fp64 with numpy's own expressions (same selections,
@@ -24,6 +24,9 @@ namespace sb {
 __device__ __forceinline__ double interp_one(const float* __restrict__ row,
                                              const double* __restrict__ fdop, int lo, int len,
                                              double s, double dfd, double x) {
+    // one sample: numpy returns it for every x, NaN included (its one-point branch makes
+    // no NaN check); longer rows map NaN to NaN
+    if (len == 1) return (double)row[lo];
     if (x != x) return x;
     const double x0 = __ddiv_rn(fdop[lo], s), xl = __ddiv_rn(fdop[lo + len - 1], s);
     if (x < x0) return (double)row[lo];
@@ -80,7 +83,9 @@ norm_sspec_rows_kernel(const float* __restrict__ sspec, int nc, const double* __
             double r = interp_one(row, fdop, lo, len, s, dfd, x);
             const bool masked = (fabs(x) > amax) || (r != r);
             out[(size_t)ii * nq + j] = masked ? qnan : (float)r;
-            if (!masked) { psum += pow(10.0, r / 10.0); ++pcnt; }
+            // the reference's np.power(10, normSspec / 10) divides with numpy.ma's safe
+            // division, which masks +-inf samples: their terms are left out of the mean
+            if (!masked && isfinite(r)) { psum += pow(10.0, r / 10.0); ++pcnt; }
         }
     } else {
         for (int j = tid; j < nq; j += blockDim.x) out[(size_t)ii * nq + j] = qnan;

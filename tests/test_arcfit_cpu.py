@@ -12,7 +12,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def numpy_norm_rows(sspec, fdop, tdel, eta, maxnormfac, fdopnew, weights_fn, want_2d=True):
-    """dynspec.py:2076-2166 in numpy (oracle/dynspec_oracle.norm_sspec's loop)."""
+    """dynspec.py:2076-2166 in numpy (oracle/dynspec_oracle.norm_sspec's loop).  avg is
+    what the device returns: the weighted mean of the unmasked samples, +-inf where one
+    of them is infinite (np.ma.average masks those), NaN where the weights sum to zero."""
     rows, mask = [], []
     for ii in range(len(tdel)):
         s = np.sqrt(tdel[ii] / eta)
@@ -22,11 +24,17 @@ def numpy_norm_rows(sspec, fdop, tdel, eta, maxnormfac, fdopnew, weights_fn, wan
         mask.append(np.abs(fdopnew) > np.max(np.abs(ifdop)))
     norm = np.array(rows).squeeze()
     mask = np.array(mask).squeeze() + np.isnan(norm)
-    nm = np.ma.array(norm, mask=mask)
+    nm = nm_all = np.ma.array(norm, mask=mask)
     power = np.ma.filled(np.ma.mean(np.power(10, nm / 10), axis=1), np.nan)
     w = weights_fn(power)
-    avg = np.ma.filled(np.ma.average(nm, axis=0, weights=w), np.nan)
-    return np.ma.filled(nm, np.nan), power, avg
+    if isinstance(w, tuple):        # (weights, rows): only the selected rows are averaged
+        w, rows = w
+        nm, w = nm[np.asarray(rows, dtype=bool)], np.asarray(w)[np.asarray(rows, dtype=bool)]
+    if np.ndim(nm) == 2 and nm.shape[0] == 0:
+        return np.ma.filled(nm_all, np.nan), power, np.full(np.shape(fdopnew)[0], np.nan)
+    a = np.ma.average(nm, axis=0, weights=w)
+    avg = np.where(np.ma.getmaskarray(a) & ~np.isinf(np.ma.getdata(a)), np.nan, np.ma.getdata(a))
+    return np.ma.filled(nm_all, np.nan), power, avg
 
 
 @pytest.fixture()
