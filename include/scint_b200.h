@@ -480,6 +480,36 @@ int sb_bandpass_divide(const float* A, int32_t nf, int32_t nt, int32_t zero_as_n
 int sb_slow_ft_f32(const float* x, int32_t ntime, int32_t nfreq, const double* fscale, void* out,
                    void* stream);
 
+/* ---- gap filling ---------------------------------------------------------- */
+
+/* Dynspec.refill (dynspec.py:3273-3323), method='biharmonic': the inpainting of
+ * skimage.restoration.inpaint_biharmonic (split_into_regions=False), solved on the device.
+ * img: device float64 [nf][nt], read only at known pixels; pix: device int32 [n], the
+ * masked pixels (flat row-major indices, ascending, 1 <= n <= nf nt).  Row k of the system
+ * is S = laplace(laplace(e_p)) (scipy.ndimage, mode 'reflect') on the 5x5 box around pix[k]
+ * clipped to the image; masked neighbours are unknowns, known ones go to the right-hand
+ * side.  The caller supplies the stencils: rcls uint8 [nf] and ccls uint8 [nt] give each
+ * row's / column's class (< nrc, < ncc, both <= 5), tables float64 [nrc][ncc][5][5] the
+ * stencil of each class pair centred on the pixel, zero outside the clipped box.
+ * Matrix-free BiCGSTAB with Jacobi scaling in float64 stops when ||b - A x|| <= tol ||b||
+ * (true residual) or after maxit steps; out: device float64 [n] = clip(x, lo, hi).
+ * info_host int32 [3]: steps, converged (0/1), restarts; resid_host [1]: the final
+ * ||b - A x|| / ||b||.  Synchronous (the host reads the state every 32 steps).  Shapes
+ * 1..32768 x 1..16384, else SB_ERR_UNSUPPORTED.  Fixed-order sums: repeated calls are
+ * bit-identical.  Workspace: 11 n + 3 maxit doubles and an nf x nt int32 map. */
+int sb_inpaint_biharmonic_f64(const double* img, int32_t nf, int32_t nt, const int32_t* pix,
+                              int32_t n, const double* tables, const uint8_t* rcls, int32_t nrc,
+                              const uint8_t* ccls, int32_t ncc, double lo, double hi, double tol,
+                              int32_t maxit, double* out, int32_t* info_host, double* resid_host,
+                              void* stream);
+/* Dynspec.refill(method='median'): out[k] = scipy.signal.medfilt(img', (kh, kw))[pix[k]],
+ * img' = img with NaN read as nan_value, zero padding outside the image; kh, kw odd, at
+ * most 31 (else SB_ERR_ARG / SB_ERR_UNSUPPORTED).  Exact (a median is one of the inputs).
+ * img float64 [nf][nt], pix int32 [n], out float64 [n], all on the device.  Shapes as
+ * sb_inpaint_biharmonic_f64. */
+int sb_medfilt_masked_f64(const double* img, int32_t nf, int32_t nt, const int32_t* pix, int32_t n,
+                          int32_t kh, int32_t kw, double nan_value, double* out, void* stream);
+
 /* ---- scint_sim.Simulation ------------------------------------------------ */
 
 typedef struct sb_sim_params {

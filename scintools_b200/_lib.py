@@ -99,6 +99,9 @@ _SIGS = {
     "sb_bandpass_cols": (c_int, [vp, c_int, c_int, c_int, vp, vp, vp]),
     "sb_bandpass_divide": (c_int, [vp, c_int, c_int, c_int, vp, vp, vp, vp]),
     "sb_slow_ft_f32": (c_int, [vp, c_int, c_int, vp, vp, vp]),
+    "sb_inpaint_biharmonic_f64": (c_int, [vp, c_int, c_int, vp, c_int, vp, vp, c_int, vp, c_int,
+                                          c_dbl, c_dbl, c_dbl, c_int, vp, vp, vp, vp]),
+    "sb_medfilt_masked_f64": (c_int, [vp, c_int, c_int, vp, c_int, c_int, c_int, c_dbl, vp, vp]),
     "sb_sim_weights": (c_int, [ctypes.POINTER(SimParams), vp, vp]),
     "sb_sim_screen": (c_int, [c_int, c_int, vp, vp, vp, ctypes.c_uint64, vp, vp]),
     "sb_sim_intensity": (c_int, [c_int, c_int, c_int, vp, vp, c_dbl, c_dbl, vp,

@@ -186,6 +186,14 @@ int bandpass_divide(const float* A, int nf, int nt, int zero_as_nan, const doubl
 
 int slow_ft(const float* x, int nt, int nf, const double* s, float2* out, cudaStream_t st);
 
+int inpaint_biharmonic(const double* img, int nf, int nt, const int* pix, int n,
+                       const double* tables, const unsigned char* rcls, int nrc,
+                       const unsigned char* ccls, int ncc, double lo, double hi, double tol,
+                       int maxit, double* out, int* info_host, double* resid_host,
+                       cudaStream_t st);
+int medfilt_masked(const double* img, int nf, int nt, const int* pix, int n, int kh, int kw,
+                   double nan_value, double* out, cudaStream_t st);
+
 int gerchberg_saxton(float2* W, const float* amp, const unsigned char* rowmask, int n0, int n1,
                      int niter, cudaStream_t st);
 
@@ -576,6 +584,20 @@ int sb_slow_ft_f32(const float* x, int32_t ntime, int32_t nfreq, const double* f
                    void* stream) {
     SB_ARG(x && fscale && out);
     return sb::slow_ft(x, ntime, nfreq, fscale, (float2*)out, (cudaStream_t)stream);
+}
+
+int sb_inpaint_biharmonic_f64(const double* img, int32_t nf, int32_t nt, const int32_t* pix,
+                              int32_t n, const double* tables, const uint8_t* rcls, int32_t nrc,
+                              const uint8_t* ccls, int32_t ncc, double lo, double hi, double tol,
+                              int32_t maxit, double* out, int32_t* info_host, double* resid_host,
+                              void* stream) {
+    return sb::inpaint_biharmonic(img, nf, nt, pix, n, tables, rcls, nrc, ccls, ncc, lo, hi, tol,
+                                  maxit, out, info_host, resid_host, (cudaStream_t)stream);
+}
+
+int sb_medfilt_masked_f64(const double* img, int32_t nf, int32_t nt, const int32_t* pix, int32_t n,
+                          int32_t kh, int32_t kw, double nan_value, double* out, void* stream) {
+    return sb::medfilt_masked(img, nf, nt, pix, n, kh, kw, nan_value, out, (cudaStream_t)stream);
 }
 
 int sb_convert_f64_f32(const double* src, float* dst, int64_t n, void* stream) {

@@ -9,12 +9,14 @@ the reference for the arc-measurement hot path:
   thetatheta_single  dynspec.py:1539-1655  -> sb_cs_f32 + sb_eta_sweep
   fit_thetatheta     dynspec.py:1657-1763  -> per chunk ththmod.single_search
 
-Everything outside that path (file I/O, cleaning, plotting, arc fitting,
+Everything outside that path (file I/O, cleaning other than refill, plotting, arc fitting,
 lmfit models) is deliberately not here: use the reference for those and hand
 the arrays over with ``BasicDyn`` exactly as the reference's tutorials do.
 Units: times in s, freqs in MHz, eta in s^3, edges in mHz, tau in us.
 
-Also here: correct_dyn (dynspec.py:3325-3410 -> sb_svd_topk + sb_svd_apply, or the
+Also here: refill (dynspec.py:3273-3323 -> sb_inpaint_biharmonic_f64 or
+sb_medfilt_masked_f64; the first step of real data, so this is the one piece of cleaning in
+the port), correct_dyn (dynspec.py:3325-3410 -> sb_svd_topk + sb_svd_apply, or the
 sb_bandpass_* passes), scale_dyn('lambda') (dynspec.py:3926-3957 -> sb_scale_dyn_lambda_f32),
 thetatheta_chunks / calc_wavefield / gerchberg_saxton (:1765-1896), and, through
 ``arcfit.ArcFitMixin``, norm_sspec / fit_arc (:1920-2183, :970-1346).
@@ -58,6 +60,143 @@ def get_window(nt, nf, window="hanning", frac=0.1):
 def is_valid(array):
     """scint_utils.py:87-91."""
     return np.isfinite(array) * (~np.isnan(array))
+
+
+# ----------------------------------------------------------------------
+# gap filling (csrc/inpaint.cu)
+# ----------------------------------------------------------------------
+_FILL_MAX_NF, _FILL_MAX_NT = 32768, 16384
+_MEDFILT_MAX_SIDE = 31
+
+
+def _fill_check(image, mask):
+    """ValueError, before any device work, for what the gap fills do not take."""
+    if image.ndim != 2 or mask.shape != image.shape:
+        raise ValueError("need a 2-D image and a mask of its shape")
+    nf, nt = image.shape
+    if not (1 <= nf <= _FILL_MAX_NF and 1 <= nt <= _FILL_MAX_NT):
+        raise ValueError("shape %s is outside 1..%d x 1..%d" % (image.shape, _FILL_MAX_NF,
+                                                                  _FILL_MAX_NT))
+    if np.any(np.isinf(image)):
+        raise ValueError("the image has an infinite pixel")
+    if np.all(mask):
+        raise ValueError("every pixel is masked: nothing to fill from")
+
+
+def _axis_classes(n):
+    """Class of every index along an axis of length n: the (extent, centre offset) of the
+    5-point window [i-2, i+2] clipped to [0, n).  Returns (cls uint8 [n], [(extent, offset)])."""
+    i = np.arange(n)
+    lo = np.maximum(i - 2, 0)
+    key = np.minimum(i + 3, n) - lo, i - lo
+    kinds = sorted(set(zip(*(k.tolist() for k in key))))
+    index = {k: c for c, k in enumerate(kinds)}
+    return np.array([index[k] for k in zip(*(k.tolist() for k in key))], np.uint8), kinds
+
+
+def _stencil_tables(nf, nt):
+    """Stencils of the biharmonic system, S = laplace(laplace(e_p)) on the clipped 5x5 box
+    (scipy.ndimage, mode 'reflect'), one per pair of row and column classes, centred on the
+    pixel: tables float64 [nrc][ncc][5][5], zero outside the box."""
+    from scipy.ndimage import laplace
+    rcls, rk = _axis_classes(nf)
+    ccls, ck = _axis_classes(nt)
+    tables = np.zeros((len(rk), len(ck), 5, 5))
+    for a, (er, orow) in enumerate(rk):
+        for c, (ec, ocol) in enumerate(ck):
+            box = np.zeros((er, ec))
+            box[orow, ocol] = 1.0
+            tables[a, c, 2 - orow:2 - orow + er, 2 - ocol:2 - ocol + ec] = laplace(laplace(box))
+    return rcls, ccls, tables
+
+
+def _biharmonic_values(image, mask, tol, maxit):
+    """Inpainted values at the masked pixels, in row-major order, and the solver info."""
+    import torch
+    nf, nt = image.shape
+    pix = np.flatnonzero(mask).astype(np.int32)
+    known = image[~mask]
+    rcls, ccls, tables = _stencil_tables(nf, nt)
+    d_img = D.upload(np.ascontiguousarray(image, dtype=np.float64))
+    d_pix, d_tab = D.upload(pix), D.upload(tables)
+    d_rc, d_cc = D.upload(rcls), D.upload(ccls)
+    out = D.empty((pix.size,), torch.float64)
+    info = np.zeros(3, np.int32)
+    resid = np.zeros(1)
+    _lib.check(_lib.lib.sb_inpaint_biharmonic_f64(
+        d_img.data_ptr(), nf, nt, d_pix.data_ptr(), pix.size, d_tab.data_ptr(),
+        d_rc.data_ptr(), tables.shape[0], d_cc.data_ptr(), tables.shape[1],
+        float(known.min()), float(known.max()), float(tol), int(maxit), out.data_ptr(),
+        info.ctypes.data, resid.ctypes.data, D.stream_ptr()))
+    info = {"iterations": int(info[0]), "residual": float(resid[0]),
+            "converged": bool(info[1]), "restarts": int(info[2])}
+    if not info["converged"]:
+        import warnings
+        warnings.warn("biharmonic inpainting stopped after %d iterations at relative residual "
+                      "%.3g (tol %.3g)" % (info["iterations"], info["residual"], tol),
+                      RuntimeWarning, stacklevel=3)
+    return D.download(out), info
+
+
+def inpaint_biharmonic(image, mask, return_info=False, tol=1e-10, maxit=50000):
+    """Biharmonic inpainting of the pixels where mask is non-zero: skimage >= 0.19's
+    ``restoration.inpaint_biharmonic(image, mask, split_into_regions=False)`` for a 2-D
+    image, solved on the device.
+
+    One unknown per masked pixel; its equation is the stencil laplace(laplace(e_p))
+    (scipy.ndimage, mode 'reflect') on the 5x5 box around it clipped to the image, with the
+    known pixels moved to the right-hand side.  The system is solved matrix-free by
+    BiCGSTAB with Jacobi scaling in float64 until ||b - A x|| <= tol ||b||, or for at most
+    ``maxit`` steps; the result is clipped to [min, max] of the known pixels.  Returns a
+    float64 copy of the image with the masked pixels filled, and with return_info=True also
+    a dict: iterations, residual (the final ||b - A x|| / ||b||), converged, restarts.  A
+    solve that stops at the cap warns (RuntimeWarning) and still returns its result.
+
+    ValueError, before any device work: an image that is not 2-D, a mask of another shape,
+    a shape outside 1..32768 x 1..16384, an infinite pixel (the deviation from skimage:
+    there the result depends on SuperLU's elimination order), a NaN pixel that is not
+    masked, or a mask that covers every pixel.  No masked pixel: the copy, 0 iterations."""
+    image = np.array(image, dtype=np.float64)
+    mask = np.asarray(mask).astype(bool)
+    _fill_check(image, mask)
+    if np.any(np.isnan(image[~mask])):
+        raise ValueError("the image has a NaN pixel outside the mask")
+    info = {"iterations": 0, "residual": 0.0, "converged": True, "restarts": 0}
+    if np.any(mask):
+        vals, info = _biharmonic_values(image, mask, tol, maxit)
+        image[mask] = vals
+    return (image, info) if return_info else image
+
+
+def _median_values(image, mask, kernel_size, nan_value):
+    """scipy.signal.medfilt(image with NaN read as nan_value, kernel_size) at the masked
+    pixels, in row-major order."""
+    import torch
+    nf, nt = image.shape
+    pix = np.flatnonzero(mask).astype(np.int32)
+    kh, kw = kernel_size
+    d_img = D.upload(np.ascontiguousarray(image, dtype=np.float64))
+    d_pix = D.upload(pix)
+    out = D.empty((pix.size,), torch.float64)
+    _lib.check(_lib.lib.sb_medfilt_masked_f64(d_img.data_ptr(), nf, nt, d_pix.data_ptr(),
+                                              pix.size, kh, kw, float(nan_value),
+                                              out.data_ptr(), D.stream_ptr()))
+    return D.download(out)
+
+
+def _medfilt_size(kernel_size):
+    """medfilt's kernel_size for a 2-D array: a scalar or one size per axis, each odd."""
+    ks = np.asarray(kernel_size)
+    if ks.shape == ():
+        ks = np.repeat(ks, 2)
+    if ks.shape != (2,) or not np.issubdtype(ks.dtype, np.integer):
+        raise ValueError("kernel_size must be an integer or two integers")
+    for k in ks:
+        if k % 2 != 1:
+            raise ValueError("Each element of kernel_size should be odd.")
+        if not 1 <= k <= _MEDFILT_MAX_SIDE:
+            raise ValueError("kernel sizes above %d are not supported" % _MEDFILT_MAX_SIDE)
+    return int(ks[0]), int(ks[1])
 
 
 class BasicDyn:
@@ -126,6 +265,67 @@ class Dynspec(ArcFitMixin):
             self.calc_sspec(lamsteps=lamsteps)
         if verbose:
             print("LOADED DYNSPEC OBJECT {0}".format(self.name))
+
+    # ------------------------------------------------------------------
+    # gap filling (csrc/inpaint.cu)
+    # ------------------------------------------------------------------
+    def refill(self, method='biharmonic', zeros=True, kernel_size=5, linear=True, tol=1e-10,
+               maxit=50000):
+        """Replace the NaN pixels of self.dyn, and its zeros if ``zeros`` (reference
+        dynspec.py:3273-3323), in place, in the reference's order:
+
+        1. zeros: self.dyn[self.dyn == 0] = NaN;
+        2. 'biharmonic': inpaint_biharmonic of the NaN pixels (skimage's system, solved
+           on the device, see ``inpaint_biharmonic``), written into those pixels;
+           'median': scipy.signal.medfilt(kernel_size) of a copy whose NaN pixels hold the
+           mean of the valid ones (zero padding at the edges), computed on the device at
+           the NaN pixels only and written there; 'linear' / 'cubic' / 'nearest' with
+           linear=True: NotImplementedError (the reference's griddata triangulates the
+           valid pixels, and on a pixel lattice qhull's choice among co-circular points
+           cannot be matched); with linear=False, or any other name (e.g. 'mean'), nothing;
+        3. the NaN pixels left get np.mean of the valid ones.
+
+        The means are the reference's numpy expressions on the host.  For 'biharmonic' and
+        'median', ValueError before anything is changed when self.dyn has an infinite pixel
+        (a deliberate deviation: the reference's biharmonic result there depends on
+        SuperLU's elimination order), every pixel would be masked, or the shape is outside
+        1..32768 x 1..16384; 'median' also rejects an even size (as medfilt does) and sizes
+        above 31.  A biharmonic solve that does not converge warns (RuntimeWarning) and
+        its result is still stored.
+
+        tol and maxit (not in the reference) are the biharmonic solver's stopping rule,
+        ||b - A x|| <= tol ||b||, and its step cap.  The error the rule leaves grows with
+        the size of the largest hole (about L^4 for a hole L pixels wide): at the default
+        1e-10, holes up to 32 x 32 come within 1e-7 of the known range of the direct
+        solution, but a 64 x 256 block only within about 1e-4; tol=1e-13 brings that to
+        about 5e-8 for twice the steps."""
+        if method in ('linear', 'cubic', 'nearest') and linear:
+            raise NotImplementedError(
+                "griddata interpolation is not on the GPU path: its triangulation of a pixel "
+                "lattice is not reproducible; use method='biharmonic' or 'median'")
+        if method in ('biharmonic', 'median'):
+            dyn = np.asarray(self.dyn)
+            masked = np.isnan(dyn)
+            if zeros:
+                masked |= dyn == 0
+            _fill_check(dyn, masked)
+            if method == 'median':
+                size = _medfilt_size(kernel_size)
+        if zeros:
+            self.dyn[self.dyn == 0] = np.nan
+        if method == 'biharmonic':
+            nan = np.isnan(self.dyn)
+            if np.any(nan):
+                self.dyn[nan] = _biharmonic_values(self.dyn, nan, tol, maxit)[0]
+        elif method == 'median':
+            if kernel_size == 5:
+                print("Warning: kernel size is set to default.")
+            nan = np.isnan(self.dyn)
+            if np.any(nan):
+                meanval = np.mean(self.dyn[is_valid(self.dyn)])
+                self.dyn[nan] = _median_values(self.dyn, nan, size, meanval)
+        meanval = np.mean(self.dyn[is_valid(self.dyn)])
+        self.dyn[np.isnan(self.dyn)] = meanval
 
     # ------------------------------------------------------------------
     # flux-variation correction (csrc/svd.cu)
