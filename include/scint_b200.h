@@ -510,6 +510,46 @@ int sb_inpaint_biharmonic_f64(const double* img, int32_t nf, int32_t nt, const i
 int sb_medfilt_masked_f64(const double* img, int32_t nf, int32_t nt, const int32_t* pix, int32_t n,
                           int32_t kh, int32_t kw, double nan_value, double* out, void* stream);
 
+/* ---- Dynspec.get_scint_params ------------------------------------------- */
+
+/* One least-squares fit of the ACF (host struct; the pointers are device memory).
+ * Parameter slots 0..4: tau, dnu, amp, alpha, phasegrad; p0 holds every slot's starting
+ * (or fixed) value, bit s of `vary` frees slot s, bit s of `bounded` fits it with min 0,
+ * max inf in lmfit's internal variable.  acf: float64 ACF with row pitch `pitch`.
+ *   1-D (sb_scint_fit_1d): time cut acf[r0][c0 .. c0 + n0), lags s0 * i (s0 = dt);
+ *       frequency cut acf[r1 .. r1 + n1)[c1], lags s1 * i (s1 = df); aux [n0 + n1] the
+ *       weights of both cuts (the weight of lag 0 of each is taken as 0).
+ *   2-D (sb_scint_fit_2d): the box acf[r0 .. r0 + n0)[c0 .. c0 + n1) (frequency lag by
+ *       time lag); s0 = tobs, s1 = bw, c = nsub nchan; aux [2 n1 + 2 n0]: tdata [n1],
+ *       fdata [n0], T / max(tticks) [n1], F / max(fticks) [n0]; shf, sht, pf, pt, zf, zt
+ *       place the weights (see csrc/scintfit.cu); weighted 0 or 1.
+ * max_nfev caps the evaluations. */
+typedef struct sb_scint_fit {
+    const double* acf;
+    const double* aux;
+    int64_t pitch;
+    double s0, s1, c;
+    double p0[5];
+    int32_t r0, c0, r1, c1, n0, n1;
+    int32_t shf, sht, pf, pt, zf, zt;
+    int32_t vary, bounded, weighted, max_nfev;
+} sb_scint_fit;
+
+/* Dynspec.get_scint_params (dynspec.py:2470-3156), the lmfit least-squares fits of
+ * method='acf1d' (scint_acf_model, scint_models.py:62-120; replaces the fitter() call at
+ * dynspec.py:2698-2702) and method='acf2d_approx' (scint_acf_model_2d_approx,
+ * scint_models.py:123-161; replaces dynspec.py:2836-2841), batched over nfit fits with an
+ * analytic float64 Jacobian.  fits: host [nfit].  out: device float64 [nfit][11]: the five
+ * slots' values, their standard errors (NaN where not estimated: fixed, singular J^T J, or
+ * not converged) and chi-square; info: device int32 [nfit][2]: evaluations and status (1
+ * converged, 2 stopped with no decrease left at float64 precision, -1 hit max_nfev, -2 a
+ * non-finite residual).  Synchronous (the host reads the state every 32 iterations).  A
+ * fit's result is bit-identical alone or in any batch. */
+int sb_scint_fit_1d(const sb_scint_fit* fits, int32_t nfit, double* out, int32_t* info,
+                    void* stream);
+int sb_scint_fit_2d(const sb_scint_fit* fits, int32_t nfit, double* out, int32_t* info,
+                    void* stream);
+
 /* ---- scint_sim.Simulation ------------------------------------------------ */
 
 typedef struct sb_sim_params {

@@ -49,6 +49,16 @@ class SimParams(ctypes.Structure):
                 ("inner", c_dbl), ("consp", c_dbl)]
 
 
+class ScintFit(ctypes.Structure):
+    """struct sb_scint_fit"""
+    _fields_ = [("acf", vp), ("aux", vp), ("pitch", c_i64), ("s0", c_dbl), ("s1", c_dbl),
+                ("c", c_dbl), ("p0", c_dbl * 5),
+                ("r0", c_int), ("c0", c_int), ("r1", c_int), ("c1", c_int), ("n0", c_int),
+                ("n1", c_int), ("shf", c_int), ("sht", c_int), ("pf", c_int), ("pt", c_int),
+                ("zf", c_int), ("zt", c_int), ("vary", c_int), ("bounded", c_int),
+                ("weighted", c_int), ("max_nfev", c_int)]
+
+
 _SIGS = {
     "sb_abi_version": (c_int, []),
     "sb_last_error": (ctypes.c_char_p, []),
@@ -102,6 +112,8 @@ _SIGS = {
     "sb_inpaint_biharmonic_f64": (c_int, [vp, c_int, c_int, vp, c_int, vp, vp, c_int, vp, c_int,
                                           c_dbl, c_dbl, c_dbl, c_int, vp, vp, vp, vp]),
     "sb_medfilt_masked_f64": (c_int, [vp, c_int, c_int, vp, c_int, c_int, c_int, c_dbl, vp, vp]),
+    "sb_scint_fit_1d": (c_int, [ctypes.POINTER(ScintFit), c_int, vp, vp, vp]),
+    "sb_scint_fit_2d": (c_int, [ctypes.POINTER(ScintFit), c_int, vp, vp, vp]),
     "sb_sim_weights": (c_int, [ctypes.POINTER(SimParams), vp, vp]),
     "sb_sim_screen": (c_int, [c_int, c_int, vp, vp, vp, ctypes.c_uint64, vp, vp]),
     "sb_sim_intensity": (c_int, [c_int, c_int, c_int, vp, vp, c_dbl, c_dbl, vp,

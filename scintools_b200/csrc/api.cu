@@ -193,6 +193,8 @@ int inpaint_biharmonic(const double* img, int nf, int nt, const int* pix, int n,
                        cudaStream_t st);
 int medfilt_masked(const double* img, int nf, int nt, const int* pix, int n, int kh, int kw,
                    double nan_value, double* out, cudaStream_t st);
+int scint_fit_1d(const sb_scint_fit* fits, int nfit, double* out, int* info, cudaStream_t st);
+int scint_fit_2d(const sb_scint_fit* fits, int nfit, double* out, int* info, cudaStream_t st);
 
 int gerchberg_saxton(float2* W, const float* amp, const unsigned char* rowmask, int n0, int n1,
                      int niter, cudaStream_t st);
@@ -598,6 +600,16 @@ int sb_inpaint_biharmonic_f64(const double* img, int32_t nf, int32_t nt, const i
 int sb_medfilt_masked_f64(const double* img, int32_t nf, int32_t nt, const int32_t* pix, int32_t n,
                           int32_t kh, int32_t kw, double nan_value, double* out, void* stream) {
     return sb::medfilt_masked(img, nf, nt, pix, n, kh, kw, nan_value, out, (cudaStream_t)stream);
+}
+
+int sb_scint_fit_1d(const sb_scint_fit* fits, int32_t nfit, double* out, int32_t* info,
+                    void* stream) {
+    return sb::scint_fit_1d(fits, nfit, out, info, (cudaStream_t)stream);
+}
+
+int sb_scint_fit_2d(const sb_scint_fit* fits, int32_t nfit, double* out, int32_t* info,
+                    void* stream) {
+    return sb::scint_fit_2d(fits, nfit, out, info, (cudaStream_t)stream);
 }
 
 int sb_convert_f64_f32(const double* src, float* dst, int64_t n, void* stream) {

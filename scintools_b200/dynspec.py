@@ -9,12 +9,13 @@ the reference for the arc-measurement hot path:
   thetatheta_single  dynspec.py:1539-1655  -> sb_cs_f32 + sb_eta_sweep
   fit_thetatheta     dynspec.py:1657-1763  -> per chunk ththmod.single_search
 
-Everything outside that path (file I/O, cleaning other than refill, plotting, arc fitting,
-lmfit models) is deliberately not here: use the reference for those and hand
-the arrays over with ``BasicDyn`` exactly as the reference's tutorials do.
+Everything outside that path (file I/O, cleaning other than refill, plotting, the lmfit
+models other than get_scint_params's) is deliberately not here: use the reference for
+those and hand the arrays over with ``BasicDyn`` exactly as the reference's tutorials do.
 Units: times in s, freqs in MHz, eta in s^3, edges in mHz, tau in us.
 
-Also here: refill (dynspec.py:3273-3323 -> sb_inpaint_biharmonic_f64 or
+Also here: get_scint_params / get_acf_tilt (dynspec.py:2283-3156 -> sb_scint_fit_1d /
+sb_scint_fit_2d, batched over spectra by get_scint_params_batch), refill (dynspec.py:3273-3323 -> sb_inpaint_biharmonic_f64 or
 sb_medfilt_masked_f64; the first step of real data, so this is the one piece of cleaning in
 the port), correct_dyn (dynspec.py:3325-3410 -> sb_svd_topk + sb_svd_apply, or the
 sb_bandpass_* passes), scale_dyn('lambda') (dynspec.py:3926-3957 -> sb_scale_dyn_lambda_f32),
@@ -197,6 +198,544 @@ def _medfilt_size(kernel_size):
         if not 1 <= k <= _MEDFILT_MAX_SIDE:
             raise ValueError("kernel sizes above %d are not supported" % _MEDFILT_MAX_SIDE)
     return int(ks[0]), int(ks[1])
+
+
+# ----------------------------------------------------------------------
+# scintillation scales (csrc/scintfit.cu)
+# ----------------------------------------------------------------------
+_ACF_MIN_NF, _ACF_MAX_NF, _ACF_MIN_NT, _ACF_MAX_NT = 2, 32768, 5, 16384
+_SLOTS = ("tau", "dnu", "amp", "alpha", "phasegrad")
+_FIT_STATUS = {1: "converged", 2: "converged (no decrease left at float64 precision)",
+               -1: "stopped at max_nfev", -2: "non-finite residual"}
+
+
+class FitParam:
+    """One fitted parameter: value, and stderr (None where not estimated)."""
+
+    def __init__(self, name, value, stderr=None, vary=True):
+        self.name, self.value, self.stderr, self.vary = name, value, stderr, vary
+
+    def __repr__(self):
+        return "<FitParam %s = %r +/- %r>" % (self.name, self.value, self.stderr)
+
+
+class ScintFitResult:
+    """What get_scint_params returns: the fields callers of the reference read from
+    lmfit's MinimizerResult.  params[name].value / .stderr, chisqr, redchi = chisqr /
+    (ndata - nvarys), ndata (every residual, zero-weight ones included, as lmfit counts),
+    nvarys, nfev (model evaluations; each also gives the analytic Jacobian), success (False
+    when the fit stopped at max_nfev), message, init_values (the starting values of the
+    varying parameters)."""
+
+    def __init__(self, params, chisqr, ndata, nvarys, nfev, status, method, init_values):
+        self.params = params
+        self.init_values = init_values
+        self.chisqr = chisqr
+        self.ndata = ndata
+        self.nvarys = nvarys
+        self.redchi = chisqr / max(1, ndata - nvarys)
+        self.nfev = nfev
+        self.status = status
+        self.success = status > 0
+        self.message = _FIT_STATUS.get(status, "status %d" % status)
+        self.method = method
+
+    def report(self):
+        """Plain-text summary (not lmfit's fit_report layout)."""
+        lines = ["[[Fit: %s, Levenberg-Marquardt on the device]]" % self.method,
+                 "    %s after %d evaluations" % (self.message, self.nfev),
+                 "    data points = %d, variables = %d" % (self.ndata, self.nvarys),
+                 "    chi-square = %.10g, reduced chi-square = %.10g" % (self.chisqr, self.redchi),
+                 "[[Variables]]"]
+        for p in self.params.values():
+            if not p.vary:
+                lines.append("    %-10s %.10g (fixed)" % (p.name + ":", p.value))
+            elif p.stderr is None:
+                lines.append("    %-10s %.10g +/- (not estimated)" % (p.name + ":", p.value))
+            else:
+                lines.append("    %-10s %.10g +/- %.4g" % (p.name + ":", p.value, p.stderr))
+        return "\n".join(lines)
+
+
+def _scint_args_check(method, plot, mcmc, nan_policy):
+    if plot:
+        raise NotImplementedError("plotting is outside the GPU path")
+    if mcmc:
+        raise NotImplementedError("mcmc sampling is outside the GPU path")
+    if method == 'acf2d':
+        raise NotImplementedError("method='acf2d' needs scint_sim.ACF, which is not ported")
+    if method == 'sspec':
+        raise NotImplementedError("method='sspec' does not work in the reference either")
+    if method not in ('nofit', 'acf1d', 'acf2d_approx'):
+        raise ValueError("method must be 'nofit', 'acf1d' or 'acf2d_approx'")
+    if nan_policy != 'raise':
+        raise NotImplementedError("only nan_policy='raise' is supported")
+
+
+def _scint_shape_check(ds):
+    nf, nt = np.shape(ds.dyn)
+    if not (_ACF_MIN_NF <= nf <= _ACF_MAX_NF and _ACF_MIN_NT <= nt <= _ACF_MAX_NT):
+        raise ValueError("dynspec %d x %d is outside the supported sizes (nf %d..%d, nt %d..%d)"
+                         % (nf, nt, _ACF_MIN_NF, _ACF_MAX_NF, _ACF_MIN_NT, _ACF_MAX_NT))
+    if hasattr(ds, 'acf') and np.shape(ds.acf) != (2 * nf, 2 * nt):
+        raise ValueError("self.acf has shape %s, not 2 x %s" % (np.shape(ds.acf), (nf, nt)))
+
+
+def _acf_stacks(dynspecs):
+    """One float64 device stack [n][2 nf][2 nt] per (nf, nt) group: the ACF a Dynspec holds
+    is uploaded into its slice; a missing one is made by the ACF driver into a float32
+    slice, widened on the device and stored as self.acf, as calc_acf would.  Returns
+    {id(ds): (stack, slice index)}."""
+    import torch
+    groups = {}
+    for ds in dynspecs:
+        groups.setdefault(np.shape(ds.dyn), []).append(ds)
+    where = {}
+    for (nf, nt), members in groups.items():
+        stack = D.empty((len(members), 2 * nf, 2 * nt), torch.float64)
+        tmp = None
+        for k, ds in enumerate(members):
+            if hasattr(ds, 'acf'):
+                stack[k].copy_(torch.from_numpy(np.ascontiguousarray(ds.acf, dtype=np.float64)))
+            else:
+                if tmp is None:
+                    tmp = D.empty((2 * nf, 2 * nt), torch.float32)
+                d = D.upload_f32(np.asarray(ds.dyn))
+                _lib.check(_lib.lib.sb_acf_f32(d.data_ptr(), nf, nt, 1, 1, tmp.data_ptr(),
+                                               D.stream_ptr()))
+                _lib.check(_lib.lib.sb_convert_f32_f64(tmp.data_ptr(), stack[k].data_ptr(),
+                                                       tmp.numel(), D.stream_ptr()))
+                ds.acf = D.download(stack[k])
+            where[id(ds)] = (stack, k)
+    return where
+
+
+def _contiguous_prefix(inds, n):
+    """(count) of a crop index vector that must be 0, 1, ..., count - 1."""
+    inds = np.atleast_1d(inds)
+    if inds.size == 0 or not np.array_equal(inds, np.arange(inds.size)) or inds.size > n:
+        raise ValueError("the ACF cut crop is not a prefix of the lags (negative dt or df?)")
+    return inds.size
+
+
+def _scint_nofit(ds, full_frame, nscale, bartlett, weighted):
+    """The reference's host steps up to the first fit (dynspec.py:2575-2687), on ds.acf:
+    initial guesses, crops, the nofit attributes and the 1-D weights.  Returns the 1-D plan."""
+    acf = ds.acf
+    nf, nt = np.shape(acf)
+    ydata_f = acf[int(nf/2):, int(nt/2)]
+    xdata_f = ds.df * np.linspace(0, len(ydata_f)-1, len(ydata_f))
+    ydata_t = acf[int(nf/2), int(nt/2):]
+    xdata_t = ds.dt * np.linspace(0, len(ydata_t)-1, len(ydata_t))
+
+    wn = min([ydata_f[0]-ydata_f[1], ydata_t[0]-ydata_t[1]])
+    amp = max([ydata_f[0] - wn, ydata_t[0] - wn])
+    if np.argwhere(ydata_t < amp/np.e).squeeze().size == 0:
+        tau = ds.dt if ydata_t[1] < 0 else ds.tobs
+    else:
+        tau = xdata_t[np.argwhere(ydata_t < amp/np.e).squeeze()[0]]
+    if np.argwhere(ydata_f < amp/2).squeeze().size == 0:
+        dnu = ds.df if ydata_f[1] < 0 else ds.bw
+    else:
+        dnu = xdata_f[np.argwhere(ydata_f < amp/2).squeeze()[0]]
+
+    if not full_frame:
+        t_inds = np.argwhere(xdata_t <= nscale*tau).squeeze()
+        f_inds = np.argwhere(xdata_f <= nscale*dnu).squeeze()
+        if nscale*tau <= 5*ds.dt:
+            t_inds = np.argwhere(xdata_t <= 5*ds.dt).squeeze()
+        if nscale*dnu <= 5*ds.df:
+            f_inds = np.argwhere(xdata_f <= 5*ds.df).squeeze()
+        nt_c = _contiguous_prefix(t_inds, len(xdata_t))
+        nf_c = _contiguous_prefix(f_inds, len(xdata_f))
+        xdata_t = xdata_t[t_inds]
+        ydata_t = ydata_t[t_inds]
+        xdata_f = xdata_f[f_inds]
+        ydata_f = ydata_f[f_inds]
+    else:
+        nt_c, nf_c = len(xdata_t), len(xdata_f)
+
+    ds.tau = tau
+    ds.dnu = dnu
+    ds.amp = amp
+    ds.wn = wn
+
+    tau_half = xdata_t[np.argmin(abs(ydata_t - amp/2))]
+    if tau_half < ds.dt:
+        tau_half = ds.dt
+    elif tau_half > ds.tobs:
+        tau_half = ds.tobs
+    nscint = (1 + 0.2*ds.bw/(ds.dnu)) * (1 + 0.2*ds.tobs/(tau_half))
+    ds.dnuerr = dnu / np.sqrt(nscint)
+    ds.tauerr = tau / np.sqrt(nscint)
+    ds.amperr = amp / np.sqrt(nscint)
+    ds.wnerr = wn / np.sqrt(nscint)
+    ds.tscat = 1/(2*np.pi*ds.dnu)
+    ds.nscint = nscint
+    ds.scint_param_method = 'nofit'
+
+    valid = ds.dyn[is_valid(ds.dyn) * (ds.dyn != 0)]
+    mean = np.mean(valid)
+    flux_var_est = mean**2
+    flux_var = np.var(valid)
+    ds.dnu_est = ds.df * (flux_var/flux_var_est - 1)
+    if ds.dnu_est < 0:
+        ds.dnu_est = 0
+    ds.dnu_esterr = ds.dnu_est / np.sqrt(nscint)
+    if ds.dnu_est > 0:
+        ds.tscat_est = 1/(2*np.pi*ds.dnu_est)
+    else:
+        ds.tscat_est = 0
+    ds.modulation_index = np.sqrt(flux_var)/mean
+
+    t_errors = np.ones(np.shape(xdata_t))/np.sqrt((nt/2))
+    t_errors[0] = 1e-3
+    f_errors = np.ones(np.shape(xdata_f))/np.sqrt((nf/2))
+    f_errors[0] = 1e-3
+    if bartlett:
+        var_t = np.ones(np.shape(ydata_t)) / (nt / 2)
+        var_t[0] = 1e-10
+        var_t[2:] *= 1 + 2 * np.cumsum(ydata_t[1:-1] ** 2)
+        t_errors = np.sqrt(var_t)
+        var_f = np.ones(np.shape(ydata_f)) / (nf / 2)
+        var_f[0] = 1e-10
+        var_f[2:] *= 1 + 2 * np.cumsum(ydata_f[1:-1] ** 2)
+        f_errors = np.sqrt(var_f)
+    weights_t = 1/t_errors if weighted else np.ones(np.shape(ydata_t))
+    weights_f = 1/f_errors if weighted else np.ones(np.shape(ydata_f))
+    return dict(tau=tau, dnu=dnu, amp=amp, nt_c=nt_c, nf_c=nf_c, xdata_t=xdata_t,
+                xdata_f=xdata_f, ydata_t=ydata_t, ydata_f=ydata_f, weights_t=weights_t,
+                weights_f=weights_f)
+
+
+def _fftshift_positions(n):
+    """Along one axis of length n, where the reference's weight shifts put things
+    (dynspec.py:2785-2789 and scint_models.py:156-158): the roll sh of the weights
+    (fftshift twice maps the weight of index (k + sh) mod n to index k), the index that
+    gets 1e10, and the index the model zeroes."""
+    ar = np.arange(n)
+    perm = np.fft.fftshift(np.fft.fftshift(ar))
+    sh = int(perm[0])
+    assert np.array_equal(perm, (ar + sh) % n)
+    m = np.zeros(n)
+    m[0] = 1
+    p = int(np.argmax(np.fft.fftshift(m)))
+    m = np.zeros(n)
+    m[-1] = 1
+    z = int(np.argmax(np.fft.ifftshift(m)))
+    return sh, p, z
+
+
+def _scint_crop_2d(ds, tau, dnu, nscale, full_frame, verbose):
+    """The 2-D crop of dynspec.py:2716-2783, as index vectors into ds.acf: returns (rows,
+    cols, tticks, fticks), rows / cols contiguous."""
+    nf, nt = np.shape(ds.acf)
+    tticks = np.linspace(-ds.tobs, ds.tobs, nt + 1)[:-1]
+    fticks = np.linspace(-ds.bw, ds.bw, nf + 1)[:-1]
+    wn_loc = np.unravel_index(np.argmax(ds.acf, axis=None), ds.acf.shape)
+    fleft = wn_loc[0]
+    fright = nf - wn_loc[0] - 1
+    fmin = wn_loc[0] - min(fleft, fright)
+    fmax = wn_loc[0] + min(fleft, fright) + 1
+    tleft = wn_loc[1]
+    tright = nt - wn_loc[1] - 1
+    tmin = wn_loc[1] - min(tleft, tright)
+    tmax = wn_loc[1] + min(tleft, tright) + 1
+    rows = np.arange(nf)[fmin:fmax]
+    cols = np.arange(nt)[tmin:tmax]
+    if nscale is not None and not full_frame:
+        ntau = nscale
+        ndnu = nscale
+        if ntau > (ds.tobs / tau):
+            if verbose:
+                print('WARNING: nscale exceeds range in time lag')
+            tmin = 0
+            tmax = nt
+        else:
+            tframe = int(round(ntau * (tau / ds.dt)))
+            tmin = int(np.floor(len(cols) / 2)) - tframe
+            tmax = int(np.floor(len(cols) / 2)) + tframe + 1
+        if ndnu > (ds.bw / dnu):
+            if verbose:
+                print('WARNING: nscale exceeds range in frequency lag')
+            # the reference sets the time bounds here (dynspec.py:2766-2767)
+            tmin = 0
+            tmax = nf
+        else:
+            fframe = int(round(ndnu * (dnu / ds.df)))
+            fmin = int(np.floor(len(rows) / 2)) - fframe
+            fmax = int(np.floor(len(rows) / 2)) + fframe + 1
+        rows = rows[fmin:fmax]
+        cols = cols[tmin:tmax]
+    if rows.size == 0 or cols.size == 0:
+        raise ValueError("the 2-D ACF crop is empty")
+    return rows, cols, tticks, fticks
+
+
+def _acf2d_model(p, tdata, fdata, tobs, bw):
+    """scint_acf_model_2d_approx's model (scint_models.py:123-161) at the parameters p
+    (dict), as [nf][nt], before the weights."""
+    amp, dnu, tau, alpha = p['amp'], p['dnu'], p['tau'], p['alpha']
+    mu = p['phasegrad']*60
+    t = np.reshape(tdata, (len(tdata), 1))
+    f = np.reshape(fdata, (1, len(fdata)))
+    model = amp * np.exp(-(abs((t - mu*f)/tau)**(3 * alpha / 2) +
+                         abs(f / (dnu / np.log(2)))**(3 / 2))**(2 / 3))
+    model = np.multiply(model, 1-np.divide(abs(t), tobs))
+    model = np.multiply(model, 1-np.divide(abs(f), bw))
+    return np.transpose(model)
+
+
+def _run_fits(kind, descs):
+    """One batched fit (sb_scint_fit_1d / _2d, synchronous) of the ScintFit descriptors;
+    returns (out [n][11], info [n][2]) on the host."""
+    import torch
+    n = len(descs)
+    arr = (_lib.ScintFit * n)(*descs)
+    out = D.empty((n, 11), torch.float64)
+    info = D.empty((n, 2), torch.int32)
+    fn = _lib.lib.sb_scint_fit_1d if kind == 1 else _lib.lib.sb_scint_fit_2d
+    _lib.check(fn(arr, n, out.data_ptr(), info.data_ptr(), D.stream_ptr()))
+    return D.download(out), D.download(info)
+
+
+def _result(out, info, desc, names, fixed, ndata, method):
+    vary = desc.vary
+    params = {}
+    for s, name in enumerate(_SLOTS):
+        if name not in names:
+            continue
+        v = bool((vary >> s) & 1)
+        err = float(out[5 + s]) if v and np.isfinite(out[5 + s]) else None
+        params[name] = FitParam(name, float(out[s]), err, v)
+    for name, value in fixed.items():
+        params[name] = FitParam(name, value, None, False)
+    init = {n: float(desc.p0[s]) for s, n in enumerate(_SLOTS) if (vary >> s) & 1}
+    return ScintFitResult(params, float(out[10]), int(ndata), bin(vary).count("1"),
+                          int(info[0]), int(info[1]), method, init)
+
+
+def _check_status(res, what):
+    if res.status == -2:
+        raise ValueError("%s: the fit met a non-finite residual (NaN values detected in the "
+                         "output of the model function)" % what)
+
+
+def get_scint_params_batch(dynspecs, method='acf1d', **kwargs):
+    """Dynspec.get_scint_params on each Dynspec of the list, with the fits of all of them
+    batched on the device: sets on each exactly what get_scint_params(**kwargs) would set on
+    it alone and returns the list of results (None for method='nofit').  The objects are
+    grouped by the shape of their dynamic spectrum; each group's ACFs form one device stack,
+    and each group's fits run as one batch.  Keyword arguments as get_scint_params."""
+    import torch
+    a = dict(plot=False, alpha=5/3, mcmc=False, full_frame=False, nscale=5, verbose=False,
+             nan_policy='raise', weighted=True, tau_vary_2d=True, tau_input=None,
+             bartlett=True, get_fit_report=True)
+    ignored = ('nwalkers', 'steps', 'burn', 'nitr', 'lnsigma', 'progress', 'display',
+               'filename', 'dpi', 'workers')
+    for k in kwargs:
+        if k not in a and k not in ignored:
+            raise TypeError("get_scint_params() got an unexpected keyword argument '%s'" % k)
+    a.update({k: v for k, v in kwargs.items() if k in a})
+    _scint_args_check(method, a['plot'], a['mcmc'], a['nan_policy'])
+    dynspecs = list(dynspecs)
+    for ds in dynspecs:
+        _scint_shape_check(ds)
+    alpha, verbose, weighted = a['alpha'], a['verbose'], a['weighted']
+    if method == 'nofit':
+        for ds in dynspecs:
+            if not hasattr(ds, 'acf'):
+                ds.calc_acf()
+            _scint_nofit(ds, a['full_frame'], a['nscale'], a['bartlett'], weighted)
+        return [None] * len(dynspecs)
+    # the host steps, and every check they make, come before the device work on an ACF the
+    # object already holds; a missing ACF is made first
+    where = _acf_stacks([ds for ds in dynspecs if not hasattr(ds, 'acf')])
+    plans = [_scint_nofit(ds, a['full_frame'], a['nscale'], a['bartlett'], weighted)
+             for ds in dynspecs]
+    for pl in plans:
+        for nm, y in (("time", pl['ydata_t']), ("frequency", pl['ydata_f'])):
+            if not np.all(np.isfinite(y)):
+                raise ValueError("the ACF %s cut has non-finite values (NaN values detected in "
+                                 "the input data)" % nm)
+    crops = []
+    if method == 'acf2d_approx':
+        for ds, pl in zip(dynspecs, plans):
+            rows, cols, tticks, fticks = _scint_crop_2d(ds, pl['tau'], pl['dnu'], a['nscale'],
+                                                        a['full_frame'], verbose)
+            box = ds.acf[rows[0]:rows[-1] + 1, cols[0]:cols[-1] + 1]
+            if not np.all(np.isfinite(box)):
+                raise ValueError("the 2-D ACF crop has non-finite values (NaN values detected "
+                                 "in the input data)")
+            crops.append((rows, cols, tticks, fticks))
+    where.update(_acf_stacks([ds for ds in dynspecs if id(ds) not in where]))
+
+    # ---- 1-D fit (dynspec.py:2651-2708) ----
+    vary1 = 0b111 | (0b1000 if alpha is None else 0)
+    descs, keep = [], []
+    for ds, pl in zip(dynspecs, plans):
+        if verbose:
+            print('Initial guesses:', '\ntau:', pl['tau'], '\ndnu:', pl['dnu'],
+                  '\namp:', pl['amp'])
+            if method == 'acf2d_approx':
+                print("\nInitialising model with 1D fit")
+            else:
+                print("\nPerforming least-squares fit to 1D ACF model")
+        stack, k = where[id(ds)]
+        nf2, nt2 = stack.shape[1:]
+        w = D.upload(np.concatenate((pl['weights_t'], pl['weights_f'])).astype(np.float64))
+        keep.append(w)
+        d = _lib.ScintFit()
+        d.acf = stack[k].data_ptr()
+        d.aux = w.data_ptr()
+        d.pitch = nt2
+        d.s0, d.s1 = float(ds.dt), float(ds.df)
+        p0 = [max(pl['tau'], 0.0), max(pl['dnu'], 0.0), max(pl['amp'], 0.0),
+              5/3 if alpha is None else alpha, 0.0]
+        d.p0 = (_lib.c_dbl * 5)(*[float(v) for v in p0])
+        d.r0, d.c0, d.n0 = nf2 // 2, nt2 // 2, pl['nt_c']
+        d.r1, d.c1, d.n1 = nf2 // 2, nt2 // 2, pl['nf_c']
+        d.vary, d.bounded, d.weighted = vary1, 0b111, 1
+        d.max_nfev = 10000 * (4 + 1)
+        descs.append(d)
+    out, info = _run_fits(1, descs)
+    names1 = ("tau", "dnu", "amp", "alpha")
+    results = []
+    for i, (ds, pl) in enumerate(zip(dynspecs, plans)):
+        fixed = {'nt': np.shape(ds.acf)[1], 'nf': np.shape(ds.acf)[0]}
+        r = _result(out[i], info[i], descs[i], names1, fixed, pl['nt_c'] + pl['nf_c'], 'acf1d')
+        _check_status(r, "1-D fit")
+        results.append(r)
+
+    # ---- 2-D fit (dynspec.py:2710-2841) ----
+    if method == 'acf2d_approx':
+        descs, keep, cuts = [], [], []
+        vary2 = 0b10110 | (0b1000 if alpha is None else 0) | (1 if a['tau_vary_2d'] else 0)
+        for i, (ds, pl) in enumerate(zip(dynspecs, plans)):
+            r1 = results[i]
+            p0 = {'tau': pl['tau'], 'dnu': pl['dnu'], 'amp': pl['amp']}
+            if r1.params['dnu'].stderr is not None:
+                p0 = {n: r1.params[n].value for n in ('tau', 'dnu', 'amp')}
+            if a['tau_input'] is not None:
+                p0['tau'] = a['tau_input']
+            p0['alpha'] = 5/3 if alpha is None else alpha
+            p0['phasegrad'] = 0.0
+            if hasattr(ds, 'acf_tilt') and ds.acf_tilt_err is not None:
+                p0['phasegrad'] = ds.acf_tilt
+            rows, cols, tticks, fticks = crops[i]
+            at = (ds.tobs - abs(tticks)) / max(tticks)
+            af = (ds.bw - abs(fticks)) / max(fticks)
+            tdata, fdata = tticks[cols], fticks[rows]
+            aux = D.upload(np.concatenate((tdata, fdata, at[cols], af[rows])).astype(np.float64))
+            keep.append(aux)
+            shf, pf, zf = _fftshift_positions(len(rows))
+            sht, pt, zt = _fftshift_positions(len(cols))
+            stack, k = where[id(ds)]
+            d = _lib.ScintFit()
+            d.acf = stack[k].data_ptr()
+            d.aux = aux.data_ptr()
+            d.pitch = stack.shape[2]
+            d.s0, d.s1, d.c = float(ds.tobs), float(ds.bw), float(ds.nsub * ds.nchan)
+            vals = [p0[n] for n in _SLOTS]
+            for s in range(3):
+                if (vary2 >> s) & 1:
+                    vals[s] = max(vals[s], 0.0)
+            d.p0 = (_lib.c_dbl * 5)(*[float(v) for v in vals])
+            d.r0, d.c0, d.n0, d.n1 = int(rows[0]), int(cols[0]), len(rows), len(cols)
+            d.shf, d.sht, d.pf, d.pt, d.zf, d.zt = shf, sht, pf, pt, zf, zt
+            d.vary, d.bounded, d.weighted = vary2, 0b111, 1 if weighted else 0
+            d.max_nfev = 10000 * ((4 if alpha is not None else 5) + 1)
+            descs.append(d)
+            cuts.append((tdata, fdata))
+            if verbose:
+                print("\nPerforming least-squares fit to approximate 2D ACF model")
+        out, info = _run_fits(2, descs)
+        for i, ds in enumerate(dynspecs):
+            fixed = {'nt': np.shape(ds.acf)[1], 'nf': np.shape(ds.acf)[0], 'tobs': ds.tobs,
+                     'bw': ds.bw, 'freq': ds.freq}
+            nd = descs[i].n0 * descs[i].n1
+            r = _result(out[i], info[i], descs[i], _SLOTS, fixed, nd, 'acf2d_approx')
+            _check_status(r, "2-D fit")
+            results[i] = r
+        for ds, r, (tdata, fdata) in zip(dynspecs, results, cuts):
+            ds._scint_crop = (tdata, fdata)
+    for ds, r in zip(dynspecs, results):
+        _scint_finish(ds, r, method, alpha, verbose, a['get_fit_report'])
+    torch.cuda.current_stream().synchronize()
+    return results
+
+
+def _scint_finish(ds, results, method, alpha, verbose, get_fit_report):
+    """The reference's attributes after the fit (dynspec.py:2946-3049)."""
+    if results.params['tau'].stderr is None or \
+       results.params['dnu'].stderr is None:
+        print("\n Warning: Could not estimate uncertainties")
+    elif (results.params['tau'].stderr > results.params['tau'].value or
+          results.params['dnu'].stderr > results.params['dnu'].value):
+        print("\n Warning: Parameters unconstrained")
+    ds.scint_param_method = method
+    if get_fit_report:
+        ds.report = results.report()
+        if verbose:
+            print("===== Fit Report Below =====")
+            print(ds.report)
+            print(" ")
+    ds.tau = results.params['tau'].value
+    ds.dnu = results.params['dnu'].value
+    ds.tscat = 1/(2*np.pi*ds.dnu)
+    if ds.dnu < ds.df:
+        print("Warning: Scint bandwidth < channel bandwidth.")
+    nscint = (1 + 0.2*ds.bw/(ds.dnu)) * (1 + 0.2*ds.tobs/(ds.tau*np.log(2)))
+    ds.nscint = nscint
+    ds.fse_tau = ds.tau/(2*np.sqrt(nscint))
+    fit_tau = results.params['tau'].stderr
+    ds.fse_dnu = ds.dnu/(2*np.sqrt(nscint))
+    fit_dnu = results.params['dnu'].stderr
+    if verbose:
+        print("\nFinite scintle errors (tau, dnu):\n", ds.fse_tau, ds.fse_dnu)
+        print("\nFit errors (tau, dnu):\n", fit_tau, fit_dnu)
+    if fit_dnu is None:
+        fit_dnu = np.inf
+    if fit_tau is None:
+        fit_tau = np.inf
+    ds.tauerr = np.sqrt(fit_tau**2 + ds.fse_tau**2)
+    ds.dnuerr = np.sqrt(fit_dnu**2 + ds.fse_dnu**2)
+    ds.amp = results.params['amp'].value
+    ds.amperr = results.params['amp'].stderr
+    ds.wn = 1 - ds.amp
+    if 'sim:mb2=' in ds.name:
+        ds.wn = 0
+    if alpha is None:
+        ds.talpha = results.params['alpha'].value
+        ds.talphaerr = results.params['alpha'].stderr
+    else:
+        ds.talpha = alpha
+        ds.talphaerr = 0
+    if method == 'acf2d_approx':
+        tdata, fdata = ds.__dict__.pop('_scint_crop')
+        p = {n: results.params[n].value for n in _SLOTS}
+        model = _acf2d_model(p, tdata, fdata, ds.tobs, ds.bw)
+        weights = np.ones(np.shape(model))
+        weights = np.fft.fftshift(weights)
+        weights[-1, -1] = 0
+        weights = np.fft.ifftshift(weights)
+        ds.acf_model = -((np.zeros(np.shape(model)) - model) * weights)
+        ds.phasegrad = results.params['phasegrad'].value
+        fit_ph = results.params['phasegrad'].stderr
+        if fit_ph is None:
+            fit_ph = np.inf
+        fse_ph = ds.phasegrad * np.sqrt((ds.fse_dnu/ds.dnu)**2 + (ds.fse_tau/ds.tau)**2)
+        ds.phasegraderr = fit_ph
+        ds.fse_phasegrad = fse_ph
+    if verbose:
+        print("\n\t ACF FIT PARAMETERS\n")
+        print("tau:\t\t\t{val} +/- {err} s".format(val=ds.tau, err=ds.tauerr))
+        print("dnu:\t\t\t{val} +/- {err} MHz".format(val=ds.dnu, err=ds.dnuerr))
+        if alpha is None:
+            print("alpha:\t\t\t{val} +/- {err}".format(val=ds.talpha, err=ds.talphaerr))
+        if method == 'acf2d_approx':
+            err = np.sqrt(ds.phasegraderr**2 + fse_ph**2)
+            print("phase grad:\t\t{val} +/- {err}".format(val=ds.phasegrad, err=err))
 
 
 class BasicDyn:
@@ -633,6 +1172,98 @@ class Dynspec(ArcFitMixin):
             self.acf = arr
         else:
             return arr
+
+    # ------------------------------------------------------------------
+    # scintillation scales (csrc/scintfit.cu)
+    # ------------------------------------------------------------------
+    def get_scint_params(self, method="acf1d", plot=False, alpha=5/3, mcmc=False,
+                         full_frame=False, nscale=5, nwalkers=50, steps=10000, burn=0.25,
+                         nitr=1, lnsigma=True, verbose=False, progress=True, display=True,
+                         filename=None, dpi=200, nan_policy='raise', weighted=True, workers=1,
+                         tau_vary_2d=True, tau_input=None, bartlett=True, get_fit_report=True):
+        """Scintillation timescale tau (s) and decorrelation bandwidth dnu (MHz) from
+        self.acf (reference dynspec.py:2470-3156), computed with calc_acf() if missing.
+
+        method 'nofit' (estimates from the 1/e and 1/2 levels, returns None), 'acf1d' (the
+        two central ACF cuts) or 'acf2d_approx' (the approximate 2-D model with a phase
+        gradient, started from the 1-D fit).  alpha=None frees the exponent.  The
+        reference's attributes are set (tau, dnu, amp, wn, their errors, tscat, nscint,
+        fse_tau, fse_dnu, talpha, talphaerr, scint_param_method; the nofit estimates
+        dnu_est, dnu_esterr, tscat_est, modulation_index, wnerr; for acf2d_approx
+        acf_model, phasegrad, phasegraderr, fse_phasegrad) and its warnings printed.
+
+        The least-squares fits run on the device (Levenberg-Marquardt with analytic float64
+        Jacobians, lmfit's bound transform for tau, dnu and amp, and lmfit's standard
+        errors); the result's fields are those of lmfit's MinimizerResult that callers
+        read (see ScintFitResult).  Deviations: self.report is a plain-text summary, not
+        lmfit's fit_report layout; the fit stops at a stationary point, tighter than
+        lmfit's 1e-7 tolerances.  NotImplementedError, before any device work, for plot,
+        mcmc, method 'acf2d' / 'sspec' and nan_policy other than 'raise'; ValueError for a
+        non-finite ACF cut or crop, a non-finite residual during a fit, or a dynamic
+        spectrum outside nf 2..32768, nt 5..16384.  nwalkers, steps, burn, nitr, lnsigma,
+        progress, display, filename, dpi and workers only concern mcmc and plotting."""
+        return get_scint_params_batch(
+            [self], method=method, plot=plot, alpha=alpha, mcmc=mcmc, full_frame=full_frame,
+            nscale=nscale, verbose=verbose, nan_policy=nan_policy, weighted=weighted,
+            tau_vary_2d=tau_vary_2d, tau_input=tau_input, bartlett=bartlett,
+            get_fit_report=get_fit_report)[0]
+
+    def get_acf_tilt(self, plot=False, tmax=None, fmax=None, display=True, filename=None,
+                     nscale=0.8, nscaleplot=2, nmin=5, dpi=200, method='acf1d', tmaxplot=None,
+                     fmaxplot=None):
+        """Tilt of the ACF in min/MHz, proportional to the phase gradient along Veff
+        (reference dynspec.py:2283-2468): a 7-point parabola through the peak of every
+        frequency-lag row within fmax, and a weighted straight line through the peaks.
+        Sets acf_tilt, acf_tilt_err and fse_tilt; runs calc_acf and get_scint_params(method)
+        first when self.acf / self.dnu are missing.  Host arithmetic on self.acf."""
+        from .arcfit import fit_parabola
+        if plot:
+            raise NotImplementedError("plotting is outside the GPU path")
+        if not hasattr(self, 'acf'):
+            self.calc_acf()
+        if not hasattr(self, 'dnu'):
+            self.get_scint_params(method=method)
+        if tmax is None:
+            tmax = nscale*self.tau/60
+        if fmax is None:
+            fmax = nscale*self.dnu
+        acf = cp(self.acf)
+        nr, nc = np.shape(acf)
+        t_delays = np.linspace(-self.tobs/60, self.tobs/60, nc+1)[:-1]
+        f_shifts = np.linspace(-self.bw, self.bw, nr+1)[:-1]
+        inds = np.argwhere(abs(f_shifts) <= fmax)
+        if len(inds) < nmin:
+            inds = np.argwhere(abs(f_shifts) <= nmin*self.df)
+        peak_array = []
+        peakerr_array = []
+        y_array = []
+        for ii in inds:
+            x_max = np.argmax(acf[ii, :]).squeeze()
+            ydata = np.array(acf[ii, x_max - 3:x_max + 4]).squeeze()
+            xdata = t_delays[x_max - 3:x_max + 4]
+            yfit, peak, peakerr = fit_parabola(xdata, ydata)
+            peak_array.append(peak)
+            peakerr_array.append(peakerr)
+            y_array.append(f_shifts[ii])
+        peak_array = np.array(peak_array).squeeze()
+        y_array = np.array(y_array).squeeze()
+        peakerr_array = np.array(peakerr_array).squeeze()
+        params, pcov = np.polyfit(peak_array, y_array, 1, cov=True, w=1/peakerr_array)
+        xfit = (y_array - params[1])/params[0]
+        errors = []
+        for i in range(len(params)):
+            errors.append(np.absolute(pcov[i][i])**0.5)
+        errors = np.array(errors).squeeze()
+        res = np.array(peak_array - xfit).squeeze()
+        reduced_chi_sq = np.sum(res**2/peakerr_array**2)/(len(xfit) - 2)
+        errors *= np.sqrt(reduced_chi_sq)
+        self.acf_tilt = 1/(float(params[0].squeeze()))
+        acf_tilt_err = float(errors[0].squeeze()) * 1/float(params[0].squeeze())**2
+        N = (1 + 0.2*self.bw/(self.dnu)) * (1 + 0.2*self.tobs/(self.tau*np.log(2)))
+        fse_tau = self.tau/(2*np.sqrt(N))
+        fse_dnu = self.dnu/(2*np.sqrt(N))
+        self.fse_tilt = self.acf_tilt * np.sqrt((fse_dnu/self.dnu)**2 + (fse_tau/self.tau)**2)
+        self.acf_tilt_err = acf_tilt_err
 
     # ------------------------------------------------------------------
     # theta-theta
