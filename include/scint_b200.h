@@ -550,6 +550,34 @@ int sb_scint_fit_1d(const sb_scint_fit* fits, int32_t nfit, double* out, int32_t
 int sb_scint_fit_2d(const sb_scint_fit* fits, int32_t nfit, double* out, int32_t* info,
                     void* stream);
 
+/* ---- scint_sim.ACF ------------------------------------------------------- */
+
+/* The analytic intensity ACF of scint_sim.ACF.calc_acf (scint_sim.py:494-678), in float64.
+ * Device arrays, built on the host with the reference's numpy expressions: snp [n1] (main
+ * grid), snp2 [n2] (core grid, used for dnun[1]), dnun [ndnun], snx and sny [nsn] (the time
+ * lags' positions).  Scalars: sigxn, sigyn (the phase-gradient offsets), sqrtar = sqrt(ar),
+ * alph2 = alpha / 2, step1 and step2 (the two grids' steps), wn_amp = wn / amp, amp.
+ * quadrant != 0 for phasegrad == 0: nsn lags from 0 and the quadrant mirrored both ways,
+ * wn_amp added at lag 0; else nsn lags across the full range, the half plane
+ * point-reflected, wn_amp added where snx == 0 exactly.
+ * Outputs (device): acf float64 [2 ndnun - 1][quadrant ? 2 nsn - 1 : nsn] = amp |gamma|^2;
+ * efield float64 [n1][n1], the e-field ACF on the main grid (acf_efield).
+ * Sizes: n1, n2 1..16384, ndnun 2..4096, nsn 1..8191, else SB_ERR_UNSUPPORTED.  Workspace:
+ * the core-grid table (8 n2^2 bytes), 512-byte partial sums and a 16-byte entry per block
+ * of the contraction; at the limits about 2.2 GB for the table and 0.6 GB for the rest.
+ * Nothing is atomic: a repeated call is bit-identical. */
+typedef struct sb_acf_model {
+    const double* snp;
+    const double* snp2;
+    const double* dnun;
+    const double* snx;
+    const double* sny;
+    int32_t n1, n2, ndnun, nsn, quadrant;
+    double sigxn, sigyn, sqrtar, alph2, step1, step2, wn_amp, amp;
+} sb_acf_model;
+
+int sb_acf_model_f64(const sb_acf_model* m, double* acf, double* efield, void* stream);
+
 /* ---- scint_sim.Simulation ------------------------------------------------ */
 
 typedef struct sb_sim_params {

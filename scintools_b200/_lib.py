@@ -59,6 +59,16 @@ class ScintFit(ctypes.Structure):
                 ("weighted", c_int), ("max_nfev", c_int)]
 
 
+
+class AcfModel(ctypes.Structure):
+    """struct sb_acf_model"""
+    _fields_ = [("snp", vp), ("snp2", vp), ("dnun", vp), ("snx", vp), ("sny", vp),
+                ("n1", c_int), ("n2", c_int), ("ndnun", c_int), ("nsn", c_int),
+                ("quadrant", c_int), ("sigxn", c_dbl), ("sigyn", c_dbl), ("sqrtar", c_dbl),
+                ("alph2", c_dbl), ("step1", c_dbl), ("step2", c_dbl), ("wn_amp", c_dbl),
+                ("amp", c_dbl)]
+
+
 _SIGS = {
     "sb_abi_version": (c_int, []),
     "sb_last_error": (ctypes.c_char_p, []),
@@ -114,6 +124,7 @@ _SIGS = {
     "sb_medfilt_masked_f64": (c_int, [vp, c_int, c_int, vp, c_int, c_int, c_int, c_dbl, vp, vp]),
     "sb_scint_fit_1d": (c_int, [ctypes.POINTER(ScintFit), c_int, vp, vp, vp]),
     "sb_scint_fit_2d": (c_int, [ctypes.POINTER(ScintFit), c_int, vp, vp, vp]),
+    "sb_acf_model_f64": (c_int, [ctypes.POINTER(AcfModel), vp, vp, vp]),
     "sb_sim_weights": (c_int, [ctypes.POINTER(SimParams), vp, vp]),
     "sb_sim_screen": (c_int, [c_int, c_int, vp, vp, vp, ctypes.c_uint64, vp, vp]),
     "sb_sim_intensity": (c_int, [c_int, c_int, c_int, vp, vp, c_dbl, c_dbl, vp,

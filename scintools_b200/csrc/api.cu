@@ -195,6 +195,7 @@ int medfilt_masked(const double* img, int nf, int nt, const int* pix, int n, int
                    double nan_value, double* out, cudaStream_t st);
 int scint_fit_1d(const sb_scint_fit* fits, int nfit, double* out, int* info, cudaStream_t st);
 int scint_fit_2d(const sb_scint_fit* fits, int nfit, double* out, int* info, cudaStream_t st);
+int acf_model(const sb_acf_model* m, double* acf, double* efield, cudaStream_t st);
 
 int gerchberg_saxton(float2* W, const float* amp, const unsigned char* rowmask, int n0, int n1,
                      int niter, cudaStream_t st);
@@ -610,6 +611,10 @@ int sb_scint_fit_1d(const sb_scint_fit* fits, int32_t nfit, double* out, int32_t
 int sb_scint_fit_2d(const sb_scint_fit* fits, int32_t nfit, double* out, int32_t* info,
                     void* stream) {
     return sb::scint_fit_2d(fits, nfit, out, info, (cudaStream_t)stream);
+}
+
+int sb_acf_model_f64(const sb_acf_model* m, double* acf, double* efield, void* stream) {
+    return sb::acf_model(m, acf, efield, (cudaStream_t)stream);
 }
 
 int sb_convert_f64_f32(const double* src, float* dst, int64_t n, void* stream) {

@@ -263,7 +263,8 @@ def _scint_args_check(method, plot, mcmc, nan_policy):
     if mcmc:
         raise NotImplementedError("mcmc sampling is outside the GPU path")
     if method == 'acf2d':
-        raise NotImplementedError("method='acf2d' needs scint_sim.ACF, which is not ported")
+        raise NotImplementedError("method='acf2d' (the fit of the scint_sim.ACF model) is "
+                                  "not ported")
     if method == 'sspec':
         raise NotImplementedError("method='sspec' does not work in the reference either")
     if method not in ('nofit', 'acf1d', 'acf2d_approx'):

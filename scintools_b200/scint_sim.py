@@ -1,5 +1,5 @@
 """CUDA-native mirror of scintools.scint_sim.Simulation
-(reference scintools/scint_sim.py:23-311).
+(reference scintools/scint_sim.py:23-311) and scint_sim.ACF (:417-765).
 
 Same constructor signature and the same attributes afterwards (w, xyp, xyi,
 spe, spi, dyn, freqs, times, df, dt, eta, betaeta, ...), so the result drops
@@ -19,7 +19,9 @@ Provenance: the scalar bookkeeping -- ``set_constants`` (scint_sim.py:137-167),
 (:81-133) -- follows the reference LINE BY LINE (same expressions, comments
 dropped), because the drop-in contract is "identical attributes" and SURVEY.md
 a12 / a15 keep this glue in Python.  It is restated reference code, not new design;
-what is new here is everything that touches the device.
+what is new here is everything that touches the device.  ``ACF`` follows the same rule:
+its axes and scalars are the reference's numpy expressions, and the double sum of every
+lag runs in libscint_b200 (sb_acf_model_f64).
 """
 import numpy as np
 import scipy.constants as sc
@@ -230,3 +232,192 @@ class Simulation():
         else:
             col = self.xyp[:, int(self.ny / 2)]
         self.dm = col * self.dlam / np.pi
+
+
+# sizes the device contraction takes (csrc/acf_model.cu)
+_ACF_MAX_GRID = 16384
+_ACF_MAX_N = 8191
+
+
+def _arange_len(start, stop, step):
+    """len(np.arange(start, stop, step)), from numpy's own formula, without allocating; a
+    zero step raises ZeroDivisionError as np.arange does."""
+    return max(int(np.ceil((float(stop) - float(start)) / float(step))), 0)
+
+
+class ACF():
+    """The theoretical intensity ACF of Rickett et al. (2014, App. A) for an anisotropic
+    medium with a phase gradient (scint_sim.py:417-765).
+
+    Same constructor signature and the same attributes afterwards: alpha ar psi phasegrad
+    theta amp wn taumax dnumax nf nt sp_fac res_fac core_fac dsp ddnun fn tn sn snp acf
+    acf_efield.  The axes are built on the host with the reference's expressions; the
+    e-field ACF and the double sum of every (time lag, frequency lag) run on the device in
+    float64 as a bilinear form (csrc/acf_model.cu).  No device memory is held afterwards.
+
+    The reference's errors are kept, raised before any device work: even nf / nt become
+    odd; nf = 1 raises IndexError, nt = 1 and amp = 0 ZeroDivisionError.  Deviations:
+    non-finite parameters, ar <= 0 and dnumax = 0 raise ValueError (the reference returns
+    NaN), as do spatial grids of more than 16384 points per side and nf or nt above 8191.
+    ``plot=True`` and the ``plot_*`` methods raise NotImplementedError.
+    """
+
+    def __init__(self, psi=0, phasegrad=0, theta=0, ar=1, alpha=5/3,
+                 taumax=4, dnumax=4, nf=51, nt=51, amp=1, wn=0,
+                 spatial_factor=2, resolution_factor=1, core_factor=2,
+                 auto_sampling=True, plot=False, display=True):
+        if plot:
+            raise NotImplementedError("plotting is outside the GPU hot path")
+        self.alpha = alpha
+        self.ar = ar
+        self.psi = psi
+        self.phasegrad = phasegrad
+        self.theta = theta
+        self.amp = amp
+        self.wn = wn
+        self.taumax = taumax
+        spmax = taumax
+        self.dnumax = dnumax
+        if nf % 2 == 0:
+            nf += 1
+        if nt % 2 == 0:
+            nt += 1
+        self.nf = nf
+        self.nt = nt
+        if auto_sampling:
+            self.sp_fac = 6 * ar/spmax
+            self.res_fac = 1 + ar/3
+            self.core_fac = 4
+        else:
+            self.sp_fac = spatial_factor
+            self.res_fac = resolution_factor
+            self.core_fac = core_factor
+        self.dsp = 4*spmax/(nt-1)
+        self.calc_acf()
+
+    def _axes(self):
+        """The host half of calc_acf (scint_sim.py:538-587, 630-637): every axis and scalar
+        in the reference's expressions and order, so its exceptions come first.  Then the
+        checks this port adds.  Returns a dict; nothing touches the device."""
+        alph2 = self.alpha/2
+        spmax = self.taumax
+        dnumax = self.dnumax
+        dsp = self.dsp
+        phasegrad = self.phasegrad
+        theta = self.theta
+        amp = self.amp
+        wn = self.wn
+        xi = 90 - self.psi
+        with np.errstate(all="ignore"):
+            Vx = np.cos(xi*np.pi/180)
+            Vy = np.sin(xi*np.pi/180)
+            sigxn = phasegrad * np.cos((xi - theta)*np.pi/180)
+            sigyn = phasegrad * np.sin((xi - theta)*np.pi/180)
+            ar = self.ar
+            sqrtar = np.sqrt(ar)
+        dnun = np.linspace(0, dnumax, int(np.ceil(self.nf/2)))
+        ddnun = np.abs(dnun[1] - dnun[0])
+        sp_fac = self.sp_fac
+        res_fac = self.res_fac
+        core_fac = self.res_fac * self.core_fac
+        start, stop1, stop2 = -sp_fac*spmax, sp_fac*spmax + dsp/res_fac, \
+            sp_fac*spmax + dsp/core_fac
+        n1 = _arange_len(start, stop1, dsp/res_fac)
+        n2 = _arange_len(start, stop2, dsp/core_fac)
+        quadrant = phasegrad == 0
+        if quadrant:
+            tn = np.linspace(0, (spmax), int(np.ceil(self.nt/2)))
+            snx = Vx*tn
+            sny = Vy*tn
+        else:
+            tn = np.linspace(-(spmax), (spmax), self.nt)
+            snx = np.cos(xi*np.pi/180)*tn
+            sny = np.sin(xi*np.pi/180)*tn
+        wn_amp = wn/amp
+        scalars = [self.alpha, self.ar, self.psi, phasegrad, theta, amp, wn, spmax, dnumax,
+                   dsp, sp_fac, res_fac, core_fac, wn_amp]
+        if not all(np.isfinite(np.asarray(v, dtype=np.float64)).all() for v in scalars):
+            raise ValueError("ACF parameters must be finite")
+        if not ar > 0:
+            raise ValueError("ar must be positive (the reference returns NaN)")
+        if dnumax == 0:
+            raise ValueError("dnumax must be non-zero (the reference divides by it)")
+        if not (1 <= n1 <= _ACF_MAX_GRID and 1 <= n2 <= _ACF_MAX_GRID):
+            raise ValueError("spatial grids of %d and %d points are outside 1..%d"
+                             % (n1, n2, _ACF_MAX_GRID))
+        if not (3 <= self.nf <= _ACF_MAX_N and 3 <= self.nt <= _ACF_MAX_N):
+            raise ValueError("nf = %s and nt = %s must be within 3..%d"
+                             % (self.nf, self.nt, _ACF_MAX_N))
+        snp = np.arange(-sp_fac*spmax, sp_fac*spmax + dsp/res_fac, dsp/res_fac)
+        snp2 = np.arange(-sp_fac*spmax, sp_fac*spmax + dsp/core_fac, dsp/core_fac)
+        assert len(snp) == n1 and len(snp2) == n2
+        if quadrant:
+            t2 = np.concatenate((np.flip(-tn[1:]), tn)).squeeze()
+        else:
+            t2 = tn
+        f2 = np.concatenate((np.flip(-dnun[1:]), dnun)).squeeze()
+        return dict(alph2=alph2, sigxn=float(sigxn), sigyn=float(sigyn),
+                    sqrtar=float(sqrtar), dnun=dnun, ddnun=ddnun, snp=snp, snp2=snp2,
+                    step1=dsp/res_fac, step2=dsp/core_fac, quadrant=bool(quadrant),
+                    snx=np.asarray(snx, dtype=np.float64),
+                    sny=np.asarray(sny, dtype=np.float64), wn_amp=float(wn_amp),
+                    amp=float(amp), fn=f2, t2=t2)
+
+    def calc_acf(self, plot=False):
+        """Computes the 2-D ACF of intensity vs time and frequency lag (scint_sim.py:494-678),
+        re-reading the attributes as the reference does."""
+        if plot:
+            raise NotImplementedError("plotting is outside the GPU hot path")
+        import torch
+        ax = self._axes()
+        snp, snp2, dnun = ax["snp"], ax["snp2"], ax["dnun"]
+        nsn, ndnun = len(ax["snx"]), len(dnun)
+        nt_out = 2 * nsn - 1 if ax["quadrant"] else nsn
+        d = [D.upload(np.ascontiguousarray(v, dtype=np.float64))
+             for v in (snp, snp2, dnun, ax["snx"], ax["sny"])]
+        m = _lib.AcfModel(d[0].data_ptr(), d[1].data_ptr(), d[2].data_ptr(), d[3].data_ptr(),
+                          d[4].data_ptr(), len(snp), len(snp2), ndnun, nsn,
+                          int(ax["quadrant"]), ax["sigxn"], ax["sigyn"], ax["sqrtar"],
+                          float(ax["alph2"]), float(ax["step1"]), float(ax["step2"]),
+                          ax["wn_amp"], ax["amp"])
+        d_acf = D.empty((2 * ndnun - 1, nt_out), torch.float64)
+        d_ef = D.empty((len(snp), len(snp)), torch.float64)
+        _lib.check(_lib.lib.sb_acf_model_f64(m, d_acf.data_ptr(), d_ef.data_ptr(),
+                                              D.stream_ptr()))
+        self.ddnun = ax["ddnun"]
+        self.fn = ax["fn"]
+        self.tn = ax["t2"]
+        self.sn = ax["t2"]
+        self.snp = snp
+        self.acf = d_acf.cpu().numpy()
+        self.acf_efield = d_ef.cpu().numpy()
+
+    def calc_sspec(self, window='hanning', window_frac=1):
+        """The secondary spectrum of the ACF, 10 log10 |fftshift(fft2(fftshift(windowed)))|
+        (scint_sim.py:728-742), through the chirp-z 2-D transform (float32).  For a real
+        input |fft2| = n0 n1 |ifft2|."""
+        import torch
+        from .dynspec import get_window
+        nf, nt = np.shape(self.acf)
+        chan_window, subint_window = get_window(nt, nf, window=window, frac=window_frac)
+        arr = np.multiply(chan_window, self.acf)
+        arr = np.transpose(np.multiply(subint_window, np.transpose(arr)))
+        arr = np.fft.fftshift(arr)
+        d_in = D.upload_f32(arr.astype(np.complex128))
+        d_out = D.empty((nf, nt, 2), torch.float32)
+        _lib.check(_lib.lib.sb_ifft2_c2c_f32(d_in.data_ptr(), nf, nt, 0, 0, 0,
+                                              float(nf) * float(nt), 0, d_out.data_ptr(),
+                                              D.stream_ptr()))
+        a = d_out.cpu().numpy().astype(np.float64)
+        amp = np.fft.fftshift(np.hypot(a[..., 0], a[..., 1]))
+        with np.errstate(divide="ignore"):
+            self.sspec = 10*np.log10(amp)
+
+    def plot_acf(self, display=True, contour=True, filled=False):
+        raise NotImplementedError("plotting is outside the GPU hot path")
+
+    def plot_acf_efield(self, display=True):
+        raise NotImplementedError("plotting is outside the GPU hot path")
+
+    def plot_sspec(self, display=True, vmin=None, vmax=None):
+        raise NotImplementedError("plotting is outside the GPU hot path")
