@@ -124,7 +124,8 @@ int sb_thth_map(const sb_thth_geom* geom, double eta, int32_t hermitian,
  * arclet curvature per trial).  center_cut: columns with |theta1| < center_cut
  * are zeroed.  power=1 gathers |CS|^2 (incoherent thin search, :609).
  * Outputs: svals float64 [neta] (NaN where numpy would raise), status (SB_ETA_*
- * bits), n1_red / n2_red (cropped sizes), iters. */
+ * bits), n1_red / n2_red (cropped sizes), iters.  Pairs run in batches whose
+ * matrices fit the 3 GiB budget of sb_eta_sweep (SB_SWEEP_SLAB_MB overrides it). */
 int sb_thin_sweep(const sb_thth_geom* geom, const double* th2_cents, int32_t n_th2,
                   double center_cut, int32_t power, const double* eta1, const double* eta2,
                   int32_t neta, double tol, int32_t max_iter, double* svals,

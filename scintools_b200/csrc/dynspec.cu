@@ -13,7 +13,6 @@
 #include <stdlib.h>
 
 #include "fft_kernels.cuh"
-#include "chisq.cuh"
 
 namespace sb {
 
@@ -632,7 +631,8 @@ int conj_spectrum_bound(const float* dyn, int nf, int nt, int npad, float pad_va
 //   X[k] = w[k] * sum_n (x[n] w[n]) conj(w)[k - n],  w[n] = exp(-i pi n^2 / N)
 // = w[k] * IFFT_M( FFT_M(x w) * FFT_M(b) )[k],  M = 2^p >= 2N - 1.
 // Full plane output (no Hermitian shortcut), generic fftshift (odd N too).
-// Chirp tables and the load / store functors of these passes: fft_functors.cuh
+// Chirp tables and the load / store functors of these passes: fft_functors.cuh; the
+// 2-D driver chirp_fft2: fft_kernels.cuh
 // ------------------------------------------------------------------------
 // chirp w[N] and the transformed kernel B = FFT_M(b)
 int bluestein_tables(int N, int M, float2* w, float2* B, float2* scratch, cudaStream_t st) {
@@ -654,52 +654,6 @@ int bluestein_tables(int N, int M, float2* w, float2* B, float2* scratch, cudaSt
     ColVecLoad la{scratch, R2};
     ColVecStore sb_{B, R1};
     return cols_generic<float, -1>(la, scratch + M, 1, M, 1, sb_, st);
-}
-
-// Forward chirp-z transform of an n0 x n1 plane whose first `live` rows are read by
-// ld (ChirpRowLoad or ChirpRowLoadC; its chirp w is set here) and whose other rows
-// are zero.  The final column pass stores through mk(R1, wF, MF) (wF: chirp of the
-// column axis, MF: its padded length); columns >= ncols are never stored.  `what`
-// begins the error message of a size outside the limits.
-template <class RowLoad, class MakeStore>
-static int chirp_fft2(RowLoad ld, int n0, int n1, int live, int ncols, MakeStore mk,
-                      const char* what, cudaStream_t st) {
-    const int MT = next_pow2(2L * n1 - 1), MF = next_pow2(2L * n0 - 1);
-    // M >= 8 on both axes: bluestein_tables transforms the kernel with a row FFT (>= 8 points)
-    if (MT < 8 || MT > 16384 || MF < 8 || MF > 65536) {
-        set_error("%s %d x %d outside 3..32768 x 3..8192 (rows 3..32768, cols 3..8192)", what,
-                  n0, n1);
-        return SB_ERR_UNSUPPORTED;
-    }
-    const long pt = ((long)n1 + 15) & ~15L;
-    float2* tabs = (float2*)workspace(6, (size_t)(n1 + 3L * MT + n0 + 3L * MF + 64) * sizeof(float2));
-    float2* R1buf = (float2*)workspace(3, (size_t)live * MT * sizeof(float2));
-    float2* Ybuf = (float2*)workspace(4, (size_t)live * pt * sizeof(float2));
-    float2* C0 = (float2*)workspace(5, (size_t)MF * pt * sizeof(float2));
-    float2* C1 = (float2*)workspace(7, (size_t)MF * pt * sizeof(float2));
-    if (!tabs || !R1buf || !Ybuf || !C0 || !C1) return SB_ERR_NOMEM;
-    float2* wT = tabs;
-    float2* BT = wT + n1;
-    float2* wF = BT + MT;
-    float2* BF = wF + n0;
-    float2* scratch = BF + MF;      // 2*max(MT, MF)
-    int rc = bluestein_tables(n1, MT, wT, BT, scratch, st);
-    if (rc) return rc;
-    rc = bluestein_tables(n0, MF, wF, BF, scratch, st);
-    if (rc) return rc;
-    // rows: chirp, FFT, multiply, inverse FFT, chirp
-    rc = chirp_rows(ld, ChirpOutRowStore{Ybuf, pt, wT, n1, 1.0f / (float)MT}, R1buf, MT, live,
-                    wT, BT, st);
-    if (rc) return rc;
-    // columns
-    int R1, R2;
-    split_len(MF, &R1, &R2);
-    ChirpColALoad la{Ybuf, pt, R2, live, wF};
-    MulVecColStore mc{C1, pt, R1, BF};
-    rc = cols_generic<float, -1>(la, C0, pt, MF, ncols, mc, st);
-    if (rc) return rc;
-    StrideALoad<float2> pa{C1, pt, R2};
-    return cols_generic<float, +1>(pa, C0, pt, MF, ncols, mk(R1, wF, MF), st);
 }
 
 // conjugate spectrum of a zero(/constant)-padded chunk
@@ -766,46 +720,6 @@ int conj_spectrum(const float* dyn, int nf, int nt, int npad, float pad_value,
     CsStore cs{CS, NF, NT, R1, rowmask, pad_value * (float)NF * (float)NT, half, cs_pitch,
                dev_mean ? stats : nullptr};
     return cols_forward(H, A, pitch, NF, nf, ncols, cs, st, PROF_CS_COLA, PROF_CS_COLB);
-}
-
-
-// out[:crop0, :crop1] = scale * ifft2(ifftshift(in)) for ANY sizes (phase retrieval
-// on the tutorial's 256 x 600 conjugate spectrum), by the chirp-z transform:
-// ifft2(X) = conj(fft2(conj X)) / (N0 N1).  conj_in != 0: returns ifft2(conj(in)) =
-// conj(fft2(in)) / (n0 n1) (the forward transform of the Gerchberg-Saxton loop)
-int ifft2_c2c_any(const float2* in, int n0, int n1, int centred, int crop0, int crop1,
-                  double scale, int real_only, void* out, cudaStream_t st, int conj_in) {
-    if (crop0 <= 0 || crop0 > n0) crop0 = n0;
-    if (crop1 <= 0 || crop1 > n1) crop1 = n1;
-    return chirp_fft2(ChirpRowLoadC{in, n0, n1, centred, conj_in, nullptr}, n0, n1, n0, crop1,
-                      [&](int R1, const float2* wF, int MF) {
-                          const double den = (double)MF * (double)n0 * (double)n1;
-                          return ChirpCropStore{real_only ? nullptr : (float2*)out,
-                                                real_only ? (float*)out : nullptr, R1,
-                                                crop0, crop1, wF, (float)(scale / den)};
-                      }, "ifft2 (chirp-z):", st);
-}
-
-// chisq_sweep (retrieval.cu): sum over the mask of (real(ifft2(ifftshift(in)))[:nf, :nt] -
-// dspec)^2 for any size, added to the sink's partial sums
-struct ChirpResidualStore {
-    int R1;
-    const float2* w;
-    float scale;
-    ResidualSink sink;
-    __device__ __forceinline__ void operator()(int y, int k, int c, float2 v) const {
-        const int kf = y + R1 * k;
-        if (kf >= sink.nf || c >= sink.nt) return;
-        sink(kf, c, cmul(v, w[kf]).x * scale);
-    }
-};
-int ifft2_any_residual(const float2* in, int n0, int n1, const ResidualSink& sink,
-                       cudaStream_t st) {
-    return chirp_fft2(ChirpRowLoadC{in, n0, n1, 1, 0, nullptr}, n0, n1, n0, sink.nt,
-                      [&](int R1, const float2* wF, int MF) {
-                          const double den = (double)MF * (double)n0 * (double)n1;
-                          return ChirpResidualStore{R1, wF, (float)(1.0 / den), sink};
-                      }, "ifft2 (chirp-z):", st);
 }
 
 // Dynspec.calc_acf(method='direct') (dynspec.py:3780-3797)

@@ -192,19 +192,41 @@ struct ChirpRowLoadC {   // a[n] = conj(x[r'][n']) * w[n] with the ifftshift fol
         return cmul(v, w[n]);
     }
 };
-struct ChirpCropStore {  // out[k][c] = conj(v * wF[k]) * scale, k < crop0, c < crop1
-    float2* outc;
-    float* outr;
-    int R1, crop0, crop1;
+
+// ------------------------------------------- inverse 2-D transforms (retrieval.cu)
+// The last column pass of the power-of-two and of the chirp-z inverse each reach a base
+// store, base(row, c, v) with v element (row, c) of the unnormalised inverse, through one
+// adapter that forms the output row, drops what lies outside rows x cols and, on the
+// chirp-z path, applies the column chirp.  Base stores: CropStore, ResidualSink.
+template <class Base> struct RadixStore {   // base(k, c, v), k = k1 + R1 k2
+    int R1, rows, cols;
+    Base base;
+    __device__ __forceinline__ void operator()(int y, int k, int c, float2 v) const {
+        const int row = y + R1 * k;
+        if (row >= rows || c >= cols) return;
+        base(row, c, v);
+    }
+};
+template <class Base> struct ChirpStore {   // base(k, c, conj(v * wF[k])), k = k1 + R1 k2
+    int R1, rows, cols;
     const float2* w;
-    float scale;
+    Base base;
     __device__ __forceinline__ void operator()(int y, int k, int c, float2 v) const {
         const int kf = y + R1 * k;
-        if (kf >= crop0 || c >= crop1) return;
+        if (kf >= rows || c >= cols) return;
         const float2 r = cmul(v, w[kf]);
-        const size_t o = (size_t)kf * crop1 + c;
-        if (outr) outr[o] = r.x * scale;
-        else outc[o] = make_float2(r.x * scale, -r.y * scale);
+        base(kf, c, make_float2(r.x, -r.y));
+    }
+};
+struct CropStore {        // out[row][c] = v * scale, or its real part
+    float2* outc;
+    float* outr;
+    int pitch;
+    float scale;
+    __device__ __forceinline__ void operator()(int row, int c, float2 v) const {
+        const size_t o = (size_t)row * pitch + c;
+        if (outr) outr[o] = v.x * scale;
+        else outc[o] = make_float2(v.x * scale, v.y * scale);
     }
 };
 

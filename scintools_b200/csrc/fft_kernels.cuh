@@ -434,4 +434,50 @@ static inline int chirp_rows(RowLoad ld, Store os, float2* buf, int MT, long nro
     return rc;
 }
 
+// Forward chirp-z transform of an n0 x n1 plane whose first `live` rows are read by
+// ld (ChirpRowLoad or ChirpRowLoadC; its chirp w is set here) and whose other rows
+// are zero.  The final column pass stores through mk(R1, wF, MF) (wF: chirp of the
+// column axis, MF: its padded length); columns >= ncols are never stored.  `what`
+// begins the error message of a size outside the limits.
+template <class RowLoad, class MakeStore>
+static inline int chirp_fft2(RowLoad ld, int n0, int n1, int live, int ncols, MakeStore mk,
+                             const char* what, cudaStream_t st) {
+    const int MT = next_pow2(2L * n1 - 1), MF = next_pow2(2L * n0 - 1);
+    // M >= 8 on both axes: bluestein_tables transforms the kernel with a row FFT (>= 8 points)
+    if (MT < 8 || MT > 16384 || MF < 8 || MF > 65536) {
+        set_error("%s %d x %d outside 3..32768 x 3..8192 (rows 3..32768, cols 3..8192)", what,
+                  n0, n1);
+        return SB_ERR_UNSUPPORTED;
+    }
+    const long pt = ((long)n1 + 15) & ~15L;
+    float2* tabs = (float2*)workspace(6, (size_t)(n1 + 3L * MT + n0 + 3L * MF + 64) * sizeof(float2));
+    float2* R1buf = (float2*)workspace(3, (size_t)live * MT * sizeof(float2));
+    float2* Ybuf = (float2*)workspace(4, (size_t)live * pt * sizeof(float2));
+    float2* C0 = (float2*)workspace(5, (size_t)MF * pt * sizeof(float2));
+    float2* C1 = (float2*)workspace(7, (size_t)MF * pt * sizeof(float2));
+    if (!tabs || !R1buf || !Ybuf || !C0 || !C1) return SB_ERR_NOMEM;
+    float2* wT = tabs;
+    float2* BT = wT + n1;
+    float2* wF = BT + MT;
+    float2* BF = wF + n0;
+    float2* scratch = BF + MF;      // 2*max(MT, MF)
+    int rc = bluestein_tables(n1, MT, wT, BT, scratch, st);
+    if (rc) return rc;
+    rc = bluestein_tables(n0, MF, wF, BF, scratch, st);
+    if (rc) return rc;
+    // rows: chirp, FFT, multiply, inverse FFT, chirp
+    rc = chirp_rows(ld, ChirpOutRowStore{Ybuf, pt, wT, n1, 1.0f / (float)MT}, R1buf, MT, live,
+                    wT, BT, st);
+    if (rc) return rc;
+    // columns
+    int R1, R2;
+    split_len(MF, &R1, &R2);
+    ChirpColALoad la{Ybuf, pt, R2, live, wF};
+    MulVecColStore mc{C1, pt, R1, BF};
+    rc = cols_generic<float, -1>(la, C0, pt, MF, ncols, mc, st);
+    if (rc) return rc;
+    StrideALoad<float2> pa{C1, pt, R2};
+    return cols_generic<float, +1>(pa, C0, pt, MF, ncols, mk(R1, wF, MF), st);
+}
+
 }  // namespace sb

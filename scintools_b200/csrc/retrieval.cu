@@ -15,7 +15,6 @@
 #include <stdlib.h>
 
 #ifndef SB_HOST_EMU            // tests/host_emu runs the scatter / eigenpair kernels on the CPU
-#include "chisq.cuh"
 #include "fft_kernels.cuh"
 #endif
 #include "lanczos.cuh"
@@ -598,8 +597,7 @@ vlbi_eigvec_kernel(const float2* __restrict__ A, int n_dish, int n, float2* __re
         return;
     }
     __shared__ int sh_info[2];
-    herm_eigvec_body(CompositeMatrix{A, N, n_dish, n}, N, Q, max_iter < N ? max_iter : N, tol, 1,
-                     w, V, sh_info);
+    herm_eigvec_body(CompositeMatrix{A, N, n_dish, n}, N, Q, max_iter, tol, 1, w, V, sh_info);
     if (threadIdx.x == 0) {        // sh_info was written by thread 0 of the body
         info[0] = sh_info[0];
         info[1] |= sh_info[1];
@@ -654,21 +652,31 @@ __global__ void vlbi_finalise_kernel(RevGeom g, float2* __restrict__ acc,
 }
 
 #ifndef SB_HOST_EMU
+// Launch setup of a top-eigenpair kernel on matrices of order n (herm_eigvec_body): tol <= 0
+// becomes 1e-7, max_iter outside 1..SB_LANCZOS_MAXIT becomes 96 and is then held to n, and
+// *smem, the body's dynamic shared memory, is set as the kernel's limit.
+template <class Kernel>
+static int eigvec_setup(Kernel kern, int n, double* tol, int* max_iter, size_t* smem) {
+    if (!(*tol > 0.0)) *tol = 1e-7;
+    if (*max_iter <= 0 || *max_iter > SB_LANCZOS_MAXIT) *max_iter = 96;
+    if (*max_iter > n) *max_iter = n;
+    *smem = sizeof(LanczosShared) + 32 * sizeof(double) + (SB_LANCZOS_MAXIT + 1) * sizeof(double2) +
+            2 * (size_t)n * sizeof(float2);
+    SB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem));
+    return SB_OK;
+}
+
 int herm_eigvec(const float2* A, int n, int ld, double tol, int max_iter, double* w_dev,
                 float2* V_dev, int* info_dev, cudaStream_t st) {
-    if (!(tol > 0.0)) tol = 1e-7;
-    if (max_iter <= 0 || max_iter > SB_LANCZOS_MAXIT) max_iter = 96;
-    if (max_iter > n) max_iter = n;
     if (n < 1 || n > 8192) {
         set_error("herm_eigvec: n = %d outside 1..8192", n);
         return SB_ERR_UNSUPPORTED;
     }
+    size_t smem;
+    int rc = eigvec_setup(herm_eigvec_kernel, n, &tol, &max_iter, &smem);
+    if (rc) return rc;
     float2* Q = (float2*)workspace(2, (size_t)(max_iter + 1) * n * sizeof(float2));
     if (!Q) return SB_ERR_NOMEM;
-    const size_t smem = sizeof(LanczosShared) + 32 * sizeof(double) +
-                        (SB_LANCZOS_MAXIT + 1) * sizeof(double2) + 2 * (size_t)n * sizeof(float2);
-    SB_CUDA(cudaFuncSetAttribute(herm_eigvec_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)smem));
     herm_eigvec_kernel<<<1, EV_THREADS, smem, st>>>(A, n, ld, Q, max_iter, tol, w_dev, V_dev,
                                                     info_dev);
     SB_LAUNCH_CHECK();
@@ -676,62 +684,111 @@ int herm_eigvec(const float2* A, int n, int ld, double tol, int max_iter, double
 }
 
 // --------------------------------------------------------------------------
-// out[:crop0, :crop1] = scale * ifft2(ifftshift(in)) for power-of-two sizes.
-// Rows (contiguous axis) in shared memory with the ifftshift folded into the
-// load, then the strided axis in four-step tiles over the kept columns only.
+// Inverse 2-D transforms of the conjugate spectra: ifft2(ifftshift(.)) of the rev_map
+// planes, cropped, into a wavefield / model or into the chi-square residual.
 // --------------------------------------------------------------------------
-struct ShiftedRowLoad {   // row r, sample n of ifftshift(in)
+// The sizes they take: powers of two 8..65536 x 8..16384 (the rows run in one
+// shared-memory row transform), other sizes 3..32768 x 3..8192 (chirp-z)
+static int ifft2_size_check(const char* who, int n0, int n1) {
+    const bool pow2 = is_pow2(n0) && is_pow2(n1);
+    if (pow2 ? (n0 < 8 || n1 < 8 || n0 > 65536 || n1 > 16384)
+             : (n0 < 3 || n1 < 3 || n0 > 32768 || n1 > 8192)) {
+        set_error("%s: conjugate spectrum %d x %d outside 8..65536 x 8..16384 (powers of two) / "
+                  "3..32768 x 3..8192 (other sizes)", who, n0, n1);
+        return SB_ERR_UNSUPPORTED;
+    }
+    return SB_OK;
+}
+
+// row r of plane p of ifftshift(in[p]), or of in[p] when not centred, for row = p n0 + r;
+// n0 and n1 are powers of two
+struct ShiftedRowLoad {
     const float2* in;
     int n0, n1, centred;
     __device__ __forceinline__ float2 operator()(long row, int n) const {
-        const int r = centred ? (int)((row + n0 / 2) & (n0 - 1)) : (int)row;
-        const int c = centred ? ((n + n1 / 2) & (n1 - 1)) : n;
-        return in[(size_t)r * n1 + c];
-    }
-};
-struct CropStore {        // out[k][c], k = k1 + R1 k2
-    float2* outc;
-    float* outr;
-    int R1, crop0, crop1;
-    float scale;
-    __device__ __forceinline__ void operator()(int y, int k, int c, float2 v) const {
-        const int row = y + R1 * k;
-        if (row >= crop0 || c >= crop1) return;
-        const size_t o = (size_t)row * crop1 + c;
-        if (outr) outr[o] = v.x * scale;
-        else outc[o] = make_float2(v.x * scale, v.y * scale);
+        const long p0 = row & ~(long)(n0 - 1);          // p n0
+        int r = (int)(row & (n0 - 1)), c = n;
+        if (centred) {
+            r = (r + n0 / 2) & (n0 - 1);
+            c = (n + n1 / 2) & (n1 - 1);
+        }
+        return in[(size_t)(p0 + r) * n1 + c];
     }
 };
 
-// dynspec.cu: chirp-z variant for arbitrary sizes
-int ifft2_c2c_any(const float2* in, int n0, int n1, int centred, int crop0, int crop1,
-                  double scale, int real_only, void* out, cudaStream_t st, int conj_in);
+// Chirp-z inverse of one [n0][n1] plane of any size, ifftshifted first when centred:
+// ifft2(X) = conj(fft2(conj X)) / (n0 n1).  conj_in != 0 transforms conj(in) instead, so
+// that the result is conj(fft2(in)) / (n0 n1).  The output rows x cols go to the base store
+// mk(den), den = the normalisation of the unnormalised inverse it receives (workspace slots
+// 3 .. 7, chirp_fft2).
+template <class MakeBase>
+static int ifft2_chirp(const float2* in, int n0, int n1, int centred, int conj_in, int rows,
+                       int cols, MakeBase mk, cudaStream_t st) {
+    return chirp_fft2(ChirpRowLoadC{in, n0, n1, centred, conj_in, nullptr}, n0, n1, n0, cols,
+                      [&](int R1, const float2* wF, int MF) {
+                          const double den = (double)MF * (double)n0 * (double)n1;
+                          return ChirpStore<decltype(mk(den))>{R1, rows, cols, wF, mk(den)};
+                      }, "ifft2 (chirp-z):", st);
+}
 
-int ifft2_c2c(const float2* in, int n0, int n1, int centred, int crop0, int crop1,
-              double scale, int real_only, void* out, cudaStream_t st) {
-    if ((n0 & (n0 - 1)) || (n1 & (n1 - 1)))
-        return ifft2_c2c_any(in, n0, n1, centred, crop0, crop1, scale, real_only, out, st, 0);
-    // rows run in one shared-memory row transform (SB_ROW_DISPATCH: 8..16384 points)
-    if (n0 < 8 || n1 < 8 || n0 > 65536 || n1 > 16384) {
-        set_error("ifft2: power-of-two sizes %d x %d outside 8..65536 x 8..16384", n0, n1);
-        return SB_ERR_UNSUPPORTED;
+// ifft2 of the nplanes planes of in [nplanes][n0][n1], each ifftshifted first when centred;
+// the output rows x cols of plane p go to the base store mk(p, den) (CropStore or
+// ResidualSink), den = the normalisation of the unnormalised inverse it receives.  Powers of
+// two: the rows of every plane in one launch, then the kept columns plane by plane
+// (workspace slots 3 and 4); other sizes: ifft2_chirp per plane.  Sizes as ifft2_size_check.
+template <class MakeBase>
+static int ifft2_planes(const float2* in, int nplanes, int n0, int n1, int centred, int rows,
+                        int cols, MakeBase mk, cudaStream_t st) {
+    const size_t bins = (size_t)n0 * n1;
+    if (!is_pow2(n0) || !is_pow2(n1)) {
+        for (int p = 0; p < nplanes; ++p) {
+            const int rc = ifft2_chirp(in + bins * p, n0, n1, centred, 0, rows, cols,
+                                       [&](double den) { return mk(p, den); }, st);
+            if (rc) return rc;
+        }
+        return SB_OK;
     }
-    if (crop0 <= 0 || crop0 > n0) crop0 = n0;
-    if (crop1 <= 0 || crop1 > n1) crop1 = n1;
-    float2* B1 = (float2*)workspace(3, (size_t)n0 * n1 * sizeof(float2));
-    float2* B2 = (float2*)workspace(4, (size_t)n0 * n1 * sizeof(float2));
+    float2* B1 = (float2*)workspace(3, nplanes * bins * sizeof(float2));
+    float2* B2 = (float2*)workspace(4, bins * sizeof(float2));
     if (!B1 || !B2) return SB_ERR_NOMEM;
     ShiftedRowLoad ld{in, n0, n1, centred};
     PlainRowStore<float2> rs{B1, n1};
     int rc = SB_OK;
-    SB_ROW_DISPATCH(n1, rc = (launch_row_c2c<float, N1, N2, +1>(ld, rs, n0, st)));
+    SB_ROW_DISPATCH(n1, rc = (launch_row_c2c<float, N1, N2, +1>(ld, rs, (long)nplanes * n0, st)));
     if (rc) return rc;
     int R1, R2;
     split_len(n0, &R1, &R2);
-    StrideALoad<float2> la{B1, n1, R2};
-    CropStore cs{real_only ? nullptr : (float2*)out, real_only ? (float*)out : nullptr, R1,
-                 crop0, crop1, (float)(scale / ((double)n0 * (double)n1))};
-    return cols_generic<float, +1>(la, B2, n1, n0, crop1, cs, st);
+    const double den = (double)n0 * (double)n1;
+    for (int p = 0; p < nplanes; ++p) {
+        StrideALoad<float2> la{B1 + bins * p, n1, R2};
+        const auto base = mk(p, den);
+        rc = cols_generic<float, +1>(la, B2, n1, n0, cols,
+                                     RadixStore<decltype(base)>{R1, rows, cols, base}, st);
+        if (rc) return rc;
+    }
+    return SB_OK;
+}
+
+// scale * ifft2(conj(in)) = scale * conj(fft2(in)) / (n0 n1) of one plane of any size: the
+// forward transform of the Gerchberg-Saxton loop and of conj_spectrum_c2c
+static int ifft2_conj_any(const float2* in, int n0, int n1, double scale, float2* out,
+                          cudaStream_t st) {
+    return ifft2_chirp(in, n0, n1, 0, 1, n0, n1, [&](double den) {
+        return CropStore{out, nullptr, n1, (float)(scale / den)};
+    }, st);
+}
+
+// out[:crop0, :crop1] = scale * ifft2(ifftshift(in)) (centred) or scale * ifft2(in)
+int ifft2_c2c(const float2* in, int n0, int n1, int centred, int crop0, int crop1,
+              double scale, int real_only, void* out, cudaStream_t st) {
+    const int rc = ifft2_size_check("ifft2", n0, n1);
+    if (rc) return rc;
+    if (crop0 <= 0 || crop0 > n0) crop0 = n0;
+    if (crop1 <= 0 || crop1 > n1) crop1 = n1;
+    return ifft2_planes(in, 1, n0, n1, centred, crop0, crop1, [&](int, double den) {
+        return CropStore{real_only ? nullptr : (float2*)out, real_only ? (float*)out : nullptr,
+                         crop1, (float)(scale / den)};
+    }, st);
 }
 
 // --------------------------------------------------------------------------
@@ -741,22 +798,24 @@ int ifft2_c2c(const float2* in, int n0, int n1, int centred, int crop0, int crop
 // sum over the mask of (model[:nf, :nt] - dspec)^2.  One launch sequence per batch of
 // curvatures, no host synchronisation.
 // --------------------------------------------------------------------------
-struct BatchShiftedRowLoad {   // row r of ifftshift(in[e]) for row = e * n0 + r (powers of two)
-    const float2* in;
-    int n0, n1;
-    __device__ __forceinline__ float2 operator()(long row, int n) const {
-        const long e = row / n0;
-        const int r = (int)((row - e * n0 + n0 / 2) & (n0 - 1));
-        const int c = (n + n1 / 2) & (n1 - 1);
-        return in[((size_t)e * n0 + r) * n1 + c];
-    }
-};
-struct ResidualStore {         // real part of out[k][c], k = k1 + R1 k2, into the sink
-    int R1;
+// fp64 partial sums per curvature; consecutive columns go to different slots so that the
+// atomics of one warp never meet on one address
+constexpr int CHISQ_SLOTS = 64;
+
+// base store of ifft2_planes: adds (scale re(v) - dspec)^2 to the partial sums where the
+// mask is set (mask == nullptr: where dspec is finite), so the model is never written
+struct ResidualSink {
+    const float* dspec;            // [nf][nt]
+    const unsigned char* mask;     // [nf][nt] or null
+    int nf, nt;
+    double* part;                  // [CHISQ_SLOTS]
     float scale;
-    ResidualSink sink;
-    __device__ __forceinline__ void operator()(int y, int k, int c, float2 v) const {
-        sink(y + R1 * k, c, v.x * scale);
+    __device__ __forceinline__ void operator()(int row, int c, float2 v) const {
+        const size_t o = (size_t)row * nt + c;
+        const float d = dspec[o];
+        if (mask ? !mask[o] : !isfinite(d)) return;
+        const double r = (double)(v.x * scale) - (double)d;
+        atomicAdd(part + (o % CHISQ_SLOTS), r * r);
     }
 };
 __global__ void chisq_finish_kernel(const double* __restrict__ part, int e0, int nb,
@@ -768,18 +827,6 @@ __global__ void chisq_finish_kernel(const double* __restrict__ part, int e0, int
     // the reference raises for these curvatures (IndexError, ARPACK error, n < 3)
     ssq[e0 + e] = (status[e0 + e] & 7) ? __longlong_as_double(0x7ff8000000000000LL) : s;
 }
-
-// thth.cu / dynspec.cu
-int thth_prep(const ThthGeom& g, const double* th_host, const double* d_etas, int neta, int ld,
-              int* d_idx, int* d_nred, int* d_status, cudaStream_t st);
-int thth_gather_source(const ThthGeom& g, const double* th_host, int neta, ThthCopy* copy,
-                       cudaStream_t st);
-int thth_gather_check(const ThthCopy& copy, cudaStream_t st);
-int thth_build_f32(const ThthGeom& g, const ThthCopy& copy, const double* d_etas, int e0, int nb,
-                   int ld, const int* d_idx, const int* d_nred, float2* d_M, cudaStream_t st);
-unsigned long long sweep_slab_bytes();
-int ifft2_any_residual(const float2* in, int n0, int n1, const ResidualSink& sink,
-                       cudaStream_t st);
 
 int chisq_sweep(const ThthGeom& g, const double* th_host, const double* d_etas, int neta,
                 const double* d_th_red, double dtau_bin, double dfd_bin, const float* dspec,
@@ -800,34 +847,28 @@ int chisq_sweep(const ThthGeom& g, const double* th_host, const double* d_etas, 
         set_error("chisq_sweep needs ascending tau / fd axes (bins must increase monotonically)");
         return SB_ERR_ARG;
     }
-    const bool pow2 = !(n0 & (n0 - 1)) && !(n1 & (n1 - 1));
-    if (pow2 ? (n0 < 8 || n1 < 8 || n0 > 65536 || n1 > 16384)
-             : (n0 < 3 || n1 < 3 || n0 > 32768 || n1 > 8192)) {
-        set_error("chisq_sweep: conjugate spectrum %d x %d outside 8..65536 x 8..16384 (powers "
-                  "of two) / 3..32768 x 3..8192 (other sizes)", n0, n1);
-        return SB_ERR_UNSUPPORTED;
-    }
+    int rc = ifft2_size_check("chisq_sweep", n0, n1);
+    if (rc) return rc;
     if (neta <= 0) return SB_OK;
-    if (!(tol > 0.0)) tol = 1e-7;
-    if (max_iter <= 0 || max_iter > SB_LANCZOS_MAXIT) max_iter = 96;
     const int ld = (g.n + 31) / 32 * 32;
-    if (max_iter > ld) max_iter = ld;
+    size_t smem;
+    rc = eigvec_setup(herm_eigvec_batch_kernel, ld, &tol, &max_iter, &smem);
+    if (rc) return rc;
     int* d_idx = (int*)workspace(1, (size_t)neta * ld * sizeof(int));
     if (!d_idx) return SB_ERR_NOMEM;
-    int rc = thth_prep(g, th_host, d_etas, neta, ld, d_idx, d_nred, d_status, st);
+    rc = thth_prep(g, th_host, d_etas, neta, ld, d_idx, d_nred, d_status, st);
     if (rc) return rc;
     ThthCopy copy;
     rc = thth_gather_source(g, th_host, neta, &copy, st);
     if (rc) return rc;
     // per curvature: matrix, Lanczos basis, eigenvector, bin sums, partial sums, counts
     // (+ the row-transformed spectrum on the radix path), all under the sweep's slab budget
+    const bool pow2 = is_pow2(n0) && is_pow2(n1);
     const size_t bins = (size_t)n0 * n1;
     const size_t mat = (size_t)ld * ld, qn = (size_t)(max_iter + 1) * ld;
     const size_t per = (mat + qn + ld + bins) * sizeof(float2) + CHISQ_SLOTS * sizeof(double) +
                        bins * sizeof(int) + (pow2 ? bins * sizeof(float2) : 0);
-    unsigned long long b = sweep_slab_bytes() / per;
-    int batch = (int)(b < 1 ? 1 : (b > 65535 ? 65535 : b));
-    if (batch > neta) batch = neta;
+    const int batch = sweep_batch(per, neta, 65535);
     unsigned char* ws = (unsigned char*)workspace(2, per * batch);
     if (!ws) return SB_ERR_NOMEM;
     float2* M = (float2*)ws;
@@ -836,24 +877,11 @@ int chisq_sweep(const ThthGeom& g, const double* th_host, const double* d_etas, 
     float2* acc = V + (size_t)ld * batch;
     double* part = (double*)(acc + bins * batch);
     int* cnt = (int*)(part + (size_t)CHISQ_SLOTS * batch);
-    float2 *B1 = nullptr, *B2 = nullptr;
-    if (pow2) {
-        B1 = (float2*)workspace(3, bins * batch * sizeof(float2));
-        B2 = (float2*)workspace(4, bins * sizeof(float2));
-        if (!B1 || !B2) return SB_ERR_NOMEM;
-    }
-    const size_t smem = sizeof(LanczosShared) + 32 * sizeof(double) +
-                        (SB_LANCZOS_MAXIT + 1) * sizeof(double2) + 2 * (size_t)ld * sizeof(float2);
-    SB_CUDA(cudaFuncSetAttribute(herm_eigvec_batch_kernel,
-                                 cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     // rev_map bins: tau[0], tau[1] - tau[0], fd[0], fd[1] - fd[0] (ththmod.py:210-215)
     const RevGeom rg{nullptr, 0, 0.0, g.tau0, dtau_bin, g.fd0, dfd_bin, n0, n1};
     int sb_ = (int)((mat + 255) / 256), fb = (int)((bins + 255) / 256);
     sb_ = sb_ > 256 ? 256 : sb_;
     fb = fb > 1024 ? 1024 : fb;
-    int R1, R2;
-    split_len(n0, &R1, &R2);
-    const float scale = (float)(1.0 / ((double)n0 * (double)n1));
     for (int e0 = 0; e0 < neta; e0 += batch) {
         const int nb = neta - e0 < batch ? neta - e0 : batch;
         rc = thth_build_f32(g, copy, d_etas, e0, nb, ld, d_idx, d_nred, M, st);
@@ -869,27 +897,11 @@ int chisq_sweep(const ThthGeom& g, const double* th_host, const double* d_etas, 
         SB_LAUNCH_CHECK();
         rev_finalise_batch_kernel<<<dim3(fb, nb), 256, 0, st>>>(rg, acc, cnt);
         SB_LAUNCH_CHECK();
-        if (pow2) {
-            // rows of every curvature in one launch, then the kept columns per curvature
-            BatchShiftedRowLoad lr{acc, n0, n1};
-            PlainRowStore<float2> rs{B1, n1};
-            SB_ROW_DISPATCH(n1, rc = (launch_row_c2c<float, N1, N2, +1>(lr, rs, (long)nb * n0, st)));
-            if (rc) return rc;
-            for (int e = 0; e < nb; ++e) {
-                StrideALoad<float2> la{B1 + bins * e, n1, R2};
-                ResidualStore cs{R1, scale,
-                                 ResidualSink{dspec, mask, nf, nt, part + (size_t)CHISQ_SLOTS * e}};
-                rc = cols_generic<float, +1>(la, B2, n1, n0, nt, cs, st);
-                if (rc) return rc;
-            }
-        } else {
-            for (int e = 0; e < nb; ++e) {
-                rc = ifft2_any_residual(acc + bins * e, n0, n1,
-                                        ResidualSink{dspec, mask, nf, nt,
-                                                     part + (size_t)CHISQ_SLOTS * e}, st);
-                if (rc) return rc;
-            }
-        }
+        rc = ifft2_planes(acc, nb, n0, n1, 1, nf, nt, [&](int e, double den) {
+            return ResidualSink{dspec, mask, nf, nt, part + (size_t)CHISQ_SLOTS * e,
+                                (float)(1.0 / den)};
+        }, st);
+        if (rc) return rc;
         chisq_finish_kernel<<<(nb + 127) / 128, 128, 0, st>>>(part, e0, nb, d_status, d_ssq);
         SB_LAUNCH_CHECK();
     }
@@ -959,7 +971,7 @@ __global__ void gs_amplitude_kernel(float2* W, const float* __restrict__ amp, lo
 }
 static int gerchberg_saxton_any(float2* W, const float* amp, const unsigned char* rowmask,
                                 int n0, int n1, int niter, cudaStream_t st) {
-    // the limits of ifft2_c2c_any, checked before the workspace is allocated
+    // the limits of ifft2_conj_any, checked before the workspace is allocated
     if (n0 < 3 || n1 < 3 || n0 > 32768 || n1 > 8192) {
         set_error("gerchberg_saxton (chirp-z): wavefield %d x %d outside 3..32768 x 3..8192",
                   n0, n1);
@@ -971,11 +983,11 @@ static int gerchberg_saxton_any(float2* W, const float* amp, const unsigned char
     int blocks = (int)((count + 255) / 256);
     if (blocks > num_sms() * 16) blocks = num_sms() * 16;
     for (int it = 0; it < niter; ++it) {
-        int rc = ifft2_c2c_any(W, n0, n1, 0, 0, 0, 1.0, 0, T, st, 1);
+        int rc = ifft2_conj_any(W, n0, n1, 1.0, T, st);
         if (rc) return rc;
         gs_rowmask_kernel<<<blocks, 256, 0, st>>>(T, rowmask, n0, n1);
         SB_LAUNCH_CHECK();
-        rc = ifft2_c2c_any(T, n0, n1, 0, 0, 0, (double)count, 0, W, st, 1);
+        rc = ifft2_conj_any(T, n0, n1, (double)count, W, st);
         if (rc) return rc;
         gs_amplitude_kernel<<<blocks, 256, 0, st>>>(W, amp, count);
         SB_LAUNCH_CHECK();
@@ -1111,7 +1123,7 @@ int conj_spectrum_c2c(const float2* in, int nf, int nt, int npad, float pad_re, 
                       const unsigned char* rowmask, float2* CS, cudaStream_t st) {
     const long NFl = (long)(npad + 1) * nf, NTl = (long)(npad + 1) * nt;
     // a complex row is one row transform of NT points (8..16384), unlike the real input's
-    // half-length rows; the chirp-z path has the limits of ifft2_c2c_any
+    // half-length rows; the chirp-z path has the limits of ifft2_conj_any
     const bool radix = is_pow2(NFl) && is_pow2(NTl) && NFl >= 8 && NTl >= 8 && NFl <= 65536 &&
                        NTl <= 16384;
     if (!radix && (NFl < 3 || NTl < 3 || NFl > 32768 || NTl > 8192)) {
@@ -1152,7 +1164,7 @@ int conj_spectrum_c2c(const float2* in, int nf, int nt, int npad, float pad_re, 
     }
     float2* T = (float2*)workspace(1, count * sizeof(float2));
     if (!T) return SB_ERR_NOMEM;
-    const int rc = ifft2_c2c_any(P, NF, NT, 0, 0, 0, (double)count, 0, T, st, 1);
+    const int rc = ifft2_conj_any(P, NF, NT, (double)count, T, st);
     if (rc) return rc;
     c2c_shift_conj_kernel<<<blocks, 256, 0, st>>>(T, NF, NT, rowmask, CS);
     SB_LAUNCH_CHECK();
@@ -1223,15 +1235,11 @@ int vlbi_retrieval(const ThthGeom& geom, const double* th_host, const float2* co
                   "exceeds the eigen solver's limit of 8192", n_dish, n, N);
         return SB_ERR_UNSUPPORTED;
     }
-    const bool pow2 = !(n0 & (n0 - 1)) && !(n1 & (n1 - 1));
-    if (pow2 ? (n0 < 8 || n1 < 8 || n0 > 65536 || n1 > 16384)
-             : (n0 < 3 || n1 < 3 || n0 > 32768 || n1 > 8192)) {
-        set_error("vlbi_retrieval: conjugate spectrum %d x %d outside 8..65536 x 8..16384 (powers "
-                  "of two) / 3..32768 x 3..8192 (other sizes)", n0, n1);
-        return SB_ERR_UNSUPPORTED;
-    }
-    if (!(tol > 0.0)) tol = 1e-7;
-    if (max_iter <= 0 || max_iter > SB_LANCZOS_MAXIT) max_iter = 96;
+    int rc = ifft2_size_check("vlbi_retrieval", n0, n1);
+    if (rc) return rc;
+    size_t smem;
+    rc = eigvec_setup(vlbi_eigvec_kernel, (int)N, &tol, &max_iter, &smem);
+    if (rc) return rc;
     const size_t bins = (size_t)n0 * n1;
     const size_t qn = (size_t)(max_iter + 1) * (N > 0 ? N : 1);
     // slot 1: eta, spectrum pointers, crop indices; slot 2: composite, Lanczos basis,
@@ -1248,12 +1256,6 @@ int vlbi_retrieval(const ThthGeom& geom, const double* th_host, const float2* co
     float2* Q = A + (size_t)N * N;
     float2* acc = Q + qn;
     int* cnt = (int*)(acc + (size_t)n_dish * bins);
-    float2 *B1 = nullptr, *B2 = nullptr;
-    if (pow2) {
-        B1 = (float2*)workspace(3, (size_t)n_dish * bins * sizeof(float2));
-        B2 = (float2*)workspace(4, bins * sizeof(float2));
-        if (!B1 || !B2) return SB_ERR_NOMEM;
-    }
     for (int b = 0; b < npairs; b += VLBI_PTRS) {
         VlbiArgs a;
         a.base = b;
@@ -1263,7 +1265,7 @@ int vlbi_retrieval(const ThthGeom& geom, const double* th_host, const float2* co
         vlbi_args_kernel<<<1, VLBI_PTRS, 0, st>>>(a, d_cs, d_eta);
         SB_LAUNCH_CHECK();
     }
-    int rc = thth_prep(g, th_host, d_eta, 1, g.n, d_idx, d_info + 2, d_info + 1, st);
+    rc = thth_prep(g, th_host, d_eta, 1, g.n, d_idx, d_info + 2, d_info + 1, st);
     if (rc) return rc;
     if (N > 0) {
         int blocks = (int)((N * N + 255) / 256);
@@ -1271,10 +1273,6 @@ int vlbi_retrieval(const ThthGeom& geom, const double* th_host, const float2* co
         vlbi_composite_kernel<<<blocks, 256, 0, st>>>(g, d_eta, d_cs, n_dish, d_idx, n, A);
         SB_LAUNCH_CHECK();
     }
-    const size_t smem = sizeof(LanczosShared) + 32 * sizeof(double) +
-                        (SB_LANCZOS_MAXIT + 1) * sizeof(double2) + 2 * (size_t)N * sizeof(float2);
-    SB_CUDA(cudaFuncSetAttribute(vlbi_eigvec_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)smem));
     vlbi_eigvec_kernel<<<1, EV_THREADS, smem, st>>>(A, n_dish, n, Q, max_iter, tol, d_w, d_v,
                                                     d_info);
     SB_LAUNCH_CHECK();
@@ -1294,29 +1292,9 @@ int vlbi_retrieval(const ThthGeom& geom, const double* th_host, const float2* co
     vlbi_finalise_kernel<<<dim3(fb, n_dish), 256, 0, st>>>(rg, acc, cnt);
     SB_LAUNCH_CHECK();
     const double scale = (double)nf * (double)nt / 4.0;
-    const size_t crop = (size_t)nf * nt;
-    if (!pow2) {
-        for (int d = 0; d < n_dish; ++d) {
-            rc = ifft2_c2c_any(acc + bins * d, n0, n1, 1, nf, nt, scale, 0, d_model + crop * d, st, 0);
-            if (rc) return rc;
-        }
-        return SB_OK;
-    }
-    // rows of every station in one launch, then the kept columns per station
-    BatchShiftedRowLoad lr{acc, n0, n1};
-    PlainRowStore<float2> rs{B1, n1};
-    SB_ROW_DISPATCH(n1, rc = (launch_row_c2c<float, N1, N2, +1>(lr, rs, (long)n_dish * n0, st)));
-    if (rc) return rc;
-    int R1, R2;
-    split_len(n0, &R1, &R2);
-    for (int d = 0; d < n_dish; ++d) {
-        StrideALoad<float2> la{B1 + bins * d, n1, R2};
-        CropStore cs{d_model + crop * d, nullptr, R1, nf, nt,
-                     (float)(scale / ((double)n0 * (double)n1))};
-        rc = cols_generic<float, +1>(la, B2, n1, n0, nt, cs, st);
-        if (rc) return rc;
-    }
-    return SB_OK;
+    return ifft2_planes(acc, n_dish, n0, n1, 1, nf, nt, [&](int d, double den) {
+        return CropStore{d_model + (size_t)nf * nt * d, nullptr, nt, (float)(scale / den)};
+    }, st);
 }
 
 // --------------------------------------------------------------------------
@@ -1324,10 +1302,6 @@ int vlbi_retrieval(const ThthGeom& geom, const double* th_host, const float2* co
 // gather, top eigenpair, asymmetry of V.  Chunks run in batches under the sweep's slab
 // budget; one launch sequence, no host synchronisation, nchunk numbers per output.
 // --------------------------------------------------------------------------
-int thth_prep_table(const ThthGeom* geoms, const double* const* th_host, const ThthGeom* d_geoms,
-                    const double* d_etas, int n, int ld, int* d_idx, int* d_nred, int* d_status,
-                    cudaStream_t st);
-
 int asymmetry_batch(const ThthGeom* geoms, const double* const* th_host, int nchunk,
                     const double* d_etas, double tol, int max_iter, double* d_asym, double* d_w,
                     int* d_status, int* d_nred, int* d_iters, float2* d_v, cudaStream_t st) {
@@ -1362,16 +1336,14 @@ int asymmetry_batch(const ThthGeom* geoms, const double* const* th_host, int nch
                   "(powers of two) / 3..32768 x 3..8192 (other sizes, full plane)", n0, n1);
         return SB_ERR_UNSUPPORTED;
     }
-    if (!(tol > 0.0)) tol = 1e-7;
-    if (max_iter <= 0 || max_iter > SB_LANCZOS_MAXIT) max_iter = 96;
     const int ld = (g0.n + 31) / 32 * 32;
-    if (max_iter > ld) max_iter = ld;
+    size_t smem;
+    int rc = eigvec_setup(herm_eigvec_batch_kernel, ld, &tol, &max_iter, &smem);
+    if (rc) return rc;
     // per chunk: matrix, Lanczos basis, eigenvector, under the sweep's slab budget
     const size_t mat = (size_t)ld * ld, qn = (size_t)(max_iter + 1) * ld;
     const size_t per = (mat + qn + ld) * sizeof(float2);
-    unsigned long long b = sweep_slab_bytes() / per;
-    int batch = (int)(b < 1 ? 1 : (b > 65535 ? 65535 : b));
-    if (batch > nchunk) batch = nchunk;
+    const int batch = sweep_batch(per, nchunk, 65535);
     // slot 1: geometry table and crop indices; slot 2: the batch's matrices, bases, vectors
     const size_t tab = ((size_t)nchunk * sizeof(ThthGeom) + 255) / 256 * 256;
     unsigned char* s1 = (unsigned char*)workspace(1, tab + (size_t)nchunk * ld * sizeof(int));
@@ -1384,13 +1356,8 @@ int asymmetry_batch(const ThthGeom* geoms, const double* const* th_host, int nch
     float2* V = Q + qn * batch;
     SB_CUDA(cudaMemcpyAsync(d_geoms, geoms, (size_t)nchunk * sizeof(ThthGeom),
                             cudaMemcpyHostToDevice, st));
-    int rc = thth_prep_table(geoms, th_host, d_geoms, d_etas, nchunk, ld, d_idx, d_nred, d_status,
-                             st);
+    rc = thth_prep_table(geoms, th_host, d_geoms, d_etas, nchunk, ld, d_idx, d_nred, d_status, st);
     if (rc) return rc;
-    const size_t smem = sizeof(LanczosShared) + 32 * sizeof(double) +
-                        (SB_LANCZOS_MAXIT + 1) * sizeof(double2) + 2 * (size_t)ld * sizeof(float2);
-    SB_CUDA(cudaFuncSetAttribute(herm_eigvec_batch_kernel,
-                                 cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int gb = (int)((mat + 255) / 256);
     gb = gb > 32 ? 32 : gb;
     for (int e0 = 0; e0 < nchunk; e0 += batch) {

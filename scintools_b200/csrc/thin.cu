@@ -356,9 +356,7 @@ int thin_sweep(const ThinGeom& t, const double* d_eta1, const double* d_eta2, in
         SB_LAUNCH_CHECK();
     }
     const size_t per = (size_t)ld1 * ld2 * sizeof(float2);
-    int batch = (int)((3ull << 30) / per);
-    if (batch < 1) batch = 1;
-    if (batch > neta) batch = neta;
+    const int batch = sweep_batch(per, neta, INT_MAX);
     float2* d_M = (float2*)workspace(2, per * batch);
     if (!d_M) return SB_ERR_NOMEM;
     constexpr int TH = 256;

@@ -698,15 +698,20 @@ __global__ void thth_map_kernel(ThthGeom g, double eta, int hermitian,
 // --------------------------------------------------------------------------
 // host drivers
 // --------------------------------------------------------------------------
-// per-launch budget of the curvature-batched work buffers: 3 GiB, or SB_SWEEP_SLAB_MB
-// (tests use it to force batching)
-unsigned long long sweep_slab_bytes() {
+// Items per launch of a batched driver: as many as per_item bytes each fit the per-launch
+// budget of the work buffers, 3 GiB or SB_SWEEP_SLAB_MB (tests use it to force batching);
+// at least 1, at most cap (the largest batch the caller's grid takes) and at most count.
+int sweep_batch(size_t per_item, int count, int cap) {
     unsigned long long slab = 3ull << 30;
     if (const char* ev = getenv("SB_SWEEP_SLAB_MB")) {
         const long mb = atol(ev);
         if (mb > 0) slab = (unsigned long long)mb << 20;
     }
-    return slab;
+    unsigned long long b = slab / per_item;
+    if (b < 1) b = 1;
+    if (b > (unsigned long long)cap) b = cap;
+    if (b > (unsigned long long)count) b = count;
+    return (int)b;
 }
 
 static bool lower_check_needed(const ThthGeom& g, const double* th_host) {
@@ -928,11 +933,8 @@ int eta_sweep(const ThthGeom& g, const double* th_host, const double* d_etas,
     ThthCopy copy;
     rc = thth_gather_source(g, th_host, neta, &copy, st);
     if (rc) return rc;
-    // batch so that the matrix slab stays <= ~3 GiB
     const size_t per = (size_t)ld * ld * sizeof(float2);
-    int batch = (int)(sweep_slab_bytes() / per);
-    if (batch < 1) batch = 1;
-    if (batch > neta) batch = neta;
+    const int batch = sweep_batch(per, neta, INT_MAX);
     float2* d_M = (float2*)workspace(2, per * batch);
     if (!d_M) return SB_ERR_NOMEM;
     // default solver for ld <= 512 (eig_half.cu): iterates on the fp16 copy written by the

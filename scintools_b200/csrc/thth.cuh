@@ -137,4 +137,19 @@ __device__ __forceinline__ float2 thth_herm_upper(const ThthGeom& g, double eta,
     return v;
 }
 
+#ifndef SB_HOST_EMU
+// host drivers of thth.cu that the other sweeps and retrieval.cu share
+int sweep_batch(size_t per_item, int count, int cap);
+int thth_prep(const ThthGeom& g, const double* th_host, const double* d_etas, int neta, int ld,
+              int* d_idx, int* d_nred, int* d_status, cudaStream_t st);
+int thth_prep_table(const ThthGeom* geoms, const double* const* th_host, const ThthGeom* d_geoms,
+                    const double* d_etas, int n, int ld, int* d_idx, int* d_nred, int* d_status,
+                    cudaStream_t st);
+int thth_gather_source(const ThthGeom& g, const double* th_host, int neta, ThthCopy* copy,
+                       cudaStream_t st);
+int thth_gather_check(const ThthCopy& copy, cudaStream_t st);
+int thth_build_f32(const ThthGeom& g, const ThthCopy& copy, const double* d_etas, int e0, int nb,
+                   int ld, const int* d_idx, const int* d_nred, float2* d_M, cudaStream_t st);
+#endif
+
 }  // namespace sb

@@ -1,7 +1,7 @@
-// CPU emulation of the any-size (chirp-z) 2-D FFT driver of csrc/dynspec.cu
-// (chirp_fft2) and its two entry points, ifft2_c2c_any and the conjugate spectrum
-// of conj_spectrum: the chirp tables and every load / store functor come from
-// csrc/fft_functors.cuh unchanged; the power-of-two FFT kernels between them
+// CPU emulation of the any-size (chirp-z) 2-D FFT driver of csrc/fft_kernels.cuh
+// (chirp_fft2) and its two uses, the inverse of retrieval.cu (ifft2_chirp) and the
+// conjugate spectrum of conj_spectrum: the chirp tables and every load / store
+// functor come from csrc/fft_functors.cuh unchanged; the power-of-two FFT kernels between them
 // (verified on the GPU by the conjugate-spectrum tests) are replaced by a plain
 // DFT, and the pass order / buffers / scales mirror the driver.  TEST INFRASTRUCTURE.
 #define SB_HOST_EMU 1
@@ -108,9 +108,9 @@ extern "C" int emu_ifft2_any(const float* in_, int n0, int n1, int centred, int 
     chirp_fft2(ChirpRowLoadC{in, n0, n1, centred, conj_in, nullptr}, n0, n1, n0, crop1,
                [&](int R1, const float2* wF, int MF) {
                    const double den = (double)MF * (double)n0 * (double)n1;
-                   return ChirpCropStore{real_only ? nullptr : reinterpret_cast<float2*>(out),
-                                         real_only ? out : nullptr, R1, crop0, crop1, wF,
-                                         (float)(scale / den)};
+                   const CropStore base{real_only ? nullptr : reinterpret_cast<float2*>(out),
+                                        real_only ? out : nullptr, crop1, (float)(scale / den)};
+                   return ChirpStore<CropStore>{R1, crop0, crop1, wF, base};
                });
     return 0;
 }

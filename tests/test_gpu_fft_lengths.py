@@ -103,7 +103,7 @@ def templates(case):
         r1, r2 = split_len(R)
         out.update({("col", tag, prec, R, load), ("tile", prec, r1), ("tile", prec, r2)})
 
-    def chirp(tag, n0, n1):       # chirp_fft2 (conj_spectrum / ifft2_c2c_any)
+    def chirp(tag, n0, n1):       # chirp_fft2 (conj_spectrum / ifft2_chirp)
         mt, mf = next_pow2(2 * n1 - 1), next_pow2(2 * n0 - 1)
         out.add(("row", tag, "c2c", "f32", mt))
         cols(tag, "f32", mf, "plain")

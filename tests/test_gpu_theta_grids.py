@@ -434,6 +434,27 @@ def test_thin(sb, data, case):
 
 
 @pytest.mark.gpu
+def test_thin_small_slab_bit_identical(sb, data, monkeypatch):
+    """120 pairs on grids padded to 64 x 64 (32 KiB per matrix): SB_SWEEP_SLAB_MB=1 (32
+    pairs per launch) gives the bits of the default single launch."""
+    th = sb.ththmod
+    etas = np.linspace(0.012, 0.03, 120)
+
+    def run():
+        sv, info = th.thin_sweep(data["cs"], data["tau"], data["fd"], etas, grid(63), grid(50),
+                                 0.0, etasArclet=etas[::-1], return_info=True)
+        return [sv] + [info[k] for k in ("status", "n1", "n2", "iters")]
+
+    whole = run()
+    assert np.isfinite(whole[0]).all() and (whole[1] == 0).any()
+    monkeypatch.setenv("SB_SWEEP_SLAB_MB", "1")
+    sliced = run()
+    assert np.array_equal(whole[0].view(np.uint64), sliced[0].view(np.uint64))
+    for a, b in zip(whole[1:], sliced[1:]):
+        assert np.array_equal(a, b)
+
+
+@pytest.mark.gpu
 @pytest.mark.parametrize("n1,n2", [(4097, 33), (33, 4097)])
 def test_thin_limit_refused_before_any_launch(sb, data, n1, n2):
     """4097 on either axis: sb_thin_sweep refuses, naming 4096, before any launch (the

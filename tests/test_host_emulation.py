@@ -58,14 +58,18 @@ def test_scale_dyn_kernels_on_host(golden_dir, flip):
     assert np.abs(out - ref).max() < 1e-5 * np.abs(ref).max()
 
 
+# ifft2 crops down to one row / one column and the smallest chirp-z axis (3 points) check
+# where the chirp store adapter drops what lies outside the kept rows x columns
 CHIRP_CASES = [("ifft2", (12, 10, 0, 0)), ("ifft2", (9, 20, 5, 7)), ("ifft2", (16, 15, 16, 4)),
-               ("cs", (6, 5, 1, 0)), ("cs", (5, 12, 0, 1)), ("cs", (7, 9, 2, 1))]
+               ("ifft2", (7, 3, 1, 0)), ("ifft2", (3, 17, 0, 1)), ("ifft2", (11, 11, 1, 1)),
+               ("ifft2", (20, 9, 19, 8)), ("cs", (6, 5, 1, 0)), ("cs", (5, 12, 0, 1)),
+               ("cs", (7, 9, 2, 1)), ("cs", (3, 4, 1, 1)), ("cs", (9, 3, 0, 0))]
 
 
 @pytest.mark.parametrize("entry,shape", CHIRP_CASES,
                          ids=[e + "-" + "-".join(map(str, s)) for e, s in CHIRP_CASES])
 def test_chirp_fft2_functors_on_host(entry, shape):
-    """The chirp-z any-size 2-D FFT (dynspec.cu::chirp_fft2): tables and load /
+    """The chirp-z any-size 2-D FFT (fft_kernels.cuh::chirp_fft2): tables and load /
     store functors of csrc/fft_functors.cuh around a reference DFT reproduce
       ifft2: numpy's ifft2(ifftshift(x)) (and ifft2(conj x) for the
              Gerchberg-Saxton forward step), crop and scale included
