@@ -22,6 +22,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "drivers.cuh"
 
 namespace sb {
 
@@ -241,7 +242,7 @@ int acf_model(const sb_acf_model* m, double* acf, double* efield, cudaStream_t s
     const size_t nb = plan.blocks.size(), nr = plan.range.size();
     const size_t bytes = (size_t)m->n2 * m->n2 * sizeof(double) + nb * AM_TS * sizeof(double2) +
                          nb * sizeof(AmBlock) + nr * sizeof(int2) + 4 * 16;
-    char* w = (char*)workspace(3, bytes);
+    char* w = (char*)workspace(WS_PLANE0, bytes);
     if (!w) return SB_ERR_NOMEM;
     auto take = [&](size_t b) { char* p = w; w += (b + 15) & ~size_t(15); return p; };
     double* g2 = (double*)take((size_t)m->n2 * m->n2 * sizeof(double));

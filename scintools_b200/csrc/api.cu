@@ -6,13 +6,13 @@
 
 #include "../../include/scint_b200.h"
 #include "common.cuh"
-#include "thth.cuh"
+#include "drivers.cuh"
 
 namespace sb {
 
 static thread_local char g_err[512] = "";
-static void* g_ws[9] = {nullptr};
-static size_t g_ws_bytes[9] = {0};
+static void* g_ws[WS_COUNT] = {nullptr};
+static size_t g_ws_bytes[WS_COUNT] = {0};
 static int g_sms = 132;
 
 void set_error(const char* fmt, ...) {
@@ -56,8 +56,8 @@ void prof_end(int id, cudaStream_t st) {
     g_prof_pending.push_back({id, g_prof_open[id], b});
 }
 
-void* workspace(int slot, size_t bytes) {
-    if (slot < 0 || slot >= 9) return nullptr;
+void* workspace(WsSlot slot, size_t bytes) {
+    if (slot < 0 || slot >= WS_COUNT) return nullptr;
     if (bytes <= g_ws_bytes[slot] && g_ws[slot]) return g_ws[slot];
     if (g_ws[slot]) {
         cudaDeviceSynchronize();
@@ -81,42 +81,12 @@ void* workspace(int slot, size_t bytes) {
 
 void workspace_release() {
     cudaDeviceSynchronize();
-    for (int i = 0; i < 9; ++i) {
+    for (int i = 0; i < WS_COUNT; ++i) {
         if (g_ws[i]) cudaFree(g_ws[i]);
         g_ws[i] = nullptr;
         g_ws_bytes[i] = 0;
     }
 }
-
-int eta_sweep(const ThthGeom& g, const double* th_host, const double* d_etas,
-              int neta, double tol, int max_iter, double* d_eigs,
-              int* d_status, int* d_nred, int* d_iters, cudaStream_t st);
-int thth_map(const ThthGeom& g, double eta, int hermitian, float2* d_out,
-             int* d_tau_inv, int* d_fd_inv, unsigned char* d_pnts,
-             unsigned char* d_th_pnts, int* d_err, cudaStream_t st);
-
-int sspec(const float* dyn, int nf, int nt, const float* wt, const float* wf,
-          double swt, double swf, int prewhite, int halve, int db,
-          const float* pd1, const float* pd2, float* sec, cudaStream_t st,
-          int noshift = 0);
-int conj_spectrum(const float* dyn, int nf, int nt, int npad, float pad_value,
-                  const unsigned char* rowmask, int half, long pitch, int ncols_keep,
-                  float2* CS, cudaStream_t st);
-int acf(const float* dyn, int nf, int nt, int subtract_mean, int normalise,
-        float* out, cudaStream_t st);
-int acf_sspec(const float* dyn, int nf, int nt, const float* wt, const float* wf,
-              double swt, double swf, int normalise, float* out, cudaStream_t st);
-void twiddle_release();
-struct SimParams {
-    int nx, ny;
-    double dx, dy, alpha, ar, psi, inner, consp;
-};
-int sim_weights(const SimParams& p, double* w, cudaStream_t st);
-int sim_screen(int nx, int ny, const double* w, const double* n1, const double* n2,
-               unsigned long long seed, double* xyp, cudaStream_t st);
-int sim_intensity(int nx, int ny, int nf, const double* xyp, const double* scales_host,
-                  double ffconx, double ffcony, float2* spe_t, float* xyi,
-                  cudaStream_t st);
 
 template <typename A, typename B>
 __global__ void convert_kernel(const A* __restrict__ a, B* __restrict__ b, long long n) {
@@ -124,92 +94,6 @@ __global__ void convert_kernel(const A* __restrict__ a, B* __restrict__ b, long 
          i += (long long)gridDim.x * blockDim.x)
         b[i] = (B)a[i];
 }
-
-struct ThinGeom {
-    ThthGeom g;
-    const double* th2;
-    int n2;
-    double tau_max;
-    double center_cut;
-    int power;
-};
-int thin_sweep(const ThinGeom& t, const double* d_eta1, const double* d_eta2, int neta,
-               double tol, int max_iter, double* d_sv, int* d_status, int* d_n1, int* d_n2,
-               int* d_iters, cudaStream_t st);
-int thin_map(const ThinGeom& t, double e1, double e2, float2* d_out, int* d_err,
-             cudaStream_t st);
-
-int rev_map(const float2* thth, int n, const double* th_dev, double eta, double tau0,
-            double dtau, int ntau, double fd0, double dfd, int nfd, int hermitian,
-            float2* recov, cudaStream_t st);
-int herm_eigvec(const float2* A, int n, int ld, double tol, int max_iter, double* w_dev,
-                float2* V_dev, int* info_dev, cudaStream_t st);
-int ifft2_c2c(const float2* in, int n0, int n1, int centred, int crop0, int crop1,
-              double scale, int real_only, void* out, cudaStream_t st);
-int chisq_sweep(const ThthGeom& g, const double* th_host, const double* d_etas, int neta,
-                const double* d_th_red, double dtau_bin, double dfd_bin, const float* dspec,
-                const unsigned char* mask, int nf, int nt, double tol, int max_iter,
-                double* d_ssq, double* d_w, int* d_status, int* d_nred, int* d_iters,
-                cudaStream_t st);
-int conj_spectrum_c2c(const float2* in, int nf, int nt, int npad, float pad_re, float pad_im,
-                      const unsigned char* rowmask, float2* CS, cudaStream_t st);
-int vlbi_retrieval(const ThthGeom& g, const double* th_host, const float2* const* cs_host,
-                   int n_dish, double eta, const double* d_th_red, double dtau_bin,
-                   double dfd_bin, int nf, int nt, double tol, int max_iter, float2* d_model,
-                   double* d_w, float2* d_v, int* d_info, cudaStream_t st);
-int asymmetry_batch(const ThthGeom* geoms, const double* const* th_host, int nchunk,
-                    const double* d_etas, double tol, int max_iter, double* d_asym, double* d_w,
-                    int* d_status, int* d_nred, int* d_iters, float2* d_v, cudaStream_t st);
-
-int mosaic_build(const float2* chunks, int ncf, int nct, int cwf, int cwt, const double* phi,
-                 const double* amp, float2* W, cudaStream_t st);
-int mosaic_rot(const float2* chunks, int ncf, int nct, int cwf, int cwt, const double* phi,
-               const float2* W, double* power, double* der, cudaStream_t st);
-int mosaic_overlap(const float2* chunks, int ncf, int nct, int cwf, int cwt, double* C,
-                   cudaStream_t st);
-int mosaic_fit(const float2* chunks, int ncf, int nct, int cwf, int cwt, const double* phi,
-               const double* amp, const float2* W, const float* dspec, const float* noise,
-               double* fit, double* grad, cudaStream_t st);
-int mosaic_hess(const float2* chunks, int ncf, int nct, int cwf, int cwt, const double* phi,
-                const double* amp, const float2* W, const float* dspec, const float* noise,
-                long long* rows, long long* cols, double* vals, cudaStream_t st);
-
-int svd_topk(const float* A, int nf, int nt, int k, double* Y, double* s_host, double* res_host,
-             double* gap_host, int* info_host, cudaStream_t st);
-int svd_apply(const float* A, int nf, int nt, int k, const double* Y, float* out, float* model,
-              cudaStream_t st);
-int bandpass_rows(const float* A, int nf, int nt, int zero_as_nan, double* mean, cudaStream_t st);
-int bandpass_cols(const float* A, int nf, int nt, int zero_as_nan, const double* rowdiv,
-                  double* mean, cudaStream_t st);
-int bandpass_divide(const float* A, int nf, int nt, int zero_as_nan, const double* rowdiv,
-                    const double* coldiv, float* out, cudaStream_t st);
-
-int slow_ft(const float* x, int nt, int nf, const double* s, float2* out, cudaStream_t st);
-
-int inpaint_biharmonic(const double* img, int nf, int nt, const int* pix, int n,
-                       const double* tables, const unsigned char* rcls, int nrc,
-                       const unsigned char* ccls, int ncc, double lo, double hi, double tol,
-                       int maxit, double* out, int* info_host, double* resid_host,
-                       cudaStream_t st);
-int medfilt_masked(const double* img, int nf, int nt, const int* pix, int n, int kh, int kw,
-                   double nan_value, double* out, cudaStream_t st);
-int scint_fit_1d(const sb_scint_fit* fits, int nfit, double* out, int* info, cudaStream_t st);
-int scint_fit_2d(const sb_scint_fit* fits, int nfit, double* out, int* info, cudaStream_t st);
-int acf_model(const sb_acf_model* m, double* acf, double* efield, cudaStream_t st);
-
-int gerchberg_saxton(float2* W, const float* amp, const unsigned char* rowmask, int n0, int n1,
-                     int niter, cudaStream_t st);
-
-int conj_spectrum_bound(const float* dyn, int nf, int nt, int npad, float pad_value, float* out,
-                        cudaStream_t st);
-int norm_sspec_rows(const float* sspec, int nr, int nc, const double* fdop, const double* tdel,
-                    double eta, double maxnormfac, const double* fdopnew, int nq, float* out,
-                    double* power, cudaStream_t st);
-int norm_sspec_avg(const float* norm, int nr, int nq, const double* weights, double* avg,
-                   cudaStream_t st);
-int scale_dyn_lambda(const float* dyn, int nf, int nt, int flip, const float* a,
-                     const float* cp, const float* inv, const float* g, float p0, float pn,
-                     const int* idx, const float4* W, int nlam, float* out, cudaStream_t st);
 
 static int to_geom(const sb_thth_geom* in, ThthGeom* g) {
     SB_ARG(in != nullptr);

@@ -2,6 +2,7 @@
 #pragma once
 #ifndef SB_HOST_EMU            // tests/host_emu compiles the device code for the CPU
 #include <cuda_runtime.h>
+#include <stddef.h>
 #include <stdint.h>
 #include <stdio.h>
 
@@ -12,10 +13,73 @@ namespace sb {
 void set_error(const char* fmt, ...);
 const char* last_error();
 
-// grow-only per-process device workspace (one CUDA context per process,
-// one caller thread at a time; see include/scint_b200.h)
-void* workspace(int slot, size_t bytes);
+// Grow-only per-process device workspace (one CUDA context per process, one caller thread
+// at a time; see include/scint_b200.h).  A request larger than a slot's size frees the slot
+// and allocates it again, so a pointer taken earlier from that slot dangles: a driver must
+// not hold a buffer in a slot that a driver it calls takes.
+//
+//   slot          takers
+//   WS_SCALARS    the ScalarBlock below
+//   WS_INDEX      index tables of eta_sweep, thin_sweep, chisq_sweep; rev_map's bin counts;
+//                 vlbi_retrieval's and asymmetry_batch's per-call arrays; the chirp-z result
+//                 of conj_spectrum_c2c
+//   WS_BATCH      the batch slab of eta_sweep, thin_sweep, chisq_sweep, vlbi_retrieval,
+//                 asymmetry_batch; herm_eigvec's basis; the padded chunk of
+//                 conj_spectrum_c2c; gerchberg_saxton; svd_topk
+//   WS_PLANE0..4  the FFT engine: chirp_fft2 takes all five (through ifft2_chirp,
+//                 ifft2_planes, ifft2_conj_any and the chirp-z conj_spectrum); the radix
+//                 2-D transforms of sspec, acf, acf_sspec, conj_spectrum, ifft2_planes,
+//                 conj_spectrum_c2c and gerchberg_saxton take PLANE0..2.  Drivers that
+//                 call neither use them too: sim_screen, sim_intensity, slow_ft,
+//                 inpaint_biharmonic, scint_fit, acf_model, scale_dyn_lambda; eta_sweep
+//                 keeps its fp16 copy in PLANE3, eig_half_launch its Lanczos basis in PLANE4
+//   WS_TABLE      the column table and compact copy of thth_gather_source; the partial
+//                 sums of svd_topk, bandpass_cols and the mosaic tiles
+//
+// Nesting rule: a driver that calls the FFT engine keeps its own buffers in WS_SCALARS,
+// WS_INDEX, WS_BATCH and WS_TABLE only (chisq_sweep, vlbi_retrieval, conj_spectrum_c2c,
+// gerchberg_saxton, conj_spectrum).  Likewise acf_sspec holds PLANE2 across sspec, and
+// eta_sweep holds PLANE3 across eig_half_launch.
+enum WsSlot {
+    WS_SCALARS = 0,
+    WS_INDEX = 1,
+    WS_BATCH = 2,
+    WS_PLANE0 = 3,
+    WS_PLANE1 = 4,
+    WS_PLANE2 = 5,
+    WS_PLANE3 = 6,
+    WS_PLANE4 = 7,
+    WS_TABLE = 8,
+    WS_COUNT = 9
+};
+void* workspace(WsSlot slot, size_t bytes);
 void workspace_release();
+
+// The device scalars in WS_SCALARS.  Kernels take plain pointers to the fields.
+struct ScalarBlock {
+    union {
+        double stats[8];      // stats_pass (dynspec.cu): sums [0..3], means [4..6], ACF power [7]
+        double c2c_sum[2];    // conj_spectrum_c2c: sum of the chunk's re, im
+    };
+    float acf_factor;         // acf: the factor of the final row pass
+    float pad0[15];
+    unsigned sweep_scale;     // eta_sweep: scale of the fp16 copy (the bits of a float)
+    unsigned pad1[15];
+    double l1;                // conj_spectrum_bound: L1 norm accumulator
+    double pad2[7];
+    double acf_part[32];      // acf: partial power sums
+};
+static_assert(offsetof(ScalarBlock, stats) == 0, "ScalarBlock layout");
+static_assert(offsetof(ScalarBlock, c2c_sum) == 0, "ScalarBlock layout");
+static_assert(offsetof(ScalarBlock, acf_factor) == 8 * sizeof(double), "ScalarBlock layout");
+static_assert(offsetof(ScalarBlock, sweep_scale) == 16 * sizeof(double), "ScalarBlock layout");
+static_assert(offsetof(ScalarBlock, l1) == 24 * sizeof(double), "ScalarBlock layout");
+static_assert(offsetof(ScalarBlock, acf_part) == 32 * sizeof(double), "ScalarBlock layout");
+static_assert(sizeof(ScalarBlock) == 64 * sizeof(double), "ScalarBlock fills its allocation");
+
+inline ScalarBlock* scalar_block() {
+    return (ScalarBlock*)workspace(WS_SCALARS, sizeof(ScalarBlock));
+}
 int num_sms();
 
 // optional per-kernel timing with CUDA events on the launching stream

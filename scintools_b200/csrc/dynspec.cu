@@ -12,6 +12,7 @@
 #include <map>
 #include <stdlib.h>
 
+#include "drivers.cuh"
 #include "fft_kernels.cuh"
 
 namespace sb {
@@ -344,18 +345,21 @@ struct AcfRowStore {
     }
 };
 
-// stats[7] = full-plane power sum (32 slots at stats[32..63]); the factor the row pass
-// multiplies with, as a float at stats[8]: 1 / sum (normalise) or the raw ifft2 scale
+// stats[7] = full-plane power sum (of the 32 partials acf_part); acf_factor = the factor the
+// row pass multiplies with: 1 / sum (normalise) or the raw ifft2 scale
 __global__ void acf_scale_kernel(double* stats, int normalise, double raw_scale) {
-    double v = stats[32 + threadIdx.x];
+    ScalarBlock* sc = reinterpret_cast<ScalarBlock*>(stats);
+    constexpr unsigned part = offsetof(ScalarBlock, acf_part) / sizeof(double);
+    double v = stats[part + threadIdx.x];
     v = warp_sum(v);
     if (threadIdx.x == 0) {
-        stats[7] = v;
-        *reinterpret_cast<float*>(stats + 8) = (float)(normalise ? 1.0 / v : raw_scale);
+        sc->stats[7] = v;
+        sc->acf_factor = (float)(normalise ? 1.0 / v : raw_scale);
     }
 }
 
 // ------------------------------------------------------------ host drivers
+// clears the whole ScalarBlock at stats, then fills stats[0..7]
 int stats_pass(const float* dyn, int nf, int nt, const float* wt, const float* wf,
                double swt, double swf, double* stats, cudaStream_t st);
 static long half_pitch(long NT) { return ((NT / 2 + 1) + 15) & ~15L; }
@@ -465,7 +469,7 @@ static int cols_forward(const float2* H, float2* A, long pitch, int NF, int live
 
 int stats_pass(const float* dyn, int nf, int nt, const float* wt, const float* wf,
                double swt, double swf, double* stats, cudaStream_t st) {
-    SB_CUDA(cudaMemsetAsync(stats, 0, 64 * sizeof(double), st));
+    SB_CUDA(cudaMemsetAsync(stats, 0, sizeof(ScalarBlock), st));
     const bool vec = nt % 4 == 0 && ((uintptr_t)dyn & 15) == 0 && (!wt || ((uintptr_t)wt & 15) == 0);
     if (vec) dyn_stats_kernel<true><<<num_sms() * 8, 256, 0, st>>>(dyn, nf, nt, wt, wf, stats);
     else dyn_stats_kernel<false><<<num_sms() * 8, 256, 0, st>>>(dyn, nf, nt, wt, wf, stats);
@@ -533,8 +537,8 @@ static int sspec_prewhite_f64(const float* dyn, int nf, int nt, const float* wt,
     }
     const long pitch = half_pitch(NT);
     const int live = nf - 1;
-    double2* H = (double2*)workspace(3, (size_t)live * pitch * sizeof(double2));
-    double2* A = (double2*)workspace(4, (size_t)NF * pitch * sizeof(double2));
+    double2* H = (double2*)workspace(WS_PLANE0, (size_t)live * pitch * sizeof(double2));
+    double2* A = (double2*)workspace(WS_PLANE1, (size_t)NF * pitch * sizeof(double2));
     if (!H || !A) return SB_ERR_NOMEM;
     DynRowLoadD ld{dyn, nf, nt, wt, wf, stats};
     PlainRowStore<double2> hs{H, pitch};
@@ -553,7 +557,7 @@ static int sspec_prewhite_f64(const float* dyn, int nf, int nt, const float* wt,
 int sspec(const float* dyn, int nf, int nt, const float* wt, const float* wf,
           double swt, double swf, int prewhite, int halve, int db,
           const float* pd1, const float* pd2, float* sec, cudaStream_t st,
-          int noshift = 0) {
+          int noshift) {
     ProfScope prof(PROF_SSPEC, st);
     const int NF = 2 * next_pow2(nf), NT = 2 * next_pow2(nt);  // 2^(ceil(log2 n)+1)
     if (NT / 2 < 8 || NT / 2 > 16384 || NF > 65536 || NF < 4) {
@@ -562,11 +566,13 @@ int sspec(const float* dyn, int nf, int nt, const float* wt, const float* wf,
         return SB_ERR_UNSUPPORTED;
     }
     const long pitch = half_pitch(NT);
-    double* stats = (double*)workspace(0, 64 * sizeof(double));
+    ScalarBlock* sc = scalar_block();
+    if (!sc) return SB_ERR_NOMEM;
+    double* stats = sc->stats;
     const int live = prewhite ? nf - 1 : nf;
-    float2* H = (float2*)workspace(3, (size_t)live * pitch * sizeof(float2));
-    float2* A = (float2*)workspace(4, (size_t)NF * pitch * sizeof(float2));
-    if (!stats || !H || !A) return SB_ERR_NOMEM;
+    float2* H = (float2*)workspace(WS_PLANE0, (size_t)live * pitch * sizeof(float2));
+    float2* A = (float2*)workspace(WS_PLANE1, (size_t)NF * pitch * sizeof(float2));
+    if (!H || !A) return SB_ERR_NOMEM;
     int rc = stats_pass(dyn, nf, nt, wt, wf, swt, swf, stats, st);
     if (rc) return rc;
     if (prewhite) return sspec_prewhite_f64(dyn, nf, nt, wt, wf, stats, db, sec, NF, NT, st);
@@ -605,14 +611,15 @@ __global__ void dyn_l1_final_kernel(const double* acc, const double* stats, int 
 // transformed (dyn - c on the live pixels) + the DC correction |c| NF NT
 int conj_spectrum_bound(const float* dyn, int nf, int nt, int npad, float pad_value, float* out,
                         cudaStream_t st) {
-    double* stats = (double*)workspace(0, 64 * sizeof(double));
-    if (!stats) return SB_ERR_NOMEM;
+    ScalarBlock* sc = scalar_block();
+    if (!sc) return SB_ERR_NOMEM;
+    double* stats = sc->stats;
     const bool dev_mean = pad_value != pad_value;
     if (dev_mean) {
         int rc = stats_pass(dyn, nf, nt, nullptr, nullptr, 0, 0, stats, st);
         if (rc) return rc;
     }
-    double* acc = stats + 24;
+    double* acc = &sc->l1;
     SB_CUDA(cudaMemsetAsync(acc, 0, sizeof(double), st));
     dyn_l1_kernel<<<num_sms() * 4, 256, 0, st>>>(dyn, (long)nf * nt, stats, dev_mean ? 1 : 0,
                                                  dev_mean ? 0.f : pad_value, acc);
@@ -671,8 +678,9 @@ int conj_spectrum(const float* dyn, int nf, int nt, int npad, float pad_value,
         }
         double* bstats = nullptr;
         if (pad_value != pad_value) {
-            bstats = (double*)workspace(0, 64 * sizeof(double));
-            if (!bstats) return SB_ERR_NOMEM;
+            ScalarBlock* sc = scalar_block();
+            if (!sc) return SB_ERR_NOMEM;
+            bstats = sc->stats;
             int rc0 = stats_pass(dyn, nf, nt, nullptr, nullptr, 0, 0, bstats, st);
             if (rc0) return rc0;
             pad_value = 0.f;
@@ -691,16 +699,17 @@ int conj_spectrum(const float* dyn, int nf, int nt, int npad, float pad_value,
     }
     const int NF = (int)NFl, NT = (int)NTl;
     const long pitch = half_pitch(NT);
-    float2* H = (float2*)workspace(3, (size_t)nf * pitch * sizeof(float2));
-    float2* A = (float2*)workspace(4, (size_t)NF * pitch * sizeof(float2));
+    float2* H = (float2*)workspace(WS_PLANE0, (size_t)nf * pitch * sizeof(float2));
+    float2* A = (float2*)workspace(WS_PLANE1, (size_t)NF * pitch * sizeof(float2));
     if (!H || !A) return SB_ERR_NOMEM;
     // pad_value = NaN: pad with the mean of the chunk (ththmod.py:781), which
     // is then computed on the device instead of a host pass over the data
     const bool dev_mean = pad_value != pad_value;
     double* stats = nullptr;
     if (dev_mean) {
-        stats = (double*)workspace(0, 64 * sizeof(double));
-        if (!stats) return SB_ERR_NOMEM;
+        ScalarBlock* sc = scalar_block();
+        if (!sc) return SB_ERR_NOMEM;
+        stats = sc->stats;
         int rc0 = stats_pass(dyn, nf, nt, nullptr, nullptr, 0, 0, stats, st);
         if (rc0) return rc0;
         pad_value = 0.f;
@@ -733,11 +742,13 @@ int acf(const float* dyn, int nf, int nt, int subtract_mean, int normalise,
         return SB_ERR_UNSUPPORTED;
     }
     const long pitch = half_pitch(PT);
-    double* stats = (double*)workspace(0, 64 * sizeof(double));
-    float2* H = (float2*)workspace(3, (size_t)nf * pitch * sizeof(float2));
-    float2* A = (float2*)workspace(4, (size_t)PF * pitch * sizeof(float2));
-    float2* G = (float2*)workspace(5, (size_t)PF * pitch * sizeof(float2));
-    if (!stats || !H || !A || !G) return SB_ERR_NOMEM;
+    ScalarBlock* sc = scalar_block();
+    if (!sc) return SB_ERR_NOMEM;
+    double* stats = sc->stats;
+    float2* H = (float2*)workspace(WS_PLANE0, (size_t)nf * pitch * sizeof(float2));
+    float2* A = (float2*)workspace(WS_PLANE1, (size_t)PF * pitch * sizeof(float2));
+    float2* G = (float2*)workspace(WS_PLANE2, (size_t)PF * pitch * sizeof(float2));
+    if (!H || !A || !G) return SB_ERR_NOMEM;
     int rc = stats_pass(dyn, nf, nt, nullptr, nullptr, 0, 0, stats, st);
     if (rc) return rc;
     DynRowLoad ld{dyn, nf, nt, nullptr, nullptr, stats, subtract_mean ? 1 : 2, 0, 0.f};
@@ -771,7 +782,7 @@ int acf(const float* dyn, int nf, int nt, int subtract_mean, int normalise,
             auto kern = acf_mid_kernel<LL, 32>;
             const size_t smem = (size_t)(LL * 32 + 2 * LL) * sizeof(float2);
             SB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            kern<<<grid, 256, smem, st>>>(A, G, pitch, R1, ncols, PT, twf, twi, wRi, stats + 32);
+            kern<<<grid, 256, smem, st>>>(A, G, pitch, R1, ncols, PT, twf, twi, wRi, sc->acf_part);
         });
         SB_LAUNCH_CHECK();
         acf_scale_kernel<<<1, 32, 0, st>>>(stats, normalise, 1.0 / ((double)PF * (double)PT));
@@ -791,7 +802,7 @@ int acf(const float* dyn, int nf, int nt, int subtract_mean, int normalise,
     }
     // rows: half spectrum -> real, crop to lags [-nf, nf) x [-nt, nt)
     AcfRowLoad rl{A, pitch, nf, PF};
-    AcfRowStore rs{out, nt, PT, reinterpret_cast<const float*>(stats + 8)};
+    AcfRowStore rs{out, nt, PT, &sc->acf_factor};
     const int N = PT / 2;
     SB_ROW_DISPATCH(N, return (launch_row_c2r<float, N1, N2>(rl, rs, 2L * nf, st)));
     return SB_OK;
@@ -818,7 +829,7 @@ struct RealShiftStore {
 int acf_sspec(const float* dyn, int nf, int nt, const float* wt, const float* wf,
               double swt, double swf, int normalise, float* out, cudaStream_t st) {
     const int NF = 2 * next_pow2(nf), NT = 2 * next_pow2(nt);
-    float* P = (float*)workspace(5, (size_t)NF * NT * sizeof(float));
+    float* P = (float*)workspace(WS_PLANE2, (size_t)NF * NT * sizeof(float));
     if (!P) return SB_ERR_NOMEM;
     int rc = sspec(dyn, nf, nt, wt, wf, swt, swf, 0, 0, 0, nullptr, nullptr, P, st, 1);
     if (rc) return rc;
@@ -828,10 +839,12 @@ int acf_sspec(const float* dyn, int nf, int nt, const float* wt, const float* wf
         return SB_ERR_UNSUPPORTED;
     }
     const long pitch = half_pitch(NT);
-    double* stats = (double*)workspace(0, 64 * sizeof(double));
-    float2* H = (float2*)workspace(3, (size_t)NF * pitch * sizeof(float2));
-    float2* A = (float2*)workspace(4, (size_t)NF * pitch * sizeof(float2));
-    if (!stats || !H || !A) return SB_ERR_NOMEM;
+    ScalarBlock* sc = scalar_block();
+    if (!sc) return SB_ERR_NOMEM;
+    double* stats = sc->stats;
+    float2* H = (float2*)workspace(WS_PLANE0, (size_t)NF * pitch * sizeof(float2));
+    float2* A = (float2*)workspace(WS_PLANE1, (size_t)NF * pitch * sizeof(float2));
+    if (!H || !A) return SB_ERR_NOMEM;
     rc = stats_pass(P, NF, NT, nullptr, nullptr, 0, 0, stats, st);
     if (rc) return rc;
     DynRowLoad ld{P, NF, NT, nullptr, nullptr, nullptr, 2, 0, 0.f};

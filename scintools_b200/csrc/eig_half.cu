@@ -31,6 +31,7 @@
 #include <math.h>
 #include <stdlib.h>
 
+#include "drivers.cuh"
 #include "lanczos.cuh"
 #include "tma.cuh"
 
@@ -719,11 +720,10 @@ thth_eig_half_kernel(const float2* __restrict__ Mbase, const unsigned* __restric
 }
 
 #ifndef SB_HOST_EMU
-// d_Mb: the scaled fp16 copy of d_M written by thth_build_kernel<2>.
 int eig_half_launch(const float2* d_M, const unsigned* d_Mb, int ld, const int* d_nred, int e0,
                     int nb, double* d_eigs, int* d_status, int* d_iters, double tol, double etol,
                     int max_iter, cudaStream_t st) {
-    float2* d_basis = (float2*)workspace(7, (size_t)nb * EB_SLOTS * ld * sizeof(float2));
+    float2* d_basis = (float2*)workspace(WS_PLANE4, (size_t)nb * EB_SLOTS * ld * sizeof(float2));
     if (!d_basis) return SB_ERR_NOMEM;
     double rtol_r = 1e-3;
     if (const char* ev = getenv("SB_EIG_RTOL_R")) rtol_r = atof(ev);

@@ -450,11 +450,11 @@ static inline int chirp_fft2(RowLoad ld, int n0, int n1, int live, int ncols, Ma
         return SB_ERR_UNSUPPORTED;
     }
     const long pt = ((long)n1 + 15) & ~15L;
-    float2* tabs = (float2*)workspace(6, (size_t)(n1 + 3L * MT + n0 + 3L * MF + 64) * sizeof(float2));
-    float2* R1buf = (float2*)workspace(3, (size_t)live * MT * sizeof(float2));
-    float2* Ybuf = (float2*)workspace(4, (size_t)live * pt * sizeof(float2));
-    float2* C0 = (float2*)workspace(5, (size_t)MF * pt * sizeof(float2));
-    float2* C1 = (float2*)workspace(7, (size_t)MF * pt * sizeof(float2));
+    float2* tabs = (float2*)workspace(WS_PLANE3, (size_t)(n1 + 3L * MT + n0 + 3L * MF + 64) * sizeof(float2));
+    float2* R1buf = (float2*)workspace(WS_PLANE0, (size_t)live * MT * sizeof(float2));
+    float2* Ybuf = (float2*)workspace(WS_PLANE1, (size_t)live * pt * sizeof(float2));
+    float2* C0 = (float2*)workspace(WS_PLANE2, (size_t)MF * pt * sizeof(float2));
+    float2* C1 = (float2*)workspace(WS_PLANE4, (size_t)MF * pt * sizeof(float2));
     if (!tabs || !R1buf || !Ybuf || !C0 || !C1) return SB_ERR_NOMEM;
     float2* wT = tabs;
     float2* BT = wT + n1;

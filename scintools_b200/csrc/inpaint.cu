@@ -45,6 +45,7 @@
 #endif
 
 #include "common.cuh"
+#include "drivers.cuh"
 
 namespace sb {
 
@@ -419,7 +420,7 @@ int inpaint_biharmonic(const double* img, int nf, int nt, const int* pix, int n,
     // partials (7 G), then the map (npix int32) and the state
     const size_t nd = 11 * (size_t)n + 3 * ((size_t)maxit + 1) + 7 * (size_t)G;
     const size_t bytes = nd * sizeof(double) + npix * sizeof(int) + sizeof(InpState) + 16;
-    double* w = (double*)workspace(3, bytes);
+    double* w = (double*)workspace(WS_PLANE0, bytes);
     if (!w) return SB_ERR_NOMEM;
     double* b = w;
     double* invd = b + n;

@@ -19,6 +19,7 @@
 // second kernel adds each chunk's (or pair's) partials from its at most four tiles in a
 // fixed order, so every result is deterministic.  Counts live in grid.x or in loops.
 #include "common.cuh"
+#include "drivers.cuh"
 
 namespace sb {
 
@@ -413,7 +414,7 @@ static int mosaic_tiles(const MosGeom& g, const float2* chunks, const double* ph
     constexpr int NQ = MosNq<MODE>::value;
     double* p = nullptr;
     if (MODE != MOS_BUILD) {
-        p = (double*)workspace(8, (size_t)g.ntiles * NQ * sizeof(double));
+        p = (double*)workspace(WS_TABLE, (size_t)g.ntiles * NQ * sizeof(double));
         if (!p) return SB_ERR_NOMEM;
     }
     const size_t smem = (size_t)2 * (g.hf + g.ht) * sizeof(float);

@@ -17,6 +17,7 @@
 #include <math.h>
 
 #include "common.cuh"
+#include "drivers.cuh"
 
 namespace sb {
 

@@ -17,6 +17,7 @@
 #ifndef SB_HOST_EMU            // tests/host_emu runs the scatter / eigenpair kernels on the CPU
 #include "fft_kernels.cuh"
 #endif
+#include "drivers.cuh"
 #include "lanczos.cuh"
 #include "thth.cuh"
 
@@ -183,7 +184,7 @@ int rev_map(const float2* thth, int n, const double* th_dev, double eta, double 
         return SB_ERR_ARG;
     }
     const size_t bins = (size_t)ntau * nfd;
-    int* cnt = (int*)workspace(1, bins * sizeof(int));
+    int* cnt = (int*)workspace(WS_INDEX, bins * sizeof(int));
     if (!cnt) return SB_ERR_NOMEM;
     SB_CUDA(cudaMemsetAsync(recov, 0, bins * sizeof(float2), st));
     SB_CUDA(cudaMemsetAsync(cnt, 0, bins * sizeof(int), st));
@@ -675,7 +676,7 @@ int herm_eigvec(const float2* A, int n, int ld, double tol, int max_iter, double
     size_t smem;
     int rc = eigvec_setup(herm_eigvec_kernel, n, &tol, &max_iter, &smem);
     if (rc) return rc;
-    float2* Q = (float2*)workspace(2, (size_t)(max_iter + 1) * n * sizeof(float2));
+    float2* Q = (float2*)workspace(WS_BATCH, (size_t)(max_iter + 1) * n * sizeof(float2));
     if (!Q) return SB_ERR_NOMEM;
     herm_eigvec_kernel<<<1, EV_THREADS, smem, st>>>(A, n, ld, Q, max_iter, tol, w_dev, V_dev,
                                                     info_dev);
@@ -719,8 +720,7 @@ struct ShiftedRowLoad {
 // Chirp-z inverse of one [n0][n1] plane of any size, ifftshifted first when centred:
 // ifft2(X) = conj(fft2(conj X)) / (n0 n1).  conj_in != 0 transforms conj(in) instead, so
 // that the result is conj(fft2(in)) / (n0 n1).  The output rows x cols go to the base store
-// mk(den), den = the normalisation of the unnormalised inverse it receives (workspace slots
-// 3 .. 7, chirp_fft2).
+// mk(den), den = the normalisation of the unnormalised inverse it receives.
 template <class MakeBase>
 static int ifft2_chirp(const float2* in, int n0, int n1, int centred, int conj_in, int rows,
                        int cols, MakeBase mk, cudaStream_t st) {
@@ -734,8 +734,8 @@ static int ifft2_chirp(const float2* in, int n0, int n1, int centred, int conj_i
 // ifft2 of the nplanes planes of in [nplanes][n0][n1], each ifftshifted first when centred;
 // the output rows x cols of plane p go to the base store mk(p, den) (CropStore or
 // ResidualSink), den = the normalisation of the unnormalised inverse it receives.  Powers of
-// two: the rows of every plane in one launch, then the kept columns plane by plane
-// (workspace slots 3 and 4); other sizes: ifft2_chirp per plane.  Sizes as ifft2_size_check.
+// two: the rows of every plane in one launch, then the kept columns plane by plane; other
+// sizes: ifft2_chirp per plane.  Sizes as ifft2_size_check.
 template <class MakeBase>
 static int ifft2_planes(const float2* in, int nplanes, int n0, int n1, int centred, int rows,
                         int cols, MakeBase mk, cudaStream_t st) {
@@ -748,8 +748,8 @@ static int ifft2_planes(const float2* in, int nplanes, int n0, int n1, int centr
         }
         return SB_OK;
     }
-    float2* B1 = (float2*)workspace(3, nplanes * bins * sizeof(float2));
-    float2* B2 = (float2*)workspace(4, bins * sizeof(float2));
+    float2* B1 = (float2*)workspace(WS_PLANE0, nplanes * bins * sizeof(float2));
+    float2* B2 = (float2*)workspace(WS_PLANE1, bins * sizeof(float2));
     if (!B1 || !B2) return SB_ERR_NOMEM;
     ShiftedRowLoad ld{in, n0, n1, centred};
     PlainRowStore<float2> rs{B1, n1};
@@ -854,7 +854,7 @@ int chisq_sweep(const ThthGeom& g, const double* th_host, const double* d_etas, 
     size_t smem;
     rc = eigvec_setup(herm_eigvec_batch_kernel, ld, &tol, &max_iter, &smem);
     if (rc) return rc;
-    int* d_idx = (int*)workspace(1, (size_t)neta * ld * sizeof(int));
+    int* d_idx = (int*)workspace(WS_INDEX, (size_t)neta * ld * sizeof(int));
     if (!d_idx) return SB_ERR_NOMEM;
     rc = thth_prep(g, th_host, d_etas, neta, ld, d_idx, d_nred, d_status, st);
     if (rc) return rc;
@@ -869,7 +869,7 @@ int chisq_sweep(const ThthGeom& g, const double* th_host, const double* d_etas, 
     const size_t per = (mat + qn + ld + bins) * sizeof(float2) + CHISQ_SLOTS * sizeof(double) +
                        bins * sizeof(int) + (pow2 ? bins * sizeof(float2) : 0);
     const int batch = sweep_batch(per, neta, 65535);
-    unsigned char* ws = (unsigned char*)workspace(2, per * batch);
+    unsigned char* ws = (unsigned char*)workspace(WS_BATCH, per * batch);
     if (!ws) return SB_ERR_NOMEM;
     float2* M = (float2*)ws;
     float2* Q = M + mat * batch;
@@ -978,7 +978,7 @@ static int gerchberg_saxton_any(float2* W, const float* amp, const unsigned char
         return SB_ERR_UNSUPPORTED;
     }
     const long count = (long)n0 * n1;
-    float2* T = (float2*)workspace(2, (size_t)count * sizeof(float2));
+    float2* T = (float2*)workspace(WS_BATCH, (size_t)count * sizeof(float2));
     if (!T) return SB_ERR_NOMEM;
     int blocks = (int)((count + 255) / 256);
     if (blocks > num_sms() * 16) blocks = num_sms() * 16;
@@ -1038,17 +1038,19 @@ int gerchberg_saxton(float2* W, const float* amp, const unsigned char* rowmask, 
         return SB_ERR_UNSUPPORTED;
     }
     if (n1 > 8192) {                  // fp64 rows of this length do not fit shared memory
+        const WsSlot slot[3] = {WS_PLANE0, WS_PLANE1, WS_PLANE2};
         float2* B[3];
         for (int i = 0; i < 3; ++i)
-            if (!(B[i] = (float2*)workspace(3 + i, (size_t)n0 * n1 * sizeof(float2)))) return SB_ERR_NOMEM;
+            if (!(B[i] = (float2*)workspace(slot[i], (size_t)n0 * n1 * sizeof(float2)))) return SB_ERR_NOMEM;
         return gs_pow2<float>(W, amp, rowmask, n0, n1, niter, B, st);
     }
     // fp64 iterations: the phase step divides by |w|, so where |w| is small it amplifies the
     // rounding of the transforms; with fp32 transforms that reaches 1e-5 of the wavefield's
     // scale within three iterations on random input
+    const WsSlot slot[4] = {WS_BATCH, WS_PLANE0, WS_PLANE1, WS_PLANE2};
     double2* B[4];
     for (int i = 0; i < 4; ++i)
-        if (!(B[i] = (double2*)workspace(2 + i, (size_t)n0 * n1 * sizeof(double2)))) return SB_ERR_NOMEM;
+        if (!(B[i] = (double2*)workspace(slot[i], (size_t)n0 * n1 * sizeof(double2)))) return SB_ERR_NOMEM;
     const long count = 2L * n0 * n1;
     int blocks = (int)((count + 255) / 256);
     if (blocks > num_sms() * 16) blocks = num_sms() * 16;
@@ -1133,14 +1135,16 @@ int conj_spectrum_c2c(const float2* in, int nf, int nt, int npad, float pad_re, 
     }
     const int NF = (int)NFl, NT = (int)NTl;
     const size_t count = (size_t)NF * NT;
-    double* sum = (double*)workspace(0, 64 * sizeof(double));
-    float2* P = (float2*)workspace(2, count * sizeof(float2));
-    if (!sum || !P) return SB_ERR_NOMEM;
+    ScalarBlock* sc = scalar_block();
+    if (!sc) return SB_ERR_NOMEM;
+    double* sum = sc->c2c_sum;
+    float2* P = (float2*)workspace(WS_BATCH, count * sizeof(float2));
+    if (!P) return SB_ERR_NOMEM;
     int blocks = (int)((count + 255) / 256);
     if (blocks > num_sms() * 16) blocks = num_sms() * 16;
     const bool dev_mean = pad_re != pad_re;
     if (dev_mean) {
-        SB_CUDA(cudaMemsetAsync(sum, 0, 2 * sizeof(double), st));
+        SB_CUDA(cudaMemsetAsync(sum, 0, sizeof(sc->c2c_sum), st));
         c2c_sum_kernel<<<num_sms() * 4, 256, 0, st>>>(in, (long)nf * nt, sum);
         SB_LAUNCH_CHECK();
     }
@@ -1148,8 +1152,8 @@ int conj_spectrum_c2c(const float2* in, int nf, int nt, int npad, float pad_re, 
                                            dev_mean ? sum : nullptr, P);
     SB_LAUNCH_CHECK();
     if (radix) {
-        float2* B1 = (float2*)workspace(3, count * sizeof(float2));
-        float2* B2 = (float2*)workspace(4, count * sizeof(float2));
+        float2* B1 = (float2*)workspace(WS_PLANE0, count * sizeof(float2));
+        float2* B2 = (float2*)workspace(WS_PLANE1, count * sizeof(float2));
         if (!B1 || !B2) return SB_ERR_NOMEM;
         int rc = SB_OK;
         PitchRowLoad<float2> lr{P, NT};
@@ -1162,7 +1166,7 @@ int conj_spectrum_c2c(const float2* in, int nf, int nt, int npad, float pad_re, 
         return cols_generic<float, -1>(la, B2, NT, NF, NT, CsShiftStore{CS, NF, NT, R1, rowmask},
                                        st);
     }
-    float2* T = (float2*)workspace(1, count * sizeof(float2));
+    float2* T = (float2*)workspace(WS_INDEX, count * sizeof(float2));
     if (!T) return SB_ERR_NOMEM;
     const int rc = ifft2_conj_any(P, NF, NT, (double)count, T, st);
     if (rc) return rc;
@@ -1242,12 +1246,12 @@ int vlbi_retrieval(const ThthGeom& geom, const double* th_host, const float2* co
     if (rc) return rc;
     const size_t bins = (size_t)n0 * n1;
     const size_t qn = (size_t)(max_iter + 1) * (N > 0 ? N : 1);
-    // slot 1: eta, spectrum pointers, crop indices; slot 2: composite, Lanczos basis,
-    // per-station bin sums, shared bin counts
+    // s1: eta, spectrum pointers, crop indices; s2: composite, Lanczos basis, per-station bin
+    // sums, shared bin counts
     unsigned char* s1 = (unsigned char*)workspace(
-        1, sizeof(double) + (size_t)npairs * sizeof(float2*) + (size_t)g.n * sizeof(int));
+        WS_INDEX, sizeof(double) + (size_t)npairs * sizeof(float2*) + (size_t)g.n * sizeof(int));
     unsigned char* s2 = (unsigned char*)workspace(
-        2, ((size_t)N * N + qn + (size_t)n_dish * bins) * sizeof(float2) + bins * sizeof(int));
+        WS_BATCH, ((size_t)N * N + qn + (size_t)n_dish * bins) * sizeof(float2) + bins * sizeof(int));
     if (!s1 || !s2) return SB_ERR_NOMEM;
     double* d_eta = (double*)s1;
     const float2** d_cs = (const float2**)(d_eta + 1);
@@ -1344,10 +1348,10 @@ int asymmetry_batch(const ThthGeom* geoms, const double* const* th_host, int nch
     const size_t mat = (size_t)ld * ld, qn = (size_t)(max_iter + 1) * ld;
     const size_t per = (mat + qn + ld) * sizeof(float2);
     const int batch = sweep_batch(per, nchunk, 65535);
-    // slot 1: geometry table and crop indices; slot 2: the batch's matrices, bases, vectors
+    // s1: geometry table and crop indices; s2: the batch's matrices, bases, vectors
     const size_t tab = ((size_t)nchunk * sizeof(ThthGeom) + 255) / 256 * 256;
-    unsigned char* s1 = (unsigned char*)workspace(1, tab + (size_t)nchunk * ld * sizeof(int));
-    unsigned char* s2 = (unsigned char*)workspace(2, per * batch);
+    unsigned char* s1 = (unsigned char*)workspace(WS_INDEX, tab + (size_t)nchunk * ld * sizeof(int));
+    unsigned char* s2 = (unsigned char*)workspace(WS_BATCH, per * batch);
     if (!s1 || !s2) return SB_ERR_NOMEM;
     ThthGeom* d_geoms = (ThthGeom*)s1;
     int* d_idx = (int*)(s1 + tab);

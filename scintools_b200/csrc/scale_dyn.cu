@@ -15,6 +15,7 @@
 //   out[nlam-1-k][t] = W_k0 y[i_k][t] + W_k1 y[i_k+1][t] + W_k2 M[i_k][t] + W_k3 M[i_k+1][t].
 // HBM-bound: ~7 passes over nf*nt*4 B.
 #include "common.cuh"
+#include "drivers.cuh"
 
 namespace sb {
 
@@ -76,7 +77,7 @@ int scale_dyn_lambda(const float* dyn, int nf, int nt, int flip, const float* a,
         set_error("scale_dyn: a cubic spline needs at least 4 channels (got %d)", nf);
         return SB_ERR_UNSUPPORTED;
     }
-    float* M = (float*)workspace(3, (size_t)nf * nt * sizeof(float));
+    float* M = (float*)workspace(WS_PLANE0, (size_t)nf * nt * sizeof(float));
     if (!M) return SB_ERR_NOMEM;
     spline_moments_kernel<<<(nt + 127) / 128, 128, 0, st>>>(dyn, nf, nt, flip, a, cp, inv, g, p0,
                                                            pn, M);

@@ -37,6 +37,7 @@
 #endif
 
 #include "common.cuh"
+#include "drivers.cuh"
 
 namespace sb {
 
@@ -425,7 +426,7 @@ static int scint_fit(const char* who, const FitDesc* fits_host, int nfit, double
     const size_t nch = table.size();
     const size_t bytes = nfit * (sizeof(FitDesc) + sizeof(int2) + sizeof(FitState)) +
                          nch * (sizeof(int2) + SF_NPART * sizeof(double)) + 6 * 16 + sizeof(int);
-    char* w = (char*)workspace(3, bytes);
+    char* w = (char*)workspace(WS_PLANE0, bytes);
     if (!w) return SB_ERR_NOMEM;
     auto take = [&](size_t b) { char* p = w; w += (b + 15) & ~size_t(15); return p; };
     FitDesc* d_fits = (FitDesc*)take(nfit * sizeof(FitDesc));

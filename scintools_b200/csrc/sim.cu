@@ -15,14 +15,10 @@
 //              xyi = |ifft2(.)|^2 (:232) through the full inverse.
 #include <math.h>
 
+#include "drivers.cuh"
 #include "fft_kernels.cuh"
 
 namespace sb {
-
-struct SimParams {
-    int nx, ny;
-    double dx, dy, alpha, ar, psi, inner, consp;
-};
 
 // ------------------------------------------------------------------ weights
 __device__ __forceinline__ double swdsp(const SimParams& p, double kx, double ky) {
@@ -143,8 +139,8 @@ int sim_screen(int nx, int ny, const double* w, const double* n1, const double* 
                   nx, ny);
         return SB_ERR_UNSUPPORTED;
     }
-    double2* B1 = (double2*)workspace(3, (size_t)nx * ny * sizeof(double2));
-    double2* B2 = (double2*)workspace(4, (size_t)nx * ny * sizeof(double2));
+    double2* B1 = (double2*)workspace(WS_PLANE0, (size_t)nx * ny * sizeof(double2));
+    double2* B2 = (double2*)workspace(WS_PLANE1, (size_t)nx * ny * sizeof(double2));
     if (!B1 || !B2) return SB_ERR_NOMEM;
     ScreenRowLoad ld{w, n1, n2, seed, ny};
     PlainRowStore<double2> rs{B1, ny};
@@ -272,9 +268,9 @@ int sim_intensity(int nx, int ny, int nf, const double* xyp, const double* scale
         return SB_ERR_UNSUPPORTED;
     }
     const size_t fld = (size_t)nx * ny * sizeof(float2);
-    float2* B1 = (float2*)workspace(5, fld);
-    float2* B2 = (float2*)workspace(6, fld);
-    float2* tabs_ = (float2*)workspace(7, (size_t)(nx + 2 * ny + (size_t)nf * nx) * sizeof(float2));
+    float2* B1 = (float2*)workspace(WS_PLANE2, fld);
+    float2* B2 = (float2*)workspace(WS_PLANE3, fld);
+    float2* tabs_ = (float2*)workspace(WS_PLANE4, (size_t)(nx + 2 * ny + (size_t)nf * nx) * sizeof(float2));
     if (!B1 || !B2 || !tabs_) return SB_ERR_NOMEM;
     float2* fx = tabs_;
     float2* fy = fx + nx;

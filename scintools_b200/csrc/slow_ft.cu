@@ -14,6 +14,7 @@
 // Delay axis: a length-nf FFT of every row of Y, in place in `out`, with the fftshift
 // folded into the store: the radix row kernel for powers of two from 8, the row chirp-z
 // of chirp_fft2 for every other length.
+#include "drivers.cuh"
 #include "fft_kernels.cuh"
 
 namespace sb {
@@ -26,8 +27,8 @@ int slow_ft(const float* x, int nt, int nf, const double* s, float2* out, cudaSt
     const int M = next_pow2(2L * nt - 1) < 8 ? 8 : next_pow2(2L * nt - 1);
     const long pt = ((long)nf + 15) & ~15L;
     // C0: cols_generic's intermediate; Bp: the kernel transforms B_f, then A_f B_f in place
-    float2* C0 = (float2*)workspace(5, (size_t)M * pt * sizeof(float2));
-    float2* Bp = (float2*)workspace(7, (size_t)M * pt * sizeof(float2));
+    float2* C0 = (float2*)workspace(WS_PLANE2, (size_t)M * pt * sizeof(float2));
+    float2* Bp = (float2*)workspace(WS_PLANE4, (size_t)M * pt * sizeof(float2));
     if (!C0 || !Bp) return SB_ERR_NOMEM;
     int R1, R2;
     split_len(M, &R1, &R2);
@@ -53,8 +54,8 @@ int slow_ft(const float* x, int nt, int nf, const double* s, float2* out, cudaSt
         return rc;
     }
     const int MT = next_pow2(2L * nf - 1) < 8 ? 8 : next_pow2(2L * nf - 1);
-    float2* tabs = (float2*)workspace(6, (size_t)(nf + 3L * MT) * sizeof(float2));
-    float2* buf = (float2*)workspace(3, (size_t)nt * MT * sizeof(float2));
+    float2* tabs = (float2*)workspace(WS_PLANE3, (size_t)(nf + 3L * MT) * sizeof(float2));
+    float2* buf = (float2*)workspace(WS_PLANE0, (size_t)nt * MT * sizeof(float2));
     if (!tabs || !buf) return SB_ERR_NOMEM;
     float2* wT = tabs;
     float2* BT = wT + nf;

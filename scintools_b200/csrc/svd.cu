@@ -79,6 +79,7 @@
 #endif
 
 #include "common.cuh"
+#include "drivers.cuh"
 
 namespace sb {
 
@@ -620,12 +621,12 @@ int svd_topk(const float* A, int nf, int nt, int k, double* Y, double* s_host, d
         set_error("sb_svd_topk: no launch configuration for nt = %d", nt);
         return SB_ERR_CUDA;
     }
-    double* part = (double*)workspace(8, (size_t)G * nt * sizeof(double));
+    double* part = (double*)workspace(WS_TABLE, (size_t)G * nt * sizeof(double));
     if (!part) return SB_ERR_NOMEM;
     const size_t nV = (size_t)(maxit + 1) * nt;
     const size_t nsmall = nt + 2 * (size_t)(maxit + 1) + (maxit + 1) + (maxit + 2) +
                           (size_t)maxit * k + k + 2;
-    double* V = (double*)workspace(2, (nV + nsmall) * sizeof(double));
+    double* V = (double*)workspace(WS_BATCH, (nV + nsmall) * sizeof(double));
     if (!V) return SB_ERR_NOMEM;
     double* w = V + nV;
     double* h1 = w + nt;
@@ -830,7 +831,7 @@ int bandpass_cols(const float* A, int nf, int nt, int zero_as_nan, const double*
     nchunk = nchunk < 1 ? 1 : (nchunk > nf ? nf : nchunk);
     const int rows_per = (nf + nchunk - 1) / nchunk;
     nchunk = (nf + rows_per - 1) / rows_per;
-    double* psum = (double*)workspace(8, (size_t)2 * nchunk * nt * sizeof(double));
+    double* psum = (double*)workspace(WS_TABLE, (size_t)2 * nchunk * nt * sizeof(double));
     if (!psum) return SB_ERR_NOMEM;
     double* pcnt = psum + (size_t)nchunk * nt;
     bandpass_col_kernel<<<dim3(gx, nchunk), BP_THREADS, 0, st>>>(A, nf, nt, zero_as_nan, rowdiv,

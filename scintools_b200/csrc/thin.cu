@@ -18,6 +18,7 @@
 #include <limits.h>
 #include <math.h>
 
+#include "drivers.cuh"
 #include "lanczos.cuh"
 #include "thth.cuh"
 
@@ -25,16 +26,6 @@ namespace sb {
 
 enum { TST_OK = 0, TST_INDEX_ERROR = 1, TST_ZERO_START = 2, TST_TOO_SMALL = 4,
        TST_NOT_CONVERGED = 8 };
-
-struct ThinGeom {
-    ThthGeom g;          // cs, ntau, nfd, dtau, dfd ...; tau0 := tau[1], fd0 := fd[1];
-                         // g.th / g.n = theta1 centres (columns)
-    const double* th2;   // theta2 centres (rows)
-    int n2;
-    double tau_max;      // tau.max() (not abs)
-    double center_cut;
-    int power;           // 0: CS as is, 1: |CS|^2 (incoherent thin, ththmod.py:609)
-};
 
 // crop masks + compaction for both axes, one warp per eta
 __global__ void thin_prep_kernel(ThinGeom t, const double* __restrict__ eta1,
@@ -340,7 +331,7 @@ int thin_sweep(const ThinGeom& t, const double* d_eta1, const double* d_eta2, in
         set_error("thin theta-theta grid %dx%d exceeds the supported 4096", t.n2, t.g.n);
         return SB_ERR_UNSUPPORTED;
     }
-    int* d_idx = (int*)workspace(1, (size_t)neta * (ld1 + ld2) * sizeof(int));
+    int* d_idx = (int*)workspace(WS_INDEX, (size_t)neta * (ld1 + ld2) * sizeof(int));
     if (!d_idx) return SB_ERR_NOMEM;
     int* d_idx1 = d_idx;
     int* d_idx2 = d_idx + (size_t)neta * ld1;
@@ -357,7 +348,7 @@ int thin_sweep(const ThinGeom& t, const double* d_eta1, const double* d_eta2, in
     }
     const size_t per = (size_t)ld1 * ld2 * sizeof(float2);
     const int batch = sweep_batch(per, neta, INT_MAX);
-    float2* d_M = (float2*)workspace(2, per * batch);
+    float2* d_M = (float2*)workspace(WS_BATCH, per * batch);
     if (!d_M) return SB_ERR_NOMEM;
     constexpr int TH = 256;
     const size_t smem = sizeof(LanczosShared) + 3 * (size_t)ld1 * sizeof(float2) +

@@ -14,17 +14,11 @@
 
 #include <vector>
 
+#include "drivers.cuh"
 #include "lanczos.cuh"
 #include "thth.cuh"
 
 namespace sb {
-
-#ifndef SB_HOST_EMU
-// eig_half.cu: fp16 iteration + fp32 Rayleigh quotient (default for ld <= 512)
-int eig_half_launch(const float2* d_M, const unsigned* d_Mb, int ld, const int* d_nred, int e0,
-                    int nb, double* d_eigs, int* d_status, int* d_iters, double tol, double etol,
-                    int max_iter, cudaStream_t st);
-#endif  // SB_HOST_EMU
 
 // status codes per eta (also in include/scint_b200.h)
 enum { ST_OK = 0, ST_INDEX_ERROR = 1, ST_ZERO_START = 2, ST_TOO_SMALL = 4,
@@ -817,7 +811,7 @@ int thth_gather_source(const ThthGeom& g, const double* th_host, int neta, ThthC
         return SB_OK;
     };
     if (!hit) {
-        int* tab = (int*)workspace(8, tab_bytes);
+        int* tab = (int*)workspace(WS_TABLE, tab_bytes);
         if (!tab) return SB_ERR_NOMEM;
         int rc = build_table(tab, INT_MAX);
         if (rc) return rc;
@@ -846,7 +840,7 @@ int thth_gather_source(const ThthGeom& g, const double* th_host, int neta, ThthC
         return SB_OK;
     }
     unsigned char* ws = (unsigned char*)workspace(
-        8, tab_bytes + (size_t)nslots * (size_t)tau_pitch * sizeof(float2));
+        WS_TABLE, tab_bytes + (size_t)nslots * (size_t)tau_pitch * sizeof(float2));
     if (!ws) return SB_ERR_NOMEM;
     int* tab = (int*)ws;
     float2* C = (float2*)(ws + tab_bytes);
@@ -926,7 +920,7 @@ int eta_sweep(const ThthGeom& g, const double* th_host, const double* d_etas,
         set_error("theta-theta grid of %d centres exceeds the supported 4096", g.n);
         return SB_ERR_UNSUPPORTED;
     }
-    int* d_idx = (int*)workspace(1, (size_t)neta * ld * sizeof(int));
+    int* d_idx = (int*)workspace(WS_INDEX, (size_t)neta * ld * sizeof(int));
     if (!d_idx) return SB_ERR_NOMEM;
     int rc = thth_prep(g, th_host, d_etas, neta, ld, d_idx, d_nred, d_status, st);
     if (rc) return rc;
@@ -935,7 +929,7 @@ int eta_sweep(const ThthGeom& g, const double* th_host, const double* d_etas,
     if (rc) return rc;
     const size_t per = (size_t)ld * ld * sizeof(float2);
     const int batch = sweep_batch(per, neta, INT_MAX);
-    float2* d_M = (float2*)workspace(2, per * batch);
+    float2* d_M = (float2*)workspace(WS_BATCH, per * batch);
     if (!d_M) return SB_ERR_NOMEM;
     // default solver for ld <= 512 (eig_half.cu): iterates on the fp16 copy written by the
     // build kernel.  Larger grids, and every grid with SB_EIG_FP32=1, run the fp32
@@ -947,10 +941,11 @@ int eta_sweep(const ThthGeom& g, const double* th_host, const double* d_etas,
     float span = 0.f;
     size_t smem = 0;
     if (fp16) {
-        d_Mb = (unsigned*)workspace(6, per / 2 * batch);
+        d_Mb = (unsigned*)workspace(WS_PLANE3, per / 2 * batch);
         if (!d_Mb) return SB_ERR_NOMEM;
-        d_absmax = (unsigned*)workspace(0, 64 * sizeof(double)) + 32;   // behind the dynspec stats
-        if (!d_absmax) return SB_ERR_NOMEM;
+        ScalarBlock* sc = scalar_block();
+        if (!sc) return SB_ERR_NOMEM;
+        d_absmax = &sc->sweep_scale;
         if (g.cs_bound) {       // the caller knows a bound (sb_cs_bound_f32): no scan
             SB_CUDA(cudaMemcpyAsync(d_absmax, g.cs_bound, sizeof(float), cudaMemcpyDeviceToDevice, st));
         } else {
