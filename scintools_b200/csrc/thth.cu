@@ -122,18 +122,27 @@ __device__ __forceinline__ unsigned pack_f16x2(float2 v) {
 // max |re|, |im| over the part of the conjugate spectrum the gather can touch
 // (rows x ncols of a [rows][pitch] array): the bound that keeps the scaled fp16
 // triangle finite.  out: non-negative float as uint bits (atomicMax), pre-zeroed.
+// VEC: float4 loads of two complex columns, for a 16-byte aligned cs with an even pitch
+// (every row 16-byte aligned); otherwise one float2 per column (an odd pitch starts every
+// other row 8 bytes off a 16-byte boundary).
+template <bool VEC>
 __global__ void cs_absmax_kernel(const float2* __restrict__ cs, long long rows, long long ncols,
                                  long long pitch, unsigned* __restrict__ out) {
     float m = 0.f;
-    const long long per_row4 = ncols >> 1;          // float4 = two complex columns
-    const long long total = rows * per_row4;
+    const long long per_row = VEC ? ncols >> 1 : ncols;
+    const long long total = rows * per_row;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
          i += (long long)gridDim.x * blockDim.x) {
-        const long long r = i / per_row4, c = i - r * per_row4;
-        const float4 q = __ldg(reinterpret_cast<const float4*>(cs + r * pitch) + c);
-        m = fmaxf(fmaxf(fmaxf(fabsf(q.x), fabsf(q.y)), fmaxf(fabsf(q.z), fabsf(q.w))), m);
+        const long long r = i / per_row, c = i - r * per_row;
+        if (VEC) {
+            const float4 q = __ldg(reinterpret_cast<const float4*>(cs + r * pitch) + c);
+            m = fmaxf(fmaxf(fmaxf(fabsf(q.x), fabsf(q.y)), fmaxf(fabsf(q.z), fabsf(q.w))), m);
+        } else {
+            const float2 q = __ldg(cs + r * pitch + c);
+            m = fmaxf(fmaxf(fabsf(q.x), fabsf(q.y)), m);
+        }
     }
-    if (ncols & 1) {                                 // odd tail column
+    if (VEC && (ncols & 1)) {                        // odd tail column
         for (long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x; r < rows;
              r += (long long)gridDim.x * blockDim.x) {
             const float2 q = __ldg(cs + r * pitch + ncols - 1);
@@ -952,7 +961,12 @@ int eta_sweep(const ThthGeom& g, const double* th_host, const double* d_etas,
             SB_CUDA(cudaMemsetAsync(d_absmax, 0, sizeof(unsigned), st));
             const long long ncols = g.cs_half ? (g.cs_valid_cols > 0 ? g.cs_valid_cols : g.nfd / 2 + 1)
                                               : g.nfd;
-            cs_absmax_kernel<<<num_sms() * 8, 256, 0, st>>>(g.cs, g.ntau, ncols, g.cs_pitch, d_absmax);
+            if (g.cs_pitch % 2 == 0 && ((uintptr_t)g.cs & 15) == 0)
+                cs_absmax_kernel<true><<<num_sms() * 8, 256, 0, st>>>(g.cs, g.ntau, ncols, g.cs_pitch,
+                                                                      d_absmax);
+            else
+                cs_absmax_kernel<false><<<num_sms() * 8, 256, 0, st>>>(g.cs, g.ntau, ncols, g.cs_pitch,
+                                                                       d_absmax);
             SB_LAUNCH_CHECK();
         }
         double tmin = th_host[0], tmax = th_host[0];
