@@ -279,6 +279,27 @@ int sb_acf_sspec_f32(const float* dyn, int32_t nf, int32_t nt, const float* win_
                      const float* win_f, double sum_win_t, double sum_win_f,
                      int32_t normalise, float* acf, void* stream);
 
+/* Replaces the tile loop of Dynspec.cut_dyn (scintools/dynspec.py:3158-3271): the
+ * secondary spectrum of every tile, each exactly as sb_sspec_f32 with halve=1, db=1,
+ * prewhite=0 would make it from that tile alone.  The parent dyn: float32 [nf][nt] (row
+ * pitch nt); tile (ii, jj), ii < nfc, jj < ntc, is dyn[ii*fnum + f][jj*tnum + t]
+ * (f < fnum, t < tnum), so nfc*fnum <= nf and ntc*tnum <= nt.  win_t [tnum] / win_f
+ * [fnum]: the tile's tapers (scint_utils.get_window of the tile size) or both NULL;
+ * sum_win_*: their sums.  sec: float32 [nfc][ntc][nrfft/2][ncfft] with nrfft, ncfft of
+ * sb_sspec_f32 for an fnum x tnum spectrum.  Each tile's means are its own: a NaN makes its
+ * own tile NaN and no other.  fnum 2..32768, tnum 5..16384 (SB_ERR_UNSUPPORTED otherwise);
+ * any number of tiles, run in groups whose workspace fits a fixed 1 GiB (one tile at least). */
+int sb_sspec_tiles_f32(const float* dyn, int32_t nf, int32_t nt, int32_t fnum, int32_t tnum,
+                       int32_t nfc, int32_t ntc, const float* win_t, const float* win_f,
+                       double sum_win_t, double sum_win_f, float* sec, void* stream);
+
+/* The ACFs of the tiles of sb_sspec_tiles_f32 (same dyn, nf, nt, fnum, tnum, nfc, ntc),
+ * each as sb_acf_f32(subtract_mean=0, normalise=1) makes it from that tile alone, i.e.
+ * Dynspec.calc_acf(input_dyn=tile): acf float32 [nfc][ntc][2 fnum][2 tnum], every tile
+ * divided by its own zero-lag value.  Limits and grouping as sb_sspec_tiles_f32. */
+int sb_acf_tiles_f32(const float* dyn, int32_t nf, int32_t nt, int32_t fnum, int32_t tnum,
+                     int32_t nfc, int32_t ntc, float* acf, void* stream);
+
 /* Replaces the CS stage of ththmod.single_search (scintools/ththmod.py:777-787)
  * and Dynspec.thetatheta_single (scintools/dynspec.py:1572-1579):
  *   CS = fftshift(fft2(pad(dspec, npad copies, constant pad_value)));

@@ -100,6 +100,9 @@ _SIGS = {
     "sb_ifft2_c2c_f32": (c_int, [vp, c_int, c_int, c_int, c_int, c_int, c_dbl, c_int, vp, vp]),
     "sb_acf_f32": (c_int, [vp, c_int, c_int, c_int, c_int, vp, vp]),
     "sb_acf_sspec_f32": (c_int, [vp, c_int, c_int, vp, vp, c_dbl, c_dbl, c_int, vp, vp]),
+    "sb_sspec_tiles_f32": (c_int, [vp, c_int, c_int, c_int, c_int, c_int, c_int, vp, vp, c_dbl,
+                                   c_dbl, vp, vp]),
+    "sb_acf_tiles_f32": (c_int, [vp, c_int, c_int, c_int, c_int, c_int, c_int, vp, vp]),
     "sb_cs_f32": (c_int, [vp, c_int, c_int, c_int, c_flt, vp, c_int, c_i64, c_int, vp, vp]),
     "sb_cs_bound_f32": (c_int, [vp, c_int, c_int, c_int, c_flt, vp, vp]),
     "sb_cs_c2c_f32": (c_int, [vp, c_int, c_int, c_int, c_flt, c_flt, vp, vp, vp]),

@@ -330,6 +330,21 @@ int sb_acf_sspec_f32(const float* dyn, int32_t nf, int32_t nt, const float* win_
                          acf, (cudaStream_t)stream);
 }
 
+int sb_sspec_tiles_f32(const float* dyn, int32_t nf, int32_t nt, int32_t fnum, int32_t tnum,
+                       int32_t nfc, int32_t ntc, const float* win_t, const float* win_f,
+                       double sum_win_t, double sum_win_f, float* sec, void* stream) {
+    SB_ARG(dyn && sec);
+    SB_ARG((win_t == nullptr) == (win_f == nullptr));
+    return sb::sspec_tiles(dyn, nf, nt, fnum, tnum, nfc, ntc, win_t, win_f, sum_win_t, sum_win_f,
+                           sec, (cudaStream_t)stream);
+}
+
+int sb_acf_tiles_f32(const float* dyn, int32_t nf, int32_t nt, int32_t fnum, int32_t tnum,
+                     int32_t nfc, int32_t ntc, float* acf, void* stream) {
+    SB_ARG(dyn && acf);
+    return sb::acf_tiles(dyn, nf, nt, fnum, tnum, nfc, ntc, acf, (cudaStream_t)stream);
+}
+
 int sb_cs_f32(const float* dspec, int32_t nf, int32_t nt, int32_t npad,
               float pad_value, const uint8_t* tau_rowmask, int32_t half_plane,
               int64_t cs_pitch, int32_t ncols_keep, void* cs, void* stream) {

@@ -22,13 +22,14 @@ const char* last_error();
 //   WS_SCALARS    the ScalarBlock below
 //   WS_INDEX      index tables of eta_sweep, thin_sweep, chisq_sweep; rev_map's bin counts;
 //                 vlbi_retrieval's and asymmetry_batch's per-call arrays; the chirp-z result
-//                 of conj_spectrum_c2c
+//                 of conj_spectrum_c2c; the per-tile sums of sspec_tiles and acf_tiles
 //   WS_BATCH      the batch slab of eta_sweep, thin_sweep, chisq_sweep, vlbi_retrieval,
 //                 asymmetry_batch; herm_eigvec's basis; the padded chunk of
 //                 conj_spectrum_c2c; gerchberg_saxton; svd_topk
 //   WS_PLANE0..4  the FFT engine: chirp_fft2 takes all five (through ifft2_chirp,
 //                 ifft2_planes, ifft2_conj_any and the chirp-z conj_spectrum); the radix
-//                 2-D transforms of sspec, acf, acf_sspec, conj_spectrum, ifft2_planes,
+//                 2-D transforms of sspec, acf, acf_sspec, sspec_tiles, acf_tiles,
+//                 conj_spectrum, ifft2_planes,
 //                 conj_spectrum_c2c and gerchberg_saxton take PLANE0..2.  Drivers that
 //                 call neither use them too: sim_screen, sim_intensity, slow_ft,
 //                 inpaint_biharmonic, scint_fit, acf_model, scale_dyn_lambda; eta_sweep
@@ -67,7 +68,7 @@ struct ScalarBlock {
     unsigned pad1[15];
     double l1;                // conj_spectrum_bound: L1 norm accumulator
     double pad2[7];
-    double acf_part[32];      // acf: partial power sums
+    double acf_part[32];      // acf: partial power sums (acf_tiles: written, not read)
 };
 static_assert(offsetof(ScalarBlock, stats) == 0, "ScalarBlock layout");
 static_assert(offsetof(ScalarBlock, c2c_sum) == 0, "ScalarBlock layout");

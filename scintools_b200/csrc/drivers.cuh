@@ -58,6 +58,11 @@ int acf(const float* dyn, int nf, int nt, int subtract_mean, int normalise,
         float* out, cudaStream_t st);
 int acf_sspec(const float* dyn, int nf, int nt, const float* wt, const float* wf,
               double swt, double swf, int normalise, float* out, cudaStream_t st);
+int sspec_tiles(const float* dyn, int nf, int nt, int fnum, int tnum, int nfc, int ntc,
+                const float* wt, const float* wf, double swt, double swf, float* sec,
+                cudaStream_t st);
+int acf_tiles(const float* dyn, int nf, int nt, int fnum, int tnum, int nfc, int ntc,
+              float* acf, cudaStream_t st);
 void twiddle_release();
 
 // sim.cu

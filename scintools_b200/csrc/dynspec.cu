@@ -14,6 +14,7 @@
 
 #include "drivers.cuh"
 #include "fft_kernels.cuh"
+#include "tiles.cuh"
 
 namespace sb {
 
@@ -235,41 +236,6 @@ struct CsStore {
     }
 };
 
-// secondary spectrum epilogue: |.|^2, fftshift, keep tau >= 0, post-darken, dB
-struct SspecStore {
-    float* sec;
-    int NF, NT, R1;
-    int halve, db;
-    const float* pd1;   // [NT] sin^2 over the shifted fd axis, or null
-    const float* pd2;   // [NF/2] sin^2 over td
-    int noshift;        // 1: natural (un-fftshifted) order, full frame only
-    __device__ __forceinline__ void put(int kf, int cs, float p) const {
-        int row;
-        if (noshift) {
-            row = kf;
-            cs = (cs + NT / 2) & (NT - 1);     // undo the column shift
-        } else if (halve) {
-            if (kf >= NF / 2) return;
-            row = kf;
-        } else {
-            row = (kf + NF / 2) & (NF - 1);
-        }
-        if (pd1) {
-            const float pd = (cs == NT / 2 || row == 0) ? 1.f : pd1[cs] * pd2[row];
-            p = p / pd;
-        }
-        if (db) p = 10.f * log10f(p);
-        sec[(size_t)row * NT + cs] = p;
-    }
-    __device__ __forceinline__ void operator()(int y, int k, int c, float2 v) const {
-        const int kf = y + R1 * k;
-        const float p = v.x * v.x + v.y * v.y;
-        put(kf, (c + NT / 2) & (NT - 1), p);
-        if (c != 0 && c != NT / 2)
-            put((NF - kf) & (NF - 1), ((NT - c) + NT / 2) & (NT - 1), p);
-    }
-};
-
 // ------------------------------------------------------------- ACF kernels
 // forward over r2 -> |.|^2 (+ weighted power sum) -> inverse over k2 ->
 // twiddle W_R^(+n2 k1); all inside one shared-memory tile.
@@ -317,33 +283,6 @@ acf_mid_kernel(const float2* __restrict__ A, float2* __restrict__ G, long pitch,
         }
     }
 }
-
-struct AcfRowLoad {   // output row i <- circular row (i - nf) mod PF
-    const float2* Q;
-    long pitch;
-    int nf, PF;
-    __device__ __forceinline__ float2 operator()(long row, int k) const {
-        const int n = ((int)row - nf + PF) & (PF - 1);
-        return Q[(size_t)n * pitch + k];
-    }
-};
-struct AcfRowStore {
-    float* acf;
-    int nt, PT;
-    const float* scale;    // device scalar written by acf_scale_kernel
-    __device__ __forceinline__ void one(long row, int t, float x, float sc) const {
-        int j;
-        if (t < nt) j = t + nt;
-        else if (t >= PT - nt) j = t - (PT - nt);
-        else return;
-        acf[(size_t)row * (2 * nt) + j] = x * sc;
-    }
-    __device__ __forceinline__ void operator()(long row, int n, float2 z) const {
-        const float sc = *scale;
-        one(row, 2 * n, z.x, sc);
-        one(row, 2 * n + 1, z.y, sc);
-    }
-};
 
 // stats[7] = full-plane power sum (of the 32 partials acf_part); acf_factor = the factor the
 // row pass multiplies with: 1 / sum (normalise) or the raw ifft2 scale
@@ -731,6 +670,59 @@ int conj_spectrum(const float* dyn, int nf, int nt, int npad, float pad_value,
     return cols_forward(H, A, pitch, NF, nf, ncols, cs, st, PROF_CS_COLA, PROF_CS_COLB);
 }
 
+// Column half of the ACF over the half spectra H[live][pitch] (ncols columns, zero rows up
+// to PF): forward pass A; forward pass B -> |.|^2 -> inverse over k2 in one kernel, whose
+// weighted power sums go to the 32 slots psum; the inverse over k1 -> Q = A [PF][pitch] in
+// natural row order.  G [PF][pitch] is scratch.
+static int acf_cols(const float2* H, float2* A, float2* G, long pitch, int PF, int PT, int live,
+                    int ncols, double* psum, cudaStream_t st) {
+    int rc = SB_OK;
+    int R1, R2;
+    split_len(PF, &R1, &R2);
+    // forward pass A
+    {
+        const float2* wR = twiddle_table<float>(PF, -1, st);
+        if (!wR) return SB_ERR_NOMEM;
+        ZeroPadALoad<float2> la{H, pitch, R2, live};
+        TwiddleAStore<float2> sa{A, pitch, R2, PF, wR};
+        CUtensorMap mapA;
+        if (make_tile_map(&mapA, H, pitch, ncols, live, R2, R1, 32)) {
+            SB_TILE_DISPATCH(R1, rc = (launch_tile_fft_tma<LL, 32, -1, 3>(mapA, sa, ncols, R2, st)));
+        } else {
+            SB_TILE_DISPATCH(R1, rc = (launch_tile_fft<float, LL, 32, -1>(la, sa, ncols, R2, st)));
+        }
+        if (rc) return rc;
+    }
+    // fused forward pass B -> power -> inverse over k2
+    {
+        const float2* wRi = twiddle_table<float>(PF, +1, st);
+        const float2* twf = twiddle_table<float>(R2, -1, st);
+        const float2* twi = twiddle_table<float>(R2, +1, st);
+        if (!wRi || !twf || !twi) return SB_ERR_NOMEM;
+        dim3 grid((ncols + 31) / 32, R1);
+        SB_TILE_DISPATCH(R2, {
+            auto kern = acf_mid_kernel<LL, 32>;
+            const size_t smem = (size_t)(LL * 32 + 2 * LL) * sizeof(float2);
+            SB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            kern<<<grid, 256, smem, st>>>(A, G, pitch, R1, ncols, PT, twf, twi, wRi, psum);
+        });
+        SB_LAUNCH_CHECK();
+    }
+    // inverse over k1 -> Q (reuse A)
+    {
+        StrideALoad<float2> li{G, pitch, R2};      // y = n2, i = k1
+        NaturalBStore<float2> si{A, pitch, R2};    // n = n2 + R2 n1
+        CUtensorMap mapG;
+        if (make_tile_map(&mapG, G, pitch, ncols, PF, R2, R1, 32)) {
+            SB_TILE_DISPATCH(R1, rc = (launch_tile_fft_tma<LL, 32, +1, 3>(mapG, si, ncols, R2, st)));
+        } else {
+            SB_TILE_DISPATCH(R1, rc = (launch_tile_fft<float, LL, 32, +1>(li, si, ncols, R2, st)));
+        }
+        if (rc) return rc;
+    }
+    return SB_OK;
+}
+
 // Dynspec.calc_acf(method='direct') (dynspec.py:3780-3797)
 int acf(const float* dyn, int nf, int nt, int subtract_mean, int normalise,
         float* out, cudaStream_t st) {
@@ -754,52 +746,10 @@ int acf(const float* dyn, int nf, int nt, int subtract_mean, int normalise,
     DynRowLoad ld{dyn, nf, nt, nullptr, nullptr, stats, subtract_mean ? 1 : 2, 0, 0.f};
     rc = rows_r2c(ld, H, pitch, PT, nf, st);
     if (rc) return rc;
-    int R1, R2;
-    split_len(PF, &R1, &R2);
-    const int ncols = PT / 2 + 1;
-    // forward pass A
-    {
-        const float2* wR = twiddle_table<float>(PF, -1, st);
-        if (!wR) return SB_ERR_NOMEM;
-        ZeroPadALoad<float2> la{H, pitch, R2, nf};
-        TwiddleAStore<float2> sa{A, pitch, R2, PF, wR};
-        CUtensorMap mapA;
-        if (make_tile_map(&mapA, H, pitch, ncols, nf, R2, R1, 32)) {
-            SB_TILE_DISPATCH(R1, rc = (launch_tile_fft_tma<LL, 32, -1, 3>(mapA, sa, ncols, R2, st)));
-        } else {
-            SB_TILE_DISPATCH(R1, rc = (launch_tile_fft<float, LL, 32, -1>(la, sa, ncols, R2, st)));
-        }
-        if (rc) return rc;
-    }
-    // fused forward pass B -> power -> inverse over k2
-    {
-        const float2* wRi = twiddle_table<float>(PF, +1, st);
-        const float2* twf = twiddle_table<float>(R2, -1, st);
-        const float2* twi = twiddle_table<float>(R2, +1, st);
-        if (!wRi || !twf || !twi) return SB_ERR_NOMEM;
-        dim3 grid((ncols + 31) / 32, R1);
-        SB_TILE_DISPATCH(R2, {
-            auto kern = acf_mid_kernel<LL, 32>;
-            const size_t smem = (size_t)(LL * 32 + 2 * LL) * sizeof(float2);
-            SB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            kern<<<grid, 256, smem, st>>>(A, G, pitch, R1, ncols, PT, twf, twi, wRi, sc->acf_part);
-        });
-        SB_LAUNCH_CHECK();
-        acf_scale_kernel<<<1, 32, 0, st>>>(stats, normalise, 1.0 / ((double)PF * (double)PT));
-        SB_LAUNCH_CHECK();
-    }
-    // inverse over k1 -> Q (reuse A)
-    {
-        StrideALoad<float2> li{G, pitch, R2};      // y = n2, i = k1
-        NaturalBStore<float2> si{A, pitch, R2};    // n = n2 + R2 n1
-        CUtensorMap mapG;
-        if (make_tile_map(&mapG, G, pitch, ncols, PF, R2, R1, 32)) {
-            SB_TILE_DISPATCH(R1, rc = (launch_tile_fft_tma<LL, 32, +1, 3>(mapG, si, ncols, R2, st)));
-        } else {
-            SB_TILE_DISPATCH(R1, rc = (launch_tile_fft<float, LL, 32, +1>(li, si, ncols, R2, st)));
-        }
-        if (rc) return rc;
-    }
+    rc = acf_cols(H, A, G, pitch, PF, PT, nf, PT / 2 + 1, sc->acf_part, st);
+    if (rc) return rc;
+    acf_scale_kernel<<<1, 32, 0, st>>>(stats, normalise, 1.0 / ((double)PF * (double)PT));
+    SB_LAUNCH_CHECK();
     // rows: half spectrum -> real, crop to lags [-nf, nf) x [-nt, nt)
     AcfRowLoad rl{A, pitch, nf, PF};
     AcfRowStore rs{out, nt, PT, &sc->acf_factor};
@@ -854,6 +804,133 @@ int acf_sspec(const float* dyn, int nf, int nt, const float* wt, const float* wf
     split_len(NF, &R1, &R2);
     RealShiftStore rs{out, NF, NT, R1, stats, normalise};
     return cols_forward(H, A, pitch, NF, NF, NT / 2 + 1, rs, st);
+}
+
+// ------------------------------------------------------------------------
+// Dynspec.cut_dyn (dynspec.py:3158-3271): the secondary spectrum and ACF of every
+// fnum x tnum tile of the parent dyn [nf][nt], tiles in consecutive groups whose FFT
+// workspace fits kTileBudget (one tile at least, however large).  Per group: one
+// statistics pass, one row pass and the column passes, whatever the number of tiles.
+// Layout and functors: tiles.cuh.
+// ------------------------------------------------------------------------
+static constexpr size_t kTileBudget = size_t(1) << 30;
+
+static int tile_args(int nf, int nt, int fnum, int tnum, int nfc, int ntc) {
+    if (fnum < 2 || fnum > 32768 || tnum < 5 || tnum > 16384) {
+        set_error("cut_dyn: tile %dx%d outside the supported sizes (fnum 2..32768, tnum 5..16384)",
+                  fnum, tnum);
+        return SB_ERR_UNSUPPORTED;
+    }
+    if (nfc < 1 || ntc < 1 || (long)nfc * fnum > nf || (long)ntc * tnum > nt ||
+        (long)nfc * ntc > 0x7fffffffL) {
+        set_error("cut_dyn: %d x %d tiles of %dx%d do not fit a %dx%d spectrum", nfc, ntc, fnum,
+                  tnum, nf, nt);
+        return SB_ERR_ARG;
+    }
+    return SB_OK;
+}
+
+// tiles per group: as many as kTileBudget holds at per_tile bytes of workspace each, >= 1
+static long tile_group(size_t per_tile, long ntile) {
+    const long g = (long)(kTileBudget / per_tile);
+    return g < 1 ? 1 : (g < ntile ? g : ntile);
+}
+
+// sums [ntile][4] and constants [ntile] of the group's tiles in WS_INDEX (tile_stats_kernel,
+// tile_stats_final_kernel); *cst receives the constants
+static int tile_stats(const float* dyn, long ld, int fnum, int tnum, int ntc, int tile0,
+                      int ntile, const float* wt, const float* wf, double swt, double swf,
+                      double acf_den, float2** cst, cudaStream_t st) {
+    double* sums = (double*)workspace(WS_INDEX, (size_t)ntile * (4 * sizeof(double) + sizeof(float2)));
+    if (!sums) return SB_ERR_NOMEM;
+    *cst = (float2*)(sums + 4L * ntile);
+    SB_CUDA(cudaMemsetAsync(sums, 0, (size_t)ntile * 4 * sizeof(double), st));
+    int rpi = 4096 / tnum;                      // rows per warp item: ~4096 pixels
+    rpi = rpi < 1 ? 1 : (rpi > fnum ? fnum : rpi);
+    const long items = (long)ntile * ((fnum + rpi - 1) / rpi);
+    const long blocks = (items + 7) / 8 < num_sms() * 8L ? (items + 7) / 8 : num_sms() * 8L;
+    tile_stats_kernel<<<(unsigned)blocks, 256, 0, st>>>(dyn, ld, fnum, tnum, ntc, tile0, ntile,
+                                                        rpi, wt, wf, sums);
+    SB_LAUNCH_CHECK();
+    tile_stats_final_kernel<<<(ntile + 255) / 256, 256, 0, st>>>(
+        sums, ntile, (double)fnum * tnum, swt, swf, wt != nullptr, acf_den, *cst);
+    SB_LAUNCH_CHECK();
+    return SB_OK;
+}
+
+// calc_sspec(input_dyn=tile) of every tile: window (wt [tnum], wf [fnum]) or none, halved,
+// dB.  sec: [nfc * ntc][NF / 2][NT]
+int sspec_tiles(const float* dyn, int nf, int nt, int fnum, int tnum, int nfc, int ntc,
+                const float* wt, const float* wf, double swt, double swf, float* sec,
+                cudaStream_t st) {
+    int rc = tile_args(nf, nt, fnum, tnum, nfc, ntc);
+    if (rc) return rc;
+    ProfScope prof(PROF_SSPEC, st);
+    const int NF = 2 * next_pow2(fnum), NT = 2 * next_pow2(tnum);
+    const long tp = half_pitch(NT), ntile = (long)nfc * ntc;
+    const size_t plane = (size_t)(NF / 2) * NT;
+    const long g = tile_group((size_t)(fnum + NF) * tp * sizeof(float2), ntile);
+    int R1, R2;
+    split_len(NF, &R1, &R2);
+    for (long t0 = 0; t0 < ntile; t0 += g) {
+        const int n = (int)(ntile - t0 < g ? ntile - t0 : g);
+        const long pitch = n * tp;
+        float2* H = (float2*)workspace(WS_PLANE0, (size_t)fnum * pitch * sizeof(float2));
+        float2* A = (float2*)workspace(WS_PLANE1, (size_t)NF * pitch * sizeof(float2));
+        if (!H || !A) return SB_ERR_NOMEM;
+        float2* cst = nullptr;
+        rc = tile_stats(dyn, nt, fnum, tnum, ntc, (int)t0, n, wt, wf, swt, swf, 0.0, &cst, st);
+        if (rc) return rc;
+        TileRowLoad ld{dyn, nt, fnum, tnum, ntc, (int)t0, wt, wf, cst};
+        TileHalfStore hs{H, pitch, (int)tp, fnum};
+        SB_ROW_DISPATCH(NT / 2, rc = (launch_row_r2c<float, N1, N2>(ld, hs, (long)n * fnum, st)));
+        if (rc) return rc;
+        TileSspecStore ss{SspecStore{sec + (size_t)t0 * plane, NF, NT, R1, 1, 1, nullptr, nullptr, 0},
+                          (int)tp, NT / 2 + 1, plane};
+        rc = cols_forward(H, A, pitch, NF, fnum, (int)pitch, ss, st);
+        if (rc) return rc;
+    }
+    return SB_OK;
+}
+
+// calc_acf(input_dyn=tile) of every tile: no mean subtracted, normalised to the zero lag.
+// acf: [nfc * ntc][2 fnum][2 tnum]
+int acf_tiles(const float* dyn, int nf, int nt, int fnum, int tnum, int nfc, int ntc,
+              float* acf, cudaStream_t st) {
+    int rc = tile_args(nf, nt, fnum, tnum, nfc, ntc);
+    if (rc) return rc;
+    ProfScope prof(PROF_ACF, st);
+    const int PF = next_pow2(2L * fnum), PT = next_pow2(2L * tnum);
+    const long tp = half_pitch(PT), ntile = (long)nfc * ntc;
+    const size_t plane = (size_t)(2 * fnum) * (2 * tnum);
+    const long g = tile_group((size_t)(fnum + 2L * PF) * tp * sizeof(float2), ntile);
+    ScalarBlock* sc = scalar_block();
+    if (!sc) return SB_ERR_NOMEM;
+    for (long t0 = 0; t0 < ntile; t0 += g) {
+        const int n = (int)(ntile - t0 < g ? ntile - t0 : g);
+        const long pitch = n * tp;
+        float2* H = (float2*)workspace(WS_PLANE0, (size_t)fnum * pitch * sizeof(float2));
+        float2* A = (float2*)workspace(WS_PLANE1, (size_t)PF * pitch * sizeof(float2));
+        float2* G = (float2*)workspace(WS_PLANE2, (size_t)PF * pitch * sizeof(float2));
+        if (!H || !A || !G) return SB_ERR_NOMEM;
+        float2* cst = nullptr;
+        rc = tile_stats(dyn, nt, fnum, tnum, ntc, (int)t0, n, nullptr, nullptr, 0.0, 0.0,
+                        (double)PF * (double)PT, &cst, st);
+        if (rc) return rc;
+        TileRowLoad ld{dyn, nt, fnum, tnum, ntc, (int)t0, nullptr, nullptr, nullptr};
+        TileHalfStore hs{H, pitch, (int)tp, fnum};
+        SB_ROW_DISPATCH(PT / 2, rc = (launch_row_r2c<float, N1, N2>(ld, hs, (long)n * fnum, st)));
+        if (rc) return rc;
+        // the power sums of acf_cols are not used: each tile's factor comes from its sum d^2
+        rc = acf_cols(H, A, G, pitch, PF, PT, fnum, (int)pitch, sc->acf_part, st);
+        if (rc) return rc;
+        TileAcfRowLoad rl{AcfRowLoad{A, pitch, fnum, PF}, 2 * fnum, (int)tp};
+        TileAcfRowStore rs{AcfRowStore{acf + (size_t)t0 * plane, tnum, PT, nullptr}, 2 * fnum,
+                           plane, cst};
+        SB_ROW_DISPATCH(PT / 2, rc = (launch_row_c2r<float, N1, N2>(rl, rs, 2L * n * fnum, st)));
+        if (rc) return rc;
+    }
+    return SB_OK;
 }
 
 }  // namespace sb

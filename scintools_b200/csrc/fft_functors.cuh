@@ -67,6 +67,69 @@ template <typename C> struct NaturalBStore { // out[y + S k][c] = v: natural ord
     }
 };
 
+// ------------------------------------------ secondary spectrum and ACF (dynspec.cu)
+// secondary spectrum epilogue: |.|^2, fftshift, keep tau >= 0, post-darken, dB
+struct SspecStore {
+    float* sec;
+    int NF, NT, R1;
+    int halve, db;
+    const float* pd1;   // [NT] sin^2 over the shifted fd axis, or null
+    const float* pd2;   // [NF/2] sin^2 over td
+    int noshift;        // 1: natural (un-fftshifted) order, full frame only
+    __device__ __forceinline__ void put(int kf, int cs, float p) const {
+        int row;
+        if (noshift) {
+            row = kf;
+            cs = (cs + NT / 2) & (NT - 1);     // undo the column shift
+        } else if (halve) {
+            if (kf >= NF / 2) return;
+            row = kf;
+        } else {
+            row = (kf + NF / 2) & (NF - 1);
+        }
+        if (pd1) {
+            const float pd = (cs == NT / 2 || row == 0) ? 1.f : pd1[cs] * pd2[row];
+            p = p / pd;
+        }
+        if (db) p = 10.f * log10f(p);
+        sec[(size_t)row * NT + cs] = p;
+    }
+    __device__ __forceinline__ void operator()(int y, int k, int c, float2 v) const {
+        const int kf = y + R1 * k;
+        const float p = v.x * v.x + v.y * v.y;
+        put(kf, (c + NT / 2) & (NT - 1), p);
+        if (c != 0 && c != NT / 2)
+            put((NF - kf) & (NF - 1), ((NT - c) + NT / 2) & (NT - 1), p);
+    }
+};
+
+struct AcfRowLoad {   // output row i <- circular row (i - nf) mod PF
+    const float2* Q;
+    long pitch;
+    int nf, PF;
+    __device__ __forceinline__ float2 operator()(long row, int k) const {
+        const int n = ((int)row - nf + PF) & (PF - 1);
+        return Q[(size_t)n * pitch + k];
+    }
+};
+struct AcfRowStore {
+    float* acf;
+    int nt, PT;
+    const float* scale;    // device scalar written by acf_scale_kernel
+    __device__ __forceinline__ void one(long row, int t, float x, float sc) const {
+        int j;
+        if (t < nt) j = t + nt;
+        else if (t >= PT - nt) j = t - (PT - nt);
+        else return;
+        acf[(size_t)row * (2 * nt) + j] = x * sc;
+    }
+    __device__ __forceinline__ void operator()(long row, int n, float2 z) const {
+        const float sc = *scale;
+        one(row, 2 * n, z.x, sc);
+        one(row, 2 * n + 1, z.y, sc);
+    }
+};
+
 // ------------------------------------------------------------------ chirp-z
 static __global__ void chirp_fill_kernel(float2* w, float2* b, int N, int M) {
     const int n = blockIdx.x * blockDim.x + threadIdx.x;

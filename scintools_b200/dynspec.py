@@ -19,7 +19,8 @@ sb_scint_fit_2d, batched over spectra by get_scint_params_batch), refill (dynspe
 sb_medfilt_masked_f64; the first step of real data, so this is the one piece of cleaning in
 the port), correct_dyn (dynspec.py:3325-3410 -> sb_svd_topk + sb_svd_apply, or the
 sb_bandpass_* passes), scale_dyn('lambda') (dynspec.py:3926-3957 -> sb_scale_dyn_lambda_f32),
-thetatheta_chunks / calc_wavefield / gerchberg_saxton (:1765-1896), and, through
+thetatheta_chunks / calc_wavefield / gerchberg_saxton (:1765-1896), cut_dyn (:3158-3271 ->
+sb_sspec_tiles_f32 + sb_acf_tiles_f32, every tile in one batched pass), and, through
 ``arcfit.ArcFitMixin``, norm_sspec / fit_arc (:1920-2183, :970-1346).
 
 Provenance: ``prep_thetatheta`` is the reference's dynspec.py:1348-1537 with the
@@ -739,6 +740,28 @@ def _scint_finish(ds, results, method, alpha, verbose, get_fit_report):
             print("phase grad:\t\t{val} +/- {err}".format(val=ds.phasegrad, err=err))
 
 
+def _cut_dyn_device(dyn, fnum, tnum, nfc, ntc, dtype):
+    """Secondary spectra [nfc][ntc][nrfft/2][ncfft] and ACFs [nfc][ntc][2 fnum][2 tnum] of
+    the fnum x tnum tiles of dyn [nfc fnum][ntc tnum] (Dynspec.cut_dyn), as dtype."""
+    import torch
+    nrfft = int(2 ** (np.ceil(np.log2(fnum)) + 1))
+    ncfft = int(2 ** (np.ceil(np.log2(tnum)) + 1))
+    chan_window, subint_window = get_window(tnum, fnum, window='hanning', frac=0.1)
+    d = D.upload_f32(dyn)
+    wt = D.upload(chan_window.astype(np.float32))
+    wf = D.upload(subint_window.astype(np.float32))
+    sec = D.empty((nfc, ntc, nrfft // 2, ncfft), torch.float32)
+    acf = D.empty((nfc, ntc, 2 * fnum, 2 * tnum), torch.float32)
+    _lib.check(_lib.lib.sb_sspec_tiles_f32(
+        d.data_ptr(), nfc * fnum, ntc * tnum, fnum, tnum, nfc, ntc, wt.data_ptr(),
+        wf.data_ptr(), float(chan_window.sum()), float(subint_window.sum()), sec.data_ptr(),
+        D.stream_ptr()))
+    _lib.check(_lib.lib.sb_acf_tiles_f32(
+        d.data_ptr(), nfc * fnum, ntc * tnum, fnum, tnum, nfc, ntc, acf.data_ptr(),
+        D.stream_ptr()))
+    return D.download(sec, dtype), D.download(acf, dtype)
+
+
 class BasicDyn:
     """Container with the attributes Dynspec.load_dyn_obj reads
     (dynspec.py:4146-4230)."""
@@ -1173,6 +1196,47 @@ class Dynspec(ArcFitMixin):
             self.acf = arr
         else:
             return arr
+
+    def cut_dyn(self, tcuts=0, fcuts=0, plot=False, filename=None, dpi=200, lamsteps=False,
+                maxfdop=np.inf, figsize=(8, 13), display=True, dtype=np.float64):
+        """Cut the dynamic spectrum into (fcuts+1) x (tcuts+1) tiles (reference
+        dynspec.py:3158-3271) and transform every tile in one batched pass
+        (sb_sspec_tiles_f32, sb_acf_tiles_f32).
+
+        fnum = floor(len(freqs) / (fcuts+1)) channels by tnum = floor(len(times) / (tcuts+1))
+        subintegrations per tile; trailing rows and columns that do not fill a tile are
+        dropped.  Tile (ii, jj) is self.dyn[ii*fnum:(ii+1)*fnum, jj*tnum:(jj+1)*tnum].  Sets
+        - self.cutdyn [fcuts+1][tcuts+1][fnum][tnum] (float64, the tiles themselves);
+        - self.cutsspec [fcuts+1][tcuts+1][nrfft/2][ncfft]: each tile's
+          calc_sspec(input_dyn=tile, lamsteps=lamsteps) (Hanning window, halved, dB);
+        - self.cutacf [fcuts+1][tcuts+1][2 fnum][2 tnum]: each tile's calc_acf(input_dyn=tile)
+          (no mean subtracted, normalised by its zero lag).  The reference computes these
+          ACFs and discards them; they are kept because a per-tile scintillation fit needs them.
+        A NaN makes its own tile NaN and no other.  lamsteps changes no array; as in the
+        reference, it needs self.dlam (AttributeError otherwise).  dtype=np.float32 skips
+        the widening of cutsspec and cutacf.
+
+        Errors, raised before any device work: NotImplementedError for plot=True;
+        ValueError for a tile outside the sizes the single-spectrum drivers accept
+        (fnum 2..32768, tnum 5..16384; the reference accepts smaller tiles)."""
+        if plot:
+            raise NotImplementedError("plotting is outside the GPU hot path")
+        if lamsteps:
+            self.dlam       # the reference's calc_sspec reads it here
+        nchan, nsub = len(self.freqs), len(self.times)
+        nfc, ntc = int(fcuts) + 1, int(tcuts) + 1
+        fnum, tnum = nchan // nfc, nsub // ntc
+        if not (_ACF_MIN_NF <= fnum <= _ACF_MAX_NF and _ACF_MIN_NT <= tnum <= _ACF_MAX_NT):
+            raise ValueError("cut_dyn: tiles of %d x %d are outside the supported sizes "
+                             "(fnum %d..%d, tnum %d..%d)" % (fnum, tnum, _ACF_MIN_NF, _ACF_MAX_NF,
+                                                              _ACF_MIN_NT, _ACF_MAX_NT))
+        dyn = np.asarray(self.dyn)[:nfc * fnum, :ntc * tnum]
+        if dyn.shape != (nfc * fnum, ntc * tnum):
+            raise ValueError("cut_dyn: self.dyn %s is smaller than freqs x times" %
+                             (np.shape(self.dyn),))
+        self.cutdyn = dyn.reshape(nfc, fnum, ntc, tnum).transpose(0, 2, 1, 3).astype(np.float64)
+        self.cutsspec, self.cutacf = _cut_dyn_device(dyn, fnum, tnum, nfc, ntc, dtype)
+        np.seterr(divide='ignore')      # calc_sspec's side effect (:3720)
 
     # ------------------------------------------------------------------
     # scintillation scales (csrc/scintfit.cu)
