@@ -13,8 +13,13 @@
  *  - 2-D arrays are C-contiguous (row-major); complex = interleaved
  *    (re, im) float pairs; dyn is [freq][time] like Dynspec.dyn;
  *  - one CUDA context per process, calls into one device from one host
- *    thread at a time (the library keeps a grow-only scratch workspace per
- *    process; sb_release() frees it).  Not fork-safe (CUDA is not).
+ *    thread at a time (the library keeps a grow-only scratch workspace and
+ *    twiddle tables per process; sb_release() frees them).  Not fork-safe
+ *    (CUDA is not).
+ *  - calls may use different streams.  The library orders each call after the
+ *    previous one: a call on another stream than the previous call's waits on
+ *    the device for that call's work, so the shared workspace never sees two
+ *    calls at once.  sb_convert_* touch only caller buffers and are not ordered.
  *  - sm_90a (H100) only; there is no CPU fallback.
  */
 #ifndef SCINT_B200_H
