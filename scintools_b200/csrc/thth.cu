@@ -718,13 +718,17 @@ int sweep_batch(size_t per_item, int count, int cap) {
 }
 
 static bool lower_check_needed(const ThthGeom& g, const double* th_host) {
-    // worst case fd argument over all (i, j): min(th) - max(th)
+    // The fd argument th1 - th2 spans [-(max(th) - min(th)), max(th) - min(th)]; the
+    // smallest fd_inv comes from the negative end on an ascending fd axis and from the
+    // positive end on a descending one (dfd < 0), so take the smaller of the two.
     double tmin = th_host[0], tmax = th_host[0];
     for (int k = 1; k < g.n; ++k) {
         tmin = th_host[k] < tmin ? th_host[k] : tmin;
         tmax = th_host[k] > tmax ? th_host[k] : tmax;
     }
-    double worst = floor(((tmin - tmax) - g.fd0 + g.half_dfd) / g.dfd) - 2.0;
+    const double lo = floor(((tmin - tmax) - g.fd0 + g.half_dfd) / g.dfd);
+    const double hi = floor(((tmax - tmin) - g.fd0 + g.half_dfd) / g.dfd);
+    const double worst = (lo < hi ? lo : hi) - 2.0;
     return !(worst >= -(double)g.nfd);
 }
 

@@ -481,12 +481,28 @@ def _search_launch(params, staged, pinned=False):
     time_v = U.value(time, "s")
     freq_v = U.value(freq, "MHz")
     etas_v = U.value(etas, "s3")
+    try:
+        theta_centres(U.value(edges, "mHz"))
+    except ValueError:
+        # every thth_map raises (the recentring ties on an even grid); the reference's eta
+        # loop stores NaN for each curvature
+        return _NanSweep(np.atleast_1d(etas_v).shape[0]), params, time_v, freq_v, etas_v
     fd = U.value(fft_axis(time_v, "mHz", npad), "mHz")
     tau = U.value(fft_axis(freq_v, "us", npad), "us")
     cs = conjugate_spectrum(dspec2, npad, None, tau, tauMask,
                             ncols_keep=needed_fd_columns(fd, edges))
     job = _sweep_launch(cs, tau, fd, etas_v, edges, bool(coher), pinned=pinned)
     return job, params, time_v, freq_v, etas_v
+
+
+class _NanSweep:
+    """The eigenvalues of a sweep that fails at every curvature."""
+
+    def __init__(self, neta):
+        self.neta = neta
+
+    def finish(self):
+        return np.full(self.neta, np.nan)
 
 
 def _search_finish(launched):
@@ -705,12 +721,64 @@ def _c64(t):
     return a[..., 0].astype(np.float64) + 1j * a[..., 1].astype(np.float64)
 
 
+def _hist_edges(tau, fd):
+    """The np.histogram2d bin edges of rev_map (ththmod.py:211-216), (fd, tau).  Raises
+    numpy's ValueError when either descends, as the reference's rev_map does for a
+    descending tau or fd axis (a BasicDyn with descending frequencies, say)."""
+    tau, fd = U.value(tau, "us"), U.value(fd, "mHz")
+    fe = (np.linspace(0, fd.shape[0], fd.shape[0] + 1) - .5) * (fd[1] - fd[0]) + fd[0]
+    te = (np.linspace(0, tau.shape[0], tau.shape[0] + 1) - .5) * (tau[1] - tau[0]) + tau[0]
+    for k, e in enumerate((fe, te)):
+        if np.any(e[:-1] > e[1:]):
+            raise ValueError("`bins[%d]` must be monotonically increasing, when an array" % k)
+    return fe, te
+
+
+def _index_error(th, tau, fd, eta):
+    """Does thth_map raise IndexError (fd_inv < -nfd on a point of the pnts mask,
+    ththmod.py:94-104) at curvature eta?  The reference's expressions on the host, a
+    block of rows at a time; for the error paths of non-ascending axes, where the
+    device sweeps that report it cannot run."""
+    tau, fd = np.asarray(tau, dtype=np.float64), np.asarray(fd, dtype=np.float64)
+    dtau, dfd = np.diff(tau).mean(), np.diff(fd).mean()
+    for r0 in range(0, th.shape[0], 256):
+        th2 = th[r0:r0 + 256, np.newaxis]
+        fd_inv = (((th[np.newaxis, :] - th2) - fd[0] + dfd / 2) // dfd).astype(int)
+        tau_inv = (((eta * (th[np.newaxis, :] ** 2 - th2 ** 2)) - tau[0] + dtau / 2)
+                   // dtau).astype(int)
+        pnts = (tau_inv > 0) * (tau_inv < tau.shape[0]) * (fd_inv < fd.shape[0])
+        if np.any(pnts & (fd_inv < -fd.shape[0])):
+            return True
+    return False
+
+
+def _check_rev_axes(tau, fd, edges, eta):
+    """Before any device work of an entry point whose reference ends in rev_map
+    (chisq_calc, VLBI_chunk_retrieval): on a descending axis raise what the reference
+    raises first -- IndexError from thth_map, the crop's exception from thth_redmap,
+    else rev_map's ValueError.  (A zero theta-theta matrix, whose eigsh error would come
+    before rev_map's, also gives the ValueError.)"""
+    tau, fd = U.value(tau, "us"), U.value(fd, "mHz")
+    try:
+        _hist_edges(tau, fd)
+    except ValueError:
+        th = theta_centres(U.value(edges, "mHz"))
+        if _index_error(th, tau, fd, eta):
+            raise IndexError("theta-theta point maps outside the conjugate "
+                             "spectrum (fd_inv < -nfd)") from None
+        _, errs = _rev_centres(th, tau, fd, np.array([eta]), min_crop=0)
+        if errs[0] is not None:
+            raise errs[0] from None
+        raise
+
+
 def _rev_map_device(thth_dev, n, tau, fd, eta, edges, hermetian):
     """sb_rev_map on a device theta-theta matrix; returns the device recov
     [ntau][nfd][2] (= the reference's ``recov.T`` before any host copy)."""
     import torch
     tau = U.value(tau, "us")
     fd = U.value(fd, "mHz")
+    _hist_edges(tau, fd)
     th = theta_centres(U.value(edges, "mHz"))
     if th.shape[0] != n:
         raise ValueError("thth is %d x %d but edges give %d centres" % (n, n, th.shape[0]))
@@ -731,7 +799,8 @@ def rev_map(thth, tau, fd, eta, edges, hermetian=True):
     n = thth.shape[0]
     if thth.ndim != 2 or thth.shape[1] != n:
         raise ValueError("thth must be square")
-    recov = _c64(_rev_map_device(D.upload_f32(thth.astype(np.complex128)), n, tau, fd, eta,
+    _hist_edges(tau, fd)
+    recov =_c64(_rev_map_device(D.upload_f32(thth.astype(np.complex128)), n, tau, fd, eta,
                                  edges, hermetian))
     if not hermetian:
         # the (0, 0) bin holds the zero-Jacobian diagonal points: NaN real part,
@@ -739,12 +808,10 @@ def rev_map(thth, tau, fd, eta, edges, hermetian=True):
         with np.errstate(divide="ignore", invalid="ignore"):
             h = np.sum(np.diagonal(thth).imag / 0.0)
         if np.isinf(h):
-            tauv, fdv = U.value(tau, "us"), U.value(fd, "mHz")
-            fe = (np.linspace(0, fdv.shape[0], fdv.shape[0] + 1) - .5) * (fdv[1] - fdv[0]) + fdv[0]
-            te = (np.linspace(0, tauv.shape[0], tauv.shape[0] + 1) - .5) * (tauv[1] - tauv[0]) + tauv[0]
+            fe, te = _hist_edges(tau, fd)
             bx = np.searchsorted(fe, 0.0, side="right") - 1
             by = np.searchsorted(te, 0.0, side="right") - 1
-            if 0 <= bx < fdv.shape[0] and 0 <= by < tauv.shape[0]:
+            if 0 <= bx < fe.shape[0] - 1 and 0 <= by < te.shape[0] - 1:
                 recov[by, bx] = np.nan_to_num(complex(0.0, h))
     return recov
 
@@ -867,6 +934,7 @@ def _chisq_run(dspec, CS, tau, fd, etas, edges, mask, tol, max_iter):
     d = np.asarray(dspec)
     if d.ndim != 2:
         raise ValueError("dspec must be 2-D, got shape %r" % (d.shape,))
+    _hist_edges(tau, fd)
     if mask is not None:
         mask = np.asarray(mask, dtype=bool)
         if mask.shape != d.shape:
@@ -905,7 +973,9 @@ def chisq_sweep(dspec, CS, tau, fd, etas, edges, N, mask=None, return_info=False
     (an array ``N`` broadcasts as in numpy: shape (len(etas),) + N.shape), NaN
     where chisq_calc would raise.  ``return_info`` adds a dict with the top
     eigenvalues ``w``, the SB_ETA_* ``status`` bits, the cropped sizes ``nred``
-    and the Lanczos ``iters``.  ``CS`` may be a numpy array or a DeviceCS."""
+    and the Lanczos ``iters``.  ``CS`` may be a numpy array or a DeviceCS.  A descending
+    tau or fd axis raises ValueError (every chisq_calc on it would raise) before any
+    device work."""
     ssq, info, errs = _chisq_run(dspec, CS, tau, fd, etas, edges, mask, tol, max_iter)
     ssq[(info["status"] & 8) != 0] = np.nan        # ArpackNoConvergence in the reference
     ssq[[e is not None for e in errs]] = np.nan
@@ -921,6 +991,7 @@ def chisq_calc(dspec, CS, tau, fd, eta, edges, N, mask=None):
     (ththmod.py:330-368): np.sum((model - dspec)[mask] ** 2) / N with model =
     modeler(...)[3][:dspec.shape[0], :dspec.shape[1]].  ``mask`` defaults to
     np.isfinite(dspec).  Raises where the reference raises."""
+    _check_rev_axes(tau, fd, edges, float(U.value(eta, "s3")))
     ssq, info, errs = _chisq_run(dspec, CS, tau, fd, np.array([float(U.value(eta, "s3"))]),
                                  edges, mask, 0.0, 0)
     st = int(info["status"][0])
@@ -972,6 +1043,7 @@ def _vlbi_run(dspec2_list, edges, time, freq, eta, npad, n_dish, tauMask, tol=0.
     fd = U.value(fft_axis(time_v, "mHz", npad), "mHz")
     tau = U.value(fft_axis(freq_v, "us", npad), "us")
     tm = float(U.value(tauMask, "us"))
+    _check_rev_axes(tau, fd, edges, eta_v)
     autos = _vlbi_auto_indices(n_dish)
     cs_list = [conjugate_spectrum(d, npad, None if k in autos else 0.0, tau, tm, half=False)
                for k, d in enumerate(dl)]
@@ -1004,8 +1076,8 @@ def VLBI_chunk_retrieval(params):
     wavefields.  Raises where the reference raises: IndexError when the theta grid
     reaches past the fd axis, scipy's ArpackError when every spectrum is zero,
     IndexError (0 or 1) or ValueError (2) when the crop keeps fewer than 3 theta
-    centres.  ValueError for a list length other than n_dish (n_dish + 1) / 2,
-    mismatched shapes or non-finite input."""
+    centres, rev_map's ValueError on a descending tau or fd axis.  ValueError for a list
+    length other than n_dish (n_dish + 1) / 2, mismatched shapes or non-finite input."""
     (dspec2_list, edges, time, freq, eta, idx_t, idx_f, npad, n_dish, tauMask,
      verbose) = params
     if verbose:
@@ -1068,7 +1140,7 @@ def asymmetry_batch(params_list, return_info=False, tol=0.0, max_iter=0):
     arbitrary global phase)."""
     import torch
     params_list = list(params_list)
-    prep, groups = [], {}
+    prep, groups, failed = [], {}, {}
     for k, p in enumerate(params_list):
         dspec2, edges, time, freq, eta, idx_t, idx_f, npad, verbose = p
         d = np.asarray(dspec2, dtype=np.float64)
@@ -1079,6 +1151,11 @@ def asymmetry_batch(params_list, return_info=False, tol=0.0, max_iter=0):
         NF, NT = (npad + 1) * d.shape[0], (npad + 1) * d.shape[1]
         prep.append((d, ev, U.value(time, "s"), U.value(freq, "MHz"),
                      float(U.value(eta, "s3")), npad))
+        try:
+            theta_centres(ev)
+        except ValueError as e:     # thth_map raises in the reference's try: NaN
+            failed[k] = str(e)
+            continue
         groups.setdefault((NF, NT, len(ev) - 1), []).append(k)
     for NF, NT, n_th in groups:
         _asym_check_sizes(NF, NT, n_th)
@@ -1122,6 +1199,16 @@ def asymmetry_batch(params_list, return_info=False, tol=0.0, max_iter=0):
         idx_t, idx_f, verbose = p[5], p[6], p[8]
         st = int(info["status"][k])
         msg = [m for bit, m in _ASYM_FAILURES if st & bit]
+        if k in failed:
+            msg = [failed[k]]
+        elif not msg:
+            # the reference's modeler ends in rev_map, which raises on a descending axis
+            _, _, time_v, freq_v, _, npad = prep[k]
+            try:
+                _hist_edges(fft_axis(freq_v, "us", npad), fft_axis(time_v, "mHz", npad))
+            except ValueError as e:
+                msg = [str(e)]
+                asym[k] = np.nan
         if msg:
             print(msg[0], flush=True)
         elif verbose:       # 0 / 0 (no weight off the centre element) is NaN without an error
