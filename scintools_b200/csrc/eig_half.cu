@@ -21,7 +21,7 @@
 //     triangle in one extra pass (second order in the vector error);
 //   * safety net: the same fp32 pass yields the true residual
 //     ||A y - rho y|| / |rho|; above rtol_r (1e-3) the solve continues as a plain
-//     fp32 Lanczos started from y with the stopping rule of thth_eig_kernel.
+//     fp32 Lanczos started from y, the loop of thth_eig_kernel (thth_lanczos).
 // Failure modes / status bits as thth_eig_kernel (NaN where the reference's
 // try/except stores NaN).
 #ifndef SB_HOST_EMU
@@ -31,14 +31,12 @@
 #include <math.h>
 #include <stdlib.h>
 
+#include "../../include/scint_b200.h"   // SB_ETA_* status bits, tests/host_emu too
 #include "drivers.cuh"
 #include "lanczos.cuh"
 #include "tma.cuh"
 
 namespace sb {
-
-enum { EB_ST_INDEX_ERROR = 1, EB_ST_ZERO_START = 2, EB_ST_TOO_SMALL = 4,
-       EB_ST_NOT_CONVERGED = 8 };
 
 constexpr int EB_THREADS = 256;
 constexpr int EB_NW = EB_THREADS / 32;
@@ -206,14 +204,14 @@ thth_eig_half_kernel(const float2* __restrict__ Mbase, const unsigned* __restric
     float2* basis = gbasis + (size_t)e * EB_SLOTS * ld;
     const double qnan = __longlong_as_double(0x7ff8000000000000LL);
 
-    if (status[eta0 + e] & EB_ST_INDEX_ERROR) {
+    if (status[eta0 + e] & SB_ETA_INDEX_ERROR) {
         if (tid == 0) { eigs[eta0 + e] = qnan; iters[eta0 + e] = 0; }
         return;
     }
     if (n < 3) {
         if (tid == 0) {
             eigs[eta0 + e] = qnan; iters[eta0 + e] = 0;
-            status[eta0 + e] |= EB_ST_TOO_SMALL;
+            status[eta0 + e] |= SB_ETA_TOO_SMALL;
         }
         return;
     }
@@ -440,44 +438,17 @@ thth_eig_half_kernel(const float2* __restrict__ Mbase, const unsigned* __restric
             phbits ^= 1u << st;
             const float4* sg = reinterpret_cast<const float4*>(mystage + st * 4096);
             float rx = 0.f, ry = 0.f;
-            const int jskip = first4 >> 5;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                if (j < jskip) continue;
-                const int c4 = lane + 32 * j;
-                float4 q = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (c4 >= first4 && c4 < ncol4) q = sg[c4];
-                const float4 x = (2 * c4 < ld) ? *reinterpret_cast<const float4*>(v + 2 * c4)
-                                               : make_float4(0.f, 0.f, 0.f, 0.f);
-                rx = fmaf(q.x, x.x, rx); rx = fmaf(-q.y, x.y, rx);
-                rx = fmaf(q.z, x.z, rx); rx = fmaf(-q.w, x.w, rx);
-                ry = fmaf(q.x, x.y, ry); ry = fmaf(q.y, x.x, ry);
-                ry = fmaf(q.z, x.w, ry); ry = fmaf(q.w, x.z, ry);
-                yc[j].x = fmaf(q.x, xa.x, yc[j].x); yc[j].x = fmaf(q.y, xa.y, yc[j].x);
-                yc[j].y = fmaf(q.x, xa.y, yc[j].y); yc[j].y = fmaf(-q.y, xa.x, yc[j].y);
-                yc[j].z = fmaf(q.z, xa.x, yc[j].z); yc[j].z = fmaf(q.w, xa.y, yc[j].z);
-                yc[j].w = fmaf(q.z, xa.y, yc[j].w); yc[j].w = fmaf(-q.w, xa.x, yc[j].w);
-            }
+            thth_row_fma([&](int, int c4) {
+                return (c4 >= first4 && c4 < ncol4) ? sg[c4] : make_float4(0.f, 0.f, 0.f, 0.f);
+            }, v, ld, 0, first4 >> 5, xa, rx, ry, yc);
             __syncwarp();
             if (lane == 0 && k + EB_NST < K) issue(k + EB_NST);
             rx = warp_sum(rx);
             ry = warp_sum(ry);
             if (lane == 0) w[a] = make_float2(rx, ry);
         }
-        __syncthreads();
-        if (worker) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-                *reinterpret_cast<float4*>(part + warp * 512 + 2 * (lane + 32 * j)) = yc[j];
-        }
-        __syncthreads();
-        for (int c = tidw; c < 512; c += EB_THREADS) {
-            float sx = 0.f, sy = 0.f;
-#pragma unroll
-            for (int kk = 0; kk < EB_NW; ++kk) { sx += part[kk * 512 + c].x; sy += part[kk * 512 + c].y; }
-            if (c < ld) u[c] = make_float2(sx, sy);
-        }
-        __syncthreads();
+        __syncthreads();        // part aliases the stages of other warps
+        thth_fold_columns<EB_NW>(yc, part, u, 0, ld);
         // fp32 rows may leave any bit pattern behind: the fp16 passes need zeros
         for (int i = tidw; i < EB_NW * WSL / 16; i += EB_THREADS)
             reinterpret_cast<float4*>(ring)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -485,71 +456,18 @@ thth_eig_half_kernel(const float2* __restrict__ Mbase, const unsigned* __restric
         __syncthreads();
     };
 
-    // ------------------------------------------------------------------
-    // Lanczos from the normalised vector in v (vp = 0).  lanczos_b: iterate on
-    // the fp16 triangle and keep the basis; returns false if the basis slots ran
-    // out.  S.done / S.theta / m describe the outcome.
-    // ------------------------------------------------------------------
     int m = 0;
     int mv = 0;                                 // mat-vecs done (reported as iters)
-    auto lanczos_init = [&]() {
-        if (tid == 0) {
-            S.done = 0; S.lo = 0.0; S.theta = 0.0; S.res = 0.0;
-            S.next_check = 1; S.m_last = 0; S.beta2[0] = 0.0;
-        }
-        __syncthreads();
-    };
-    // alpha, the new (unnormalised) Lanczos vector in w and beta of step `it`
-    auto step_scalars = [&](int it, float beta_prev, double& alpha, double& beta) {
-        double apart = 0.0;
-        for (int c = tidw; c < n; c += EB_THREADS) {
-            float2 x = w[c];
-            x.x += u[c].x;
-            x.y += u[c].y;
-            w[c] = x;
-            apart += (double)(v[c].x * x.x + v[c].y * x.y);
-        }
-        apart = warp_sum(apart);
-        if (lane == 0) S.red[0][warp] = apart;
-        __syncthreads();
-        alpha = 0.0;
-        for (int k = 0; k < EB_NW; ++k) alpha += S.red[0][k];
-        const float af = (float)alpha;
-        double bpart = 0.0;
-        for (int c = tidw; c < n; c += EB_THREADS) {
-            float2 x = w[c];
-            x.x -= af * v[c].x + beta_prev * vp[c].x;
-            x.y -= af * v[c].y + beta_prev * vp[c].y;
-            w[c] = x;
-            bpart += (double)x.x * x.x + (double)x.y * x.y;
-        }
-        bpart = warp_sum(bpart);
-        if (lane == 0) S.red[1][warp] = bpart;
-        __syncthreads();
-        double b2 = 0.0;
-        for (int k = 0; k < EB_NW; ++k) b2 += S.red[1][k];
-        beta = sqrt(b2);
-        if (tid == 0) { S.alpha[it] = alpha; S.beta[it + 1] = beta; S.beta2[it + 1] = b2; }
-        __syncthreads();
-    };
-    auto rotate = [&](double beta) {
-        const float ib = (float)(1.0 / beta);
-        for (int c = tidw; c < n; c += EB_THREADS) {
-            const float2 x = w[c];
-            vp[c] = v[c];
-            v[c] = make_float2(x.x * ib, x.y * ib);
-        }
-        __syncthreads();
-    };
     // ------------------------------------------------------------------
     // fp16 Lanczos from the normalised vector in v (vp = 0), basis kept.  The
     // convergence check of the tridiagonal T_it runs on warp CHKW DURING mat-vec it
     // (one step late), so nobody idles behind its Sturm sweeps; when it reports
     // convergence the step just taken is surplus and m = it.  Returns false if
-    // the basis slots ran out.
+    // the basis slots ran out.  S.done / S.theta / m describe the outcome.
     // ------------------------------------------------------------------
     auto lanczos_b = [&](double et) -> bool {
-        lanczos_init();
+        lanczos_reset(S);
+        __syncthreads();
         float beta_prev = 0.f;
         m = 0;
         for (int it = 0; it < max_iter; ++it) {
@@ -559,7 +477,7 @@ thth_eig_half_kernel(const float2* __restrict__ Mbase, const unsigned* __restric
             matvec_t(chk ? it : 0, et);
             ++mv;
             double alpha, beta;
-            step_scalars(it, beta_prev, alpha, beta);
+            lanczos_step<EB_NW>(S, it, n, v, vp, w, u, beta_prev, alpha, beta);
             if (chk && S.done) { m = it; break; }
             m = it + 1;
             if (it + 1 == max_iter || !(beta > 0.0)) {      // last word: check T_m now
@@ -568,61 +486,22 @@ thth_eig_half_kernel(const float2* __restrict__ Mbase, const unsigned* __restric
                 break;
             }
             if (!isfinite(alpha)) break;
-            rotate(beta);
+            lanczos_rotate<EB_NW>(v, vp, w, n, beta);
             beta_prev = (float)beta;
         }
         return true;
     };
-    // plain fp32 Lanczos (restart / continuation), check after every step as thth_eig_kernel
+    // plain fp32 Lanczos (restart / continuation): thth_eig_kernel's loop on matvec_f
     auto lanczos_f = [&](double et) {
-        lanczos_init();
-        float beta_prev = 0.f;
-        m = 0;
-        for (int it = 0; it < max_iter; ++it) {
-            matvec_f();
-            ++mv;
-            double alpha, beta;
-            step_scalars(it, beta_prev, alpha, beta);
-            m = it + 1;
-            const bool last = (it + 1 == max_iter);
-            if (warp == 0 && (m >= S.next_check || last || !(beta > 0.0)))
-                lanczos_check(S, m, tol, et);
-            __syncthreads();
-            if (S.done || !isfinite(alpha)) break;
-            rotate(beta);
-            beta_prev = (float)beta;
-        }
+        m = thth_lanczos<EB_NW>(S, matvec_f, v, vp, w, u, n, max_iter, tol, et);
+        mv += m;
     };
-
-    // v0 = row n//2 of the Hermitian matrix (ththmod.py:398-399), from the fp32 triangle
-    auto start_vector = [&]() -> bool {
-        const int h = n / 2;
-        double part0 = 0.0;
-        for (int c = tidw; c < ld; c += EB_THREADS) {
-            float2 x = make_float2(0.f, 0.f);
-            if (c < n && c > h) x = M[(size_t)h * ld + c];
-            else if (c < h) { x = M[(size_t)c * ld + h]; x.y = -x.y; }
-            v[c] = x;
-            vp[c] = make_float2(0.f, 0.f);
-            part0 += (double)x.x * x.x + (double)x.y * x.y;
-        }
-        part0 = warp_sum(part0);
-        __syncthreads();
-        if (lane == 0) S.red[0][warp] = part0;
-        __syncthreads();
-        double nrm2 = 0.0;
-        for (int k = 0; k < EB_NW; ++k) nrm2 += S.red[0][k];
-        if (!(nrm2 > 0.0) || !isfinite(nrm2)) return false;
-        const float s = (float)(1.0 / sqrt(nrm2));
-        for (int c = tidw; c < ld; c += EB_THREADS) { v[c].x *= s; v[c].y *= s; }
-        __syncthreads();
-        return true;
-    };
+    auto start_vector = [&]() { return thth_start_vector<EB_NW>(M, ld, n, v, vp, S.red[0]); };
 
     if (!start_vector()) {
         if (tid == 0) {
             eigs[eta0 + e] = qnan; iters[eta0 + e] = 0;
-            status[eta0 + e] |= EB_ST_ZERO_START;
+            status[eta0 + e] |= SB_ETA_ZERO_START;
         }
         return;
     }
@@ -632,25 +511,9 @@ thth_eig_half_kernel(const float2* __restrict__ Mbase, const unsigned* __restric
         start_vector();
         lanczos_f(etol);
     } else if (S.done) {
-        // ---- Ritz vector of T_m at theta (backward recurrence, grows towards s_0),
-        // y = sum_j s_j q_j, eigenvalue = Rayleigh quotient with the fp32 triangle
-        if (tid == 0) {
-            const double theta = S.theta;
-            double* s = S.piv;
-            s[m - 1] = 1.0;
-            if (m >= 2) s[m - 2] = (S.beta[m - 1] != 0.0) ? (theta - S.alpha[m - 1]) / S.beta[m - 1] : 0.0;
-            for (int i = m - 2; i >= 1; --i) {
-                const double t = (theta - S.alpha[i]) * s[i] - S.beta[i + 1] * s[i + 1];
-                s[i - 1] = (S.beta[i] != 0.0) ? t / S.beta[i] : 0.0;
-                if (fabs(s[i - 1]) > 1e150)
-                    for (int k = i - 1; k < m; ++k) s[k] *= 1e-150;
-            }
-            double nn = 0.0;
-            for (int i = 0; i < m; ++i) nn += s[i] * s[i];
-            nn = 1.0 / sqrt(nn);
-            for (int i = 0; i < m; ++i) s[i] *= nn;
-        }
-        __syncthreads();
+        // ---- Ritz vector y = sum_j s_j q_j of T_m at theta, eigenvalue = Rayleigh
+        // quotient with the fp32 triangle
+        lanczos_ritz(S, m);
         for (int c = tidw; c < ld; c += EB_THREADS) {
             float sx = 0.f, sy = 0.f;
             if (c < n) {
@@ -689,11 +552,7 @@ thth_eig_half_kernel(const float2* __restrict__ Mbase, const unsigned* __restric
             const double rx = (double)w[c].x - rho * v[c].x, ry = (double)w[c].y - rho * v[c].y;
             rpart += rx * rx + ry * ry;
         }
-        rpart = warp_sum(rpart);
-        if (lane == 0) S.red[0][warp] = rpart;
-        __syncthreads();
-        double r2 = 0.0;
-        for (int k = 0; k < EB_NW; ++k) r2 += S.red[0][k];
+        const double r2 = cta_sum<EB_NW>(rpart, S.red[0]);
         const bool accept = (sd > 0.0) && isfinite(rho) &&
                             (r2 <= rtol_r * rtol_r * rho * rho * sd);
         __syncthreads();
@@ -715,7 +574,7 @@ thth_eig_half_kernel(const float2* __restrict__ Mbase, const unsigned* __restric
     if (plain && tid == 0) {
         eigs[eta0 + e] = fabs(S.theta);
         iters[eta0 + e] = mv;
-        if (!S.done) status[eta0 + e] |= EB_ST_NOT_CONVERGED;
+        if (!S.done) status[eta0 + e] |= SB_ETA_NOT_CONVERGED;
     }
 }
 

@@ -1,8 +1,11 @@
-// Lanczos bookkeeping shared by the square (thth.cu) and the thin (thin.cu)
-// theta-theta solvers: tridiagonal storage, division-free Sturm counts, warp
-// multisection for the top Ritz values and the residual / gap stopping rule.
+// Lanczos pieces shared by the fp32 Lanczos solvers (thth_eig_kernel in thth.cu,
+// thth_eig_half_kernel in eig_half.cu, thin_sv_kernel in thin.cu, herm_eigvec_body in
+// retrieval.cu): tridiagonal storage and its reset, the CTA sum, the three-term step and
+// the rotation, division-free Sturm counts, warp multisection for the top Ritz values, the
+// residual / gap stopping rule and the Ritz coefficients.
 #pragma once
 #include <float.h>
+#include <limits.h>
 
 #include "common.cuh"
 
@@ -26,6 +29,83 @@ struct alignas(16) LanczosShared {
     int reserved2;
     int m_last;              // lanczos_check: step of the previous check (0: none)
 };
+
+// State of a new run: not converged, first check after step 1.  Written by thread 0; the
+// caller's next barrier publishes it.
+__device__ __forceinline__ void lanczos_reset(LanczosShared& S) {
+    if (threadIdx.x == 0) {
+        S.done = 0; S.lo = 0.0; S.theta = 0.0; S.res = 0.0;
+        S.next_check = 1; S.m_last = 0; S.beta2[0] = 0.0;
+    }
+}
+
+// First index of this thread in a loop strided over the threads of the first NW warps.
+// Threads past them (eig_half.cu's check warp) start beyond every bound: their loops are empty.
+template <int NW>
+__device__ __forceinline__ int lanczos_first() {
+    return threadIdx.x < NW * 32 ? (int)threadIdx.x : INT_MAX;
+}
+
+// fp64 sum of x over the first NW warps of the CTA, in a fixed order: warp_sum, then the
+// warps 0 .. NW-1 through red[warp].  Every thread calls it (it holds a barrier) and gets
+// the sum.  A barrier must separate it from the last read of red by an earlier sum.
+template <int NW>
+__device__ __forceinline__ double cta_sum(double x, double* red) {
+    x = warp_sum(x);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = x;
+    __syncthreads();
+    double s = 0.0;
+    for (int k = 0; k < NW; ++k) s += red[k];
+    return s;
+}
+
+// Step `it` of the three-term recurrence on fp32 vectors of length n, sums in fp64, once the
+// mat-vec has left A v in w -- plus the column sums u of the triangle solvers, added first
+// (null: none): alpha = Re <v, A v>, w = A v - alpha v - beta_prev vp, beta = ||w||, all
+// three recorded in S.  Ends with a barrier.
+template <int NW>
+__device__ __forceinline__ void lanczos_step(LanczosShared& S, int it, int n, const float2* v,
+                                             const float2* vp, float2* w, const float2* u,
+                                             float beta_prev, double& alpha, double& beta) {
+    const int c0 = lanczos_first<NW>();
+    double apart = 0.0;
+    for (int c = c0; c < n; c += NW * 32) {
+        float2 x = w[c];
+        if (u) {
+            x.x += u[c].x;
+            x.y += u[c].y;
+            w[c] = x;
+        }
+        apart += (double)(v[c].x * x.x + v[c].y * x.y);
+    }
+    alpha = cta_sum<NW>(apart, S.red[0]);
+    const float af = (float)alpha;
+    double bpart = 0.0;
+    for (int c = c0; c < n; c += NW * 32) {
+        float2 x = w[c];
+        x.x -= af * v[c].x + beta_prev * vp[c].x;
+        x.y -= af * v[c].y + beta_prev * vp[c].y;
+        w[c] = x;
+        bpart += (double)x.x * x.x + (double)x.y * x.y;
+    }
+    const double b2 = cta_sum<NW>(bpart, S.red[1]);
+    beta = sqrt(b2);
+    if (threadIdx.x == 0) { S.alpha[it] = alpha; S.beta[it + 1] = beta; S.beta2[it + 1] = b2; }
+    __syncthreads();
+}
+
+// vp = v, v = w / beta (elements 0 .. n-1).  Ends with a barrier.
+template <int NW>
+__device__ __forceinline__ void lanczos_rotate(float2* v, float2* vp, const float2* w, int n,
+                                               double beta) {
+    const float ib = (float)(1.0 / beta);
+    for (int c = lanczos_first<NW>(); c < n; c += NW * 32) {
+        const float2 x = w[c];
+        vp[c] = v[c];
+        v[c] = make_float2(x.x * ib, x.y * ib);
+    }
+    __syncthreads();
+}
 
 // Number of eigenvalues of the m x m tridiagonal (alpha[0..m), beta[1..m))
 // below sigma = sign changes of the Sturm sequence q_0 = 1, q_1 = alpha_0 -
@@ -182,6 +262,29 @@ __device__ inline void lanczos_check(LanczosShared& S, int m, double tol, double
         S.m_last = m;
         S.next_check = m + skip;
     }
+}
+
+// Coefficients s_0 .. s_{m-1} of the unit Ritz vector of T_m at S.theta (y = sum_j s_j q_j)
+// into S.piv: the backward recurrence from s_{m-1} = 1, which grows towards s_0 and is
+// rescaled by 1e-150 whenever it passes 1e150.  Thread 0 computes; ends with a barrier.
+__device__ __forceinline__ void lanczos_ritz(LanczosShared& S, int m) {
+    if (threadIdx.x == 0) {
+        const double theta = S.theta;
+        double* s = S.piv;
+        s[m - 1] = 1.0;
+        if (m >= 2) s[m - 2] = (S.beta[m - 1] != 0.0) ? (theta - S.alpha[m - 1]) / S.beta[m - 1] : 0.0;
+        for (int i = m - 2; i >= 1; --i) {
+            const double t = (theta - S.alpha[i]) * s[i] - S.beta[i + 1] * s[i + 1];
+            s[i - 1] = (S.beta[i] != 0.0) ? t / S.beta[i] : 0.0;
+            if (fabs(s[i - 1]) > 1e150)
+                for (int k = i - 1; k < m; ++k) s[k] *= 1e-150;
+        }
+        double nn = 0.0;
+        for (int i = 0; i < m; ++i) nn += s[i] * s[i];
+        nn = 1.0 / sqrt(nn);
+        for (int i = 0; i < m; ++i) s[i] *= nn;
+    }
+    __syncthreads();
 }
 
 }  // namespace sb

@@ -17,11 +17,21 @@
 #ifndef SB_HOST_EMU            // tests/host_emu runs the scatter / eigenpair kernels on the CPU
 #include "fft_kernels.cuh"
 #endif
+#include "../../include/scint_b200.h"   // SB_ETA_* status bits, tests/host_emu too
 #include "drivers.cuh"
 #include "lanczos.cuh"
 #include "thth.cuh"
 
 namespace sb {
+
+// Combinations of the SB_ETA_* status bits of an eigenpair
+// no eigenpair: the reference raises (IndexError, eigsh on fewer than 3 centres) or ARPACK
+// fails on a zero start vector
+constexpr int ETA_NO_EIGENPAIR = SB_ETA_INDEX_ERROR | SB_ETA_ZERO_START | SB_ETA_TOO_SMALL;
+// no eigenvector was computed (a zero matrix still yields one)
+constexpr int ETA_NO_VECTOR = SB_ETA_INDEX_ERROR | SB_ETA_TOO_SMALL;
+// the reference's try/except stores NaN
+constexpr int ETA_NAN = ETA_NO_EIGENPAIR | SB_ETA_NOT_CONVERGED;
 
 // --------------------------------------------------------------------------
 // rev_map.  np.histogram2d with explicit edges e_k = (k - 0.5) * d + x0
@@ -133,7 +143,7 @@ __global__ void rev_finalise_kernel(RevGeom g, float2* __restrict__ acc,
 // chisq_sweep: rev_map of the rank-1 model |w| V V^H of every curvature of a batch
 // (blockIdx.y), computed on the fly from V; the model matrix is never stored.
 // th_red [neta][th_pitch]: the curvature's rev_map centres (theta_centres of its
-// edges_red), nred[e] of them.  Curvatures whose matrix failed (status bits 1, 2, 4)
+// edges_red), nred[e] of them.  Curvatures without an eigenpair (ETA_NO_EIGENPAIR)
 // scatter nothing: their model is zero.
 // --------------------------------------------------------------------------
 __global__ void rev_scatter_rank1_kernel(RevGeom g, const double* __restrict__ th_red,
@@ -144,7 +154,7 @@ __global__ void rev_scatter_rank1_kernel(RevGeom g, const double* __restrict__ t
                                          const float2* __restrict__ V, int ldv,
                                          float2* __restrict__ acc, int* __restrict__ cnt) {
     const int e = blockIdx.y;
-    if (status[e0 + e] & 7) return;
+    if (status[e0 + e] & ETA_NO_EIGENPAIR) return;
     g.n = nred[e0 + e];
     g.th = th_red + (size_t)(e0 + e) * th_pitch;
     g.eta = etas[e0 + e];
@@ -213,17 +223,6 @@ int rev_map(const float2* thth, int n, const double* th_dev, double eta, double 
 constexpr int EV_THREADS = 512;
 constexpr int EV_NW = EV_THREADS / 32;
 
-__device__ __forceinline__ double ev_block_sum(double x, double* red) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    x = warp_sum(x);
-    __syncthreads();
-    if (lane == 0) red[warp] = x;
-    __syncthreads();
-    double s = 0.0;
-    for (int k = 0; k < EV_NW; ++k) s += red[k];
-    return s;
-}
-
 // element (a, c) of a full row-major matrix
 struct FullMatrix {
     const float2* A;
@@ -268,9 +267,9 @@ __device__ __forceinline__ float2 start_row(const CompositeMatrix& A, int, int c
 }
 
 // Shared body.  Start vector: row n//2 (start_row).  If it is zero, zero_start_fallback == 0
-// reports it (w = NaN, info[1] = 2); otherwise Lanczos starts from a fixed non-zero
-// vector instead, and a start vector that A maps to zero (for a zero-diagonal Hermitian
-// matrix: A == 0) gives w = 0 with that vector as V and info[1] = 2.
+// reports it (w = NaN, info[1] = SB_ETA_ZERO_START); otherwise Lanczos starts from a fixed
+// non-zero vector instead, and a start vector that A maps to zero (for a zero-diagonal
+// Hermitian matrix: A == 0) gives w = 0 with that vector as V and info[1] = SB_ETA_ZERO_START.
 template <class Mat>
 __device__ void herm_eigvec_body(Mat A, int n, float2* __restrict__ Q, int max_iter, double tol,
                                  int zero_start_fallback, double* __restrict__ w_out,
@@ -293,10 +292,8 @@ __device__ void herm_eigvec_body(Mat A, int n, float2* __restrict__ Q, int max_i
         v[c] = x;
         p0 += (double)x.x * x.x + (double)x.y * x.y;
     }
-    if (tid == 0) {
-        S.done = 0; S.lo = 0.0; S.theta = 0.0; S.res = 0.0; S.next_check = 1; S.m_last = 0; S.beta2[0] = 0.0;
-    }
-    double nrm2 = ev_block_sum(p0, red);
+    lanczos_reset(S);
+    double nrm2 = cta_sum<EV_NW>(p0, red);
     const bool fallback = zero_start_fallback && nrm2 == 0.0 && n >= 2;
     if (fallback) {
         p0 = 0.0;
@@ -304,10 +301,11 @@ __device__ void herm_eigvec_body(Mat A, int n, float2* __restrict__ Q, int max_i
             v[c] = make_float2(1.0f + 0.125f * (float)((c * 37) % 11), 0.f);
             p0 += (double)v[c].x * v[c].x;
         }
-        nrm2 = ev_block_sum(p0, red);
+        __syncthreads();                // every thread has read red
+        nrm2 = cta_sum<EV_NW>(p0, red);
     }
     if (!(nrm2 > 0.0) || !isfinite(nrm2) || n < 2) {
-        if (tid == 0) { *w_out = qnan; info[0] = 0; info[1] = 2; }
+        if (tid == 0) { *w_out = qnan; info[0] = 0; info[1] = SB_ETA_ZERO_START; }
         for (int c = tid; c < n; c += EV_THREADS) V_out[c] = make_float2(0.f, 0.f);
         return;
     }
@@ -336,7 +334,7 @@ __device__ void herm_eigvec_body(Mat A, int n, float2* __restrict__ Q, int max_i
         double ap = 0.0;
         for (int c = tid; c < n; c += EV_THREADS)
             ap += (double)v[c].x * w[c].x + (double)v[c].y * w[c].y;
-        const double alpha = ev_block_sum(ap, red);
+        const double alpha = cta_sum<EV_NW>(ap, red);
         {
             const float af = (float)alpha;
             const float2* qp = Q + (size_t)(it > 0 ? it - 1 : 0) * n;
@@ -382,13 +380,13 @@ __device__ void herm_eigvec_body(Mat A, int n, float2* __restrict__ Q, int max_i
         }
         double bp = 0.0;
         for (int c = tid; c < n; c += EV_THREADS) bp += (double)w[c].x * w[c].x + (double)w[c].y * w[c].y;
-        const double b2 = ev_block_sum(bp, red);
+        const double b2 = cta_sum<EV_NW>(bp, red);
         const double beta = sqrt(b2);
         m = it + 1;
         if (fallback && it == 0 && alpha == 0.0 && b2 == 0.0) {
             // A v = 0 for the fallback vector: report w = 0, V = v
             for (int c = tid; c < n; c += EV_THREADS) V_out[c] = v[c];
-            if (tid == 0) { *w_out = 0.0; info[0] = 1; info[1] = 2; }
+            if (tid == 0) { *w_out = 0.0; info[0] = 1; info[1] = SB_ETA_ZERO_START; }
             return;
         }
         if (tid == 0) { S.alpha[it] = alpha; S.beta[m] = beta; S.beta2[m] = b2; }
@@ -401,24 +399,8 @@ __device__ void herm_eigvec_body(Mat A, int n, float2* __restrict__ Q, int max_i
         beta_prev = (float)beta;
         __syncthreads();
     }
-    // Ritz vector of T_m at theta, backward recurrence (grows towards s_0)
-    if (tid == 0) {
-        const double theta = S.theta;
-        double* s = S.piv;
-        s[m - 1] = 1.0;
-        if (m >= 2) s[m - 2] = (S.beta[m - 1] != 0.0) ? (theta - S.alpha[m - 1]) / S.beta[m - 1] : 0.0;
-        for (int i = m - 2; i >= 1; --i) {
-            double t = (theta - S.alpha[i]) * s[i] - S.beta[i + 1] * s[i + 1];
-            s[i - 1] = (S.beta[i] != 0.0) ? t / S.beta[i] : 0.0;
-            if (fabs(s[i - 1]) > 1e150)
-                for (int k = i - 1; k < m; ++k) s[k] *= 1e-150;
-        }
-        double nn = 0.0;
-        for (int i = 0; i < m; ++i) nn += s[i] * s[i];
-        nn = 1.0 / sqrt(nn);
-        for (int i = 0; i < m; ++i) s[i] *= nn;
-    }
-    __syncthreads();
+    // Ritz vector of T_m at theta
+    lanczos_ritz(S, m);
     double yp = 0.0;
     for (int c = tid; c < n; c += EV_THREADS) {
         double sx = 0.0, sy = 0.0;
@@ -430,7 +412,7 @@ __device__ void herm_eigvec_body(Mat A, int n, float2* __restrict__ Q, int max_i
         w[c] = make_float2((float)sx, (float)sy);
         yp += sx * sx + sy * sy;
     }
-    const double yn = ev_block_sum(yp, red);
+    const double yn = cta_sum<EV_NW>(yp, red);
     const float ys = (float)(1.0 / sqrt(yn));
     for (int c = tid; c < n; c += EV_THREADS) V_out[c] = make_float2(w[c].x * ys, w[c].y * ys);
     if (tid == 0) {
@@ -439,7 +421,7 @@ __device__ void herm_eigvec_body(Mat A, int n, float2* __restrict__ Q, int max_i
         // the requested residual (1e-7 by default) is close to the fp32 rounding floor; a
         // residual <= 2e-6 |theta| at the iteration cap is still a converged pair for every
         // consumer (eigenvalue error ~ res^2 / gap), anything worse is flagged
-        info[1] = (S.done || S.res <= 2e-6 * fabs(S.theta)) ? 0 : 8;
+        info[1] = (S.done || S.res <= 2e-6 * fabs(S.theta)) ? 0 : SB_ETA_NOT_CONVERGED;
     }
 }
 
@@ -461,11 +443,11 @@ herm_eigvec_batch_kernel(const float2* __restrict__ M, int ld, const int* __rest
                          int* __restrict__ status, int* __restrict__ iters) {
     const int e = blockIdx.x, ge = e0 + e;
     const int n = nred[ge];
-    if ((status[ge] & 1) || n < 3) {          // IndexError / eigsh raises for n < 3
+    if ((status[ge] & SB_ETA_INDEX_ERROR) || n < 3) {    // IndexError / eigsh raises for n < 3
         if (threadIdx.x == 0) {
             w[ge] = __longlong_as_double(0x7ff8000000000000LL);
             iters[ge] = 0;
-            if (n < 3) status[ge] |= 4;
+            if (n < 3) status[ge] |= SB_ETA_TOO_SMALL;
         }
         return;
     }
@@ -505,8 +487,8 @@ __global__ void asym_gather_kernel(const ThthGeom* __restrict__ geoms,
 // asymm = (|V[:h]|^2 - |V[h+1:m]|^2) / (|V[:h]|^2 + |V[h+1:m]|^2), h = (m - 1) // 2, in fp64
 // from the fp32 eigenvector V [nb][ld] of each chunk (one warp per chunk).  NaN where the
 // reference's try/except stores NaN: IndexError, a zero matrix, m < 3, no convergence
-// (status bits 1, 2, 4, 8); 0 / 0 is NaN as in numpy.  v_out [nchunk][ld] (optional): V,
-// zero-padded, or zeros where no eigenvector was computed (bits 1, 4).
+// (ETA_NAN); 0 / 0 is NaN as in numpy.  v_out [nchunk][ld] (optional): V, zero-padded, or
+// zeros where no eigenvector was computed (ETA_NO_VECTOR).
 __global__ void asym_finish_kernel(const float2* __restrict__ V, int ld,
                                    const int* __restrict__ nred, const int* __restrict__ status,
                                    int e0, double* __restrict__ asym, float2* __restrict__ v_out) {
@@ -514,7 +496,7 @@ __global__ void asym_finish_kernel(const float2* __restrict__ V, int ld,
     const int m = nred[ge], st = status[ge];
     const float2* v = V + (size_t)e * ld;
     const int h = (m - 1) / 2;
-    const bool has_v = !(st & 5);
+    const bool has_v = !(st & ETA_NO_VECTOR);
     double l = 0.0, r = 0.0;
     for (int c = lane; c < ld; c += 32) {
         const float2 x = (has_v && c < m) ? v[c] : make_float2(0.f, 0.f);
@@ -526,7 +508,7 @@ __global__ void asym_finish_kernel(const float2* __restrict__ V, int ld,
     l = warp_sum(l);
     r = warp_sum(r);
     if (lane == 0)
-        asym[ge] = (st & 15) ? __longlong_as_double(0x7ff8000000000000LL) : (l - r) / (l + r);
+        asym[ge] = (st & ETA_NAN) ? __longlong_as_double(0x7ff8000000000000LL) : (l - r) / (l + r);
 }
 
 // --------------------------------------------------------------------------
@@ -581,19 +563,19 @@ __global__ void vlbi_composite_kernel(ThthGeom g, const double* __restrict__ eta
 
 // Top eigenpair of the composite (N = n_dish n), started from the sum of the stations'
 // rows n//2 or, if that is zero, from the fixed start vector.  info = {Lanczos steps,
-// SB_ETA_* status, nred}; status bit 1 comes from thth_prep.  A matrix smaller than
-// 3 x 3 is reported as bit 4 (eigsh raises).
+// SB_ETA_* status, nred}; SB_ETA_INDEX_ERROR comes from thth_prep.  A matrix smaller than
+// 3 x 3 is reported as SB_ETA_TOO_SMALL (eigsh raises).
 __global__ void __launch_bounds__(EV_THREADS)
 vlbi_eigvec_kernel(const float2* __restrict__ A, int n_dish, int n, float2* __restrict__ Q,
                    int max_iter, double tol, double* __restrict__ w, float2* __restrict__ V,
                    int* __restrict__ info) {
     const int N = n_dish * n;
-    if ((info[1] & 1) || N < 3) {
+    if ((info[1] & SB_ETA_INDEX_ERROR) || N < 3) {
         for (int c = threadIdx.x; c < N; c += EV_THREADS) V[c] = make_float2(0.f, 0.f);
         if (threadIdx.x == 0) {
             *w = __longlong_as_double(0x7ff8000000000000LL);
             info[0] = 0;
-            if (N < 3) info[1] |= 4;
+            if (N < 3) info[1] |= SB_ETA_TOO_SMALL;
         }
         return;
     }
@@ -609,12 +591,12 @@ vlbi_eigvec_kernel(const float2* __restrict__ A, int n_dish, int n, float2* __re
 // conj(V[d n : (d + 1) n]) sqrt(w) (the zero rows still count in the bin means).
 // blockIdx.y < n_dish: station blockIdx.y adds the values of row n//2 to acc[d];
 // blockIdx.y == n_dish: the counts of all n^2 - n off-diagonal points, shared by every
-// station.  A failed eigenpair (status bits 1, 2, 4) scatters nothing.
+// station.  A failed eigenpair (ETA_NO_EIGENPAIR) scatters nothing.
 __global__ void vlbi_scatter_kernel(RevGeom g, int n_dish, const int* __restrict__ info,
                                     const double* __restrict__ w,
                                     const float2* __restrict__ V, float2* __restrict__ acc,
                                     int* __restrict__ cnt) {
-    if (info[1] & 7) return;
+    if (info[1] & ETA_NO_EIGENPAIR) return;
     const int n = g.n, h = n / 2, d = blockIdx.y;
     if (d == n_dish) {
         for (long p = blockIdx.x * (long)blockDim.x + threadIdx.x; p < (long)n * n;
@@ -825,7 +807,7 @@ __global__ void chisq_finish_kernel(const double* __restrict__ part, int e0, int
     double s = 0.0;
     for (int k = 0; k < CHISQ_SLOTS; ++k) s += part[(size_t)e * CHISQ_SLOTS + k];
     // the reference raises for these curvatures (IndexError, ARPACK error, n < 3)
-    ssq[e0 + e] = (status[e0 + e] & 7) ? __longlong_as_double(0x7ff8000000000000LL) : s;
+    ssq[e0 + e] = (status[e0 + e] & ETA_NO_EIGENPAIR) ? __longlong_as_double(0x7ff8000000000000LL) : s;
 }
 
 int chisq_sweep(const ThthGeom& g, const double* th_host, const double* d_etas, int neta,

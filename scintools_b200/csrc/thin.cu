@@ -18,14 +18,12 @@
 #include <limits.h>
 #include <math.h>
 
+#include "../../include/scint_b200.h"   // SB_ETA_* status bits, tests/host_emu too
 #include "drivers.cuh"
 #include "lanczos.cuh"
 #include "thth.cuh"
 
 namespace sb {
-
-enum { TST_OK = 0, TST_INDEX_ERROR = 1, TST_ZERO_START = 2, TST_TOO_SMALL = 4,
-       TST_NOT_CONVERGED = 8 };
 
 // crop masks + compaction for both axes, one warp per eta
 __global__ void thin_prep_kernel(ThinGeom t, const double* __restrict__ eta1,
@@ -133,7 +131,7 @@ thin_build_kernel(ThinGeom t, const double* __restrict__ eta1,
         }
         if (a < ld2) Me[(size_t)a * ld1 + b] = v;
     }
-    if (bad) atomicOr(status + eta0 + e, TST_INDEX_ERROR);
+    if (bad) atomicOr(status + eta0 + e, SB_ETA_INDEX_ERROR);
 }
 
 // the index error may also sit on a point that the crop removes: scan all
@@ -149,10 +147,10 @@ __global__ void thin_indexerr_kernel(ThinGeom t, const double* __restrict__ eta1
         bad |= thin_point(t, eta1[e], eta2[e], t.g.th[j], t.th2[i]).index_error;
     }
     if (__any_sync(0xffffffffu, bad) && (threadIdx.x & 31) == 0)
-        atomicOr(status + e, TST_INDEX_ERROR);
+        atomicOr(status + e, SB_ETA_INDEX_ERROR);
 }
 
-// ---- Lanczos on A^H A (bookkeeping in lanczos.cuh) ---------------------------
+// ---- Lanczos on A^H A (step, rotation and bookkeeping in lanczos.cuh) ---------
 // one CTA per eta: sigma_max(A) with A = M[e] (n2 x n1, row pitch ld1)
 template <int THREADS>
 __global__ void __launch_bounds__(THREADS)
@@ -172,10 +170,10 @@ thin_sv_kernel(const float2* __restrict__ Mbase, int ld1, int ld2,
     const int n1 = n1r[eta0 + e], n2 = n2r[eta0 + e];
     const float2* M = Mbase + (size_t)e * ld1 * ld2;
     const double qnan = __longlong_as_double(0x7ff8000000000000LL);
-    if ((status[eta0 + e] & TST_INDEX_ERROR) || n1 < 1 || n2 < 1) {
+    if ((status[eta0 + e] & SB_ETA_INDEX_ERROR) || n1 < 1 || n2 < 1) {
         if (tid == 0) {
             svals[eta0 + e] = qnan; iters[eta0 + e] = 0;
-            if (n1 < 1 || n2 < 1) status[eta0 + e] |= TST_TOO_SMALL;
+            if (n1 < 1 || n2 < 1) status[eta0 + e] |= SB_ETA_TOO_SMALL;
         }
         return;
     }
@@ -185,7 +183,7 @@ thin_sv_kernel(const float2* __restrict__ Mbase, int ld1, int ld2,
         v[c] = c < n1 ? make_float2(1.f, 0.f) : make_float2(0.f, 0.f);
         vp[c] = make_float2(0.f, 0.f);
     }
-    if (tid == 0) { S.done = 0; S.lo = 0.0; S.theta = 0.0; S.next_check = 1; S.m_last = 0; S.beta2[0] = 0.0; }
+    lanczos_reset(S);
     __syncthreads();
     {
         const float s = rsqrtf((float)n1);
@@ -235,64 +233,25 @@ thin_sv_kernel(const float2* __restrict__ Mbase, int ld1, int ld2,
                     zc[j].w = fmaf(q.z, yy, zc[j].w); zc[j].w = fmaf(-q.w, yx, zc[j].w);
                 }
             }
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-                *reinterpret_cast<float4*>(part + warp * 512 + 2 * (lane + 32 * j)) = zc[j];
-            __syncthreads();
-            for (int c = tid; c < 512; c += THREADS) {
-                float sx = 0.f, sy = 0.f;
-#pragma unroll
-                for (int k = 0; k < NW; ++k) { sx += part[k * 512 + c].x; sy += part[k * 512 + c].y; }
-                if (cb * 512 + c < ld1) w[cb * 512 + c] = make_float2(sx, sy);
-            }
-            __syncthreads();
+            thth_fold_columns<NW>(zc, part, w, cb * 512, ld1);
         }
-        double apart = 0.0;
-        for (int c = tid; c < n1; c += THREADS)
-            apart += (double)(v[c].x * w[c].x + v[c].y * w[c].y);
-        apart = warp_sum(apart);
-        if (lane == 0) S.red[0][warp] = apart;
-        __syncthreads();
-        double alpha = 0.0;
-        for (int k = 0; k < NW; ++k) alpha += S.red[0][k];
-        const float af = (float)alpha;
-        double bpart = 0.0;
-        for (int c = tid; c < n1; c += THREADS) {
-            float2 x = w[c];
-            x.x -= af * v[c].x + beta_prev * vp[c].x;
-            x.y -= af * v[c].y + beta_prev * vp[c].y;
-            w[c] = x;
-            bpart += (double)x.x * x.x + (double)x.y * x.y;
-        }
-        bpart = warp_sum(bpart);
-        if (lane == 0) S.red[1][warp] = bpart;
-        __syncthreads();
-        double b2 = 0.0;
-        for (int k = 0; k < NW; ++k) b2 += S.red[1][k];
-        const double beta = sqrt(b2);
+        double alpha, beta;
+        lanczos_step<NW>(S, it, n1, v, vp, w, nullptr, beta_prev, alpha, beta);
         m = it + 1;
-        if (tid == 0) { S.alpha[it] = alpha; S.beta[m] = beta; S.beta2[m] = b2; }
-        __syncthreads();
         const bool last = (it + 1 == max_iter);
         if (!isfinite(alpha) || !isfinite(beta)) { nonfinite = true; break; }
         if (warp == 0 && (m >= S.next_check || last || !(beta > 0.0))) lanczos_check(S, m, tol, etol);
         __syncthreads();
         if (S.done) break;
-        const float ib = (float)(1.0 / beta);
-        for (int c = tid; c < n1; c += THREADS) {
-            const float2 x = w[c];
-            vp[c] = v[c];
-            v[c] = make_float2(x.x * ib, x.y * ib);
-        }
+        lanczos_rotate<NW>(v, vp, w, n1, beta);
         beta_prev = (float)beta;
-        __syncthreads();
     }
     if (tid == 0) {
         // an all-zero map has sigma_max = 0 (numpy returns 0, no exception)
         const double th = S.theta > 0.0 ? S.theta : 0.0;
         svals[eta0 + e] = nonfinite ? qnan : sqrt(th);
         iters[eta0 + e] = m;
-        if (!S.done && !nonfinite) status[eta0 + e] |= TST_NOT_CONVERGED;
+        if (!S.done && !nonfinite) status[eta0 + e] |= SB_ETA_NOT_CONVERGED;
     }
 }
 
@@ -304,7 +263,7 @@ __global__ void thin_map_kernel(ThinGeom t, double e1, double e2, float2* __rest
          p += (long long)gridDim.x * blockDim.x) {
         const int i = (int)(p / t.g.n), j = (int)(p % t.g.n);
         const ThinPoint pt = thin_point(t, e1, e2, t.g.th[j], t.th2[i]);
-        if (pt.index_error) atomicOr(err, TST_INDEX_ERROR);
+        if (pt.index_error) atomicOr(err, SB_ETA_INDEX_ERROR);
         out[p] = thin_value(t, e1, e2, t.g.th[j], t.th2[i], pt);
     }
 }

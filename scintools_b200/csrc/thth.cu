@@ -14,15 +14,12 @@
 
 #include <vector>
 
+#include "../../include/scint_b200.h"   // SB_ETA_* status bits, tests/host_emu too
 #include "drivers.cuh"
 #include "lanczos.cuh"
 #include "thth.cuh"
 
 namespace sb {
-
-// status codes per eta (also in include/scint_b200.h)
-enum { ST_OK = 0, ST_INDEX_ERROR = 1, ST_ZERO_START = 2, ST_TOO_SMALL = 4,
-       ST_NOT_CONVERGED = 8 };
 
 // --------------------------------------------------------------------------
 // crop mask + compaction: th_pnts of thth_redmap (ththmod.py:153-156)
@@ -80,7 +77,7 @@ __device__ __forceinline__ void thth_indexerr_body(const ThthGeom& g, double eta
         bad |= pt.index_error;
     }
     if (__any_sync(0xffffffffu, bad) && (threadIdx.x & 31) == 0)
-        atomicOr(status, ST_INDEX_ERROR);
+        atomicOr(status, SB_ETA_INDEX_ERROR);
 }
 
 __global__ void thth_indexerr_kernel(ThthGeom g, const double* __restrict__ etas,
@@ -224,7 +221,7 @@ thth_build_body(const ThthGeom& g, const double* __restrict__ etas, int eta0, in
     // per-curvature power-of-two scale of the fp16 copy, once per CTA (it was ~40 instructions
     // of log2f / exp2f per thread and curvature): 2^floor(log2(2^15 / bound)) is the exponent
     // field of the quotient
-    __shared__ float s_hscale[SB_BUILD_EB];
+    SB_SHARED float s_hscale[SB_BUILD_EB];
     if (PACK != 0) {
         const int lin = ty * 32 + tx;
         if (lin < SB_BUILD_EB) {
@@ -468,7 +465,7 @@ cs_compact_kernel(const float2* __restrict__ cs, long long ntau, long long cs_pi
 // --------------------------------------------------------------------------
 // Lanczos on the Hermitian matrix: largest ALGEBRAIC eigenvalue
 // (scipy eigsh(..., k=1, which="LA"), ththmod.py:398-401), start vector =
-// row n//2.  No re-orthogonalisation: only the top Ritz value is wanted.
+// row n//2 (thth_start_vector, thth_lanczos: thth.cuh).
 // --------------------------------------------------------------------------
 // One CTA per eta.  The matrix is stored as its strict upper triangle; a warp
 // owns rows a = warp, warp+NW, ... and for every stored element A[a][b] adds
@@ -497,55 +494,28 @@ thth_eig_kernel(const float2* __restrict__ Mbase, int ld,
     const float2* M = Mbase + (size_t)e * ld * ld;
     const double qnan = __longlong_as_double(0x7ff8000000000000LL);
 
-    if (status[eta0 + e] & ST_INDEX_ERROR) {
+    if (status[eta0 + e] & SB_ETA_INDEX_ERROR) {
         if (tid == 0) { eigs[eta0 + e] = qnan; iters[eta0 + e] = 0; }
         return;
     }
     if (n < 3) {
         if (tid == 0) {
             eigs[eta0 + e] = qnan; iters[eta0 + e] = 0;
-            status[eta0 + e] |= ST_TOO_SMALL;
+            status[eta0 + e] |= SB_ETA_TOO_SMALL;
         }
         return;
     }
-    // v0 = row n//2 of the Hermitian matrix (ththmod.py:398-399)
-    const int h = n / 2;
-    double part0 = 0.0;
-    for (int c = tid; c < ld; c += THREADS) {
-        float2 x = make_float2(0.f, 0.f);
-        if (c < n && c > h) x = M[(size_t)h * ld + c];
-        else if (c < h) { x = M[(size_t)c * ld + h]; x.y = -x.y; }
-        v[c] = x;
-        vp[c] = make_float2(0.f, 0.f);
-        part0 += (double)x.x * x.x + (double)x.y * x.y;
-    }
-    part0 = warp_sum(part0);
-    if (lane == 0) S.red[0][warp] = part0;
-    if (tid == 0) {
-        S.done = 0; S.lo = 0.0; S.theta = 0.0; S.res = 0.0;
-        S.next_check = 1; S.m_last = 0; S.beta2[0] = 0.0;
-    }
-    __syncthreads();
-    double nrm2 = 0.0;
-    for (int k = 0; k < NW; ++k) nrm2 += S.red[0][k];
-    if (!(nrm2 > 0.0) || !isfinite(nrm2)) {
+    if (!thth_start_vector<NW>(M, ld, n, v, vp, S.red[0])) {
         if (tid == 0) {
             eigs[eta0 + e] = qnan; iters[eta0 + e] = 0;
-            status[eta0 + e] |= ST_ZERO_START;
+            status[eta0 + e] |= SB_ETA_ZERO_START;
         }
         return;
     }
-    {
-        float s = (float)(1.0 / sqrt(nrm2));
-        for (int c = tid; c < ld; c += THREADS) { v[c].x *= s; v[c].y *= s; }
-    }
-    __syncthreads();
 
     const int ncol4 = (n + 1) >> 1;      // float4 = two complex columns
     const int nchunk = (n + 511) / 512;  // column chunks of 512
-    float beta_prev = 0.f;
-    int m = 0;
-    for (int it = 0; it < max_iter; ++it) {
+    auto matvec = [&]() {
         for (int c = tid; c < ld; c += THREADS) w[c] = make_float2(0.f, 0.f);
         __syncthreads();
         for (int cb = 0; cb < nchunk; ++cb) {
@@ -569,92 +539,19 @@ thth_eig_kernel(const float2* __restrict__ Mbase, int ld,
                 }
                 float rx = 0.f, ry = 0.f;
                 const int jskip = (first4 - cb * 256) >> 5;   // groups entirely left of the diagonal
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    if (j < jskip) continue;
-                    const int c4 = cb * 256 + lane + 32 * j;
-                    const float4 q = mm[j];
-                    const float4 x = (2 * c4 < ld) ? *reinterpret_cast<const float4*>(v + 2 * c4)
-                                                   : make_float4(0.f, 0.f, 0.f, 0.f);
-                    // explicit FMA chains (16 FFMA per two complex elements)
-                    rx = fmaf(q.x, x.x, rx); rx = fmaf(-q.y, x.y, rx);
-                    rx = fmaf(q.z, x.z, rx); rx = fmaf(-q.w, x.w, rx);
-                    ry = fmaf(q.x, x.y, ry); ry = fmaf(q.y, x.x, ry);
-                    ry = fmaf(q.z, x.w, ry); ry = fmaf(q.w, x.z, ry);
-                    // conj(A) * v[a]
-                    yc[j].x = fmaf(q.x, xa.x, yc[j].x); yc[j].x = fmaf(q.y, xa.y, yc[j].x);
-                    yc[j].y = fmaf(q.x, xa.y, yc[j].y); yc[j].y = fmaf(-q.y, xa.x, yc[j].y);
-                    yc[j].z = fmaf(q.z, xa.x, yc[j].z); yc[j].z = fmaf(q.w, xa.y, yc[j].z);
-                    yc[j].w = fmaf(q.z, xa.y, yc[j].w); yc[j].w = fmaf(-q.w, xa.x, yc[j].w);
-                }
+                thth_row_fma([&](int j, int) { return mm[j]; }, v, ld, cb * 256, jskip, xa, rx, ry, yc);
                 rx = warp_sum(rx);
                 ry = warp_sum(ry);
                 if (lane == 0) { w[a].x += rx; w[a].y += ry; }
             }
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-                *reinterpret_cast<float4*>(part + warp * 512 + 2 * (lane + 32 * j)) = yc[j];
-            __syncthreads();
-            for (int c = tid; c < 512; c += THREADS) {
-                float sx = 0.f, sy = 0.f;
-#pragma unroll
-                for (int k = 0; k < NW; ++k) { sx += part[k * 512 + c].x; sy += part[k * 512 + c].y; }
-                if (cb * 512 + c < ld) u[cb * 512 + c] = make_float2(sx, sy);
-            }
-            __syncthreads();
+            thth_fold_columns<NW>(yc, part, u, cb * 512, ld);
         }
-        // ---- alpha = Re <v, A v>
-        double apart = 0.0;
-        for (int c = tid; c < n; c += THREADS) {
-            float2 x = w[c];
-            x.x += u[c].x;
-            x.y += u[c].y;
-            w[c] = x;
-            apart += (double)(v[c].x * x.x + v[c].y * x.y);
-        }
-        apart = warp_sum(apart);
-        if (lane == 0) S.red[0][warp] = apart;
-        __syncthreads();
-        double alpha = 0.0;
-        for (int k = 0; k < NW; ++k) alpha += S.red[0][k];
-        // ---- w -= alpha v + beta_prev vp ; beta = ||w||
-        const float af = (float)alpha;
-        double bpart = 0.0;
-        for (int c = tid; c < n; c += THREADS) {
-            float2 x = w[c];
-            x.x -= af * v[c].x + beta_prev * vp[c].x;
-            x.y -= af * v[c].y + beta_prev * vp[c].y;
-            w[c] = x;
-            bpart += (double)x.x * x.x + (double)x.y * x.y;
-        }
-        bpart = warp_sum(bpart);
-        if (lane == 0) S.red[1][warp] = bpart;
-        __syncthreads();
-        double b2 = 0.0;
-        for (int k = 0; k < NW; ++k) b2 += S.red[1][k];
-        const double beta = sqrt(b2);
-        m = it + 1;
-        if (tid == 0) { S.alpha[it] = alpha; S.beta[m] = beta; S.beta2[m] = b2; }
-        __syncthreads();
-        const bool last = (it + 1 == max_iter);
-        if (warp == 0 && (m >= S.next_check || last || !(beta > 0.0)))
-            lanczos_check(S, m, tol, etol);
-        __syncthreads();
-        if (S.done || !isfinite(alpha)) break;
-        // ---- rotate: vp = v, v = w / beta
-        const float ib = (float)(1.0 / beta);
-        for (int c = tid; c < n; c += THREADS) {
-            float2 x = w[c];
-            vp[c] = v[c];
-            v[c] = make_float2(x.x * ib, x.y * ib);
-        }
-        beta_prev = (float)beta;
-        __syncthreads();
-    }
+    };
+    const int m = thth_lanczos<NW>(S, matvec, v, vp, w, u, n, max_iter, tol, etol);
     if (tid == 0) {
         eigs[eta0 + e] = fabs(S.theta);  // np.abs(w[0])
         iters[eta0 + e] = m;
-        if (!S.done) status[eta0 + e] |= ST_NOT_CONVERGED;
+        if (!S.done) status[eta0 + e] |= SB_ETA_NOT_CONVERGED;
     }
 }
 
@@ -673,7 +570,7 @@ __global__ void thth_map_kernel(ThthGeom g, double eta, int hermitian,
         int i = (int)(p / g.n), j = (int)(p % g.n);
         double thi = g.th[i], thj = g.th[j];
         ThthPoint pt = thth_point(g, eta, thj, thi);
-        if (pt.index_error) atomicOr(err, ST_INDEX_ERROR);
+        if (pt.index_error) atomicOr(err, SB_ETA_INDEX_ERROR);
         if (tau_inv) tau_inv[p] = (int)max(min(pt.tq, (long long)INT_MAX), (long long)INT_MIN);
         if (fd_inv) fd_inv[p] = (int)max(min(pt.fq, (long long)INT_MAX), (long long)INT_MIN);
         if (pnts) pnts[p] = pt.pnt ? 1 : 0;

@@ -1,8 +1,10 @@
-// theta-theta geometry shared by the gather / eigen kernels.
+// theta-theta geometry shared by the gather / eigen kernels, and the Lanczos pieces of the
+// two solvers on its strict upper triangles (thth_eig_kernel, thth_eig_half_kernel).
 #pragma once
 #include <limits.h>
 
 #include "common.cuh"
+#include "lanczos.cuh"
 
 namespace sb {
 
@@ -135,6 +137,115 @@ __device__ __forceinline__ float2 thth_herm_upper(const ThthGeom& g, double eta,
     v.x = nan_to_num(v.x);
     v.y = nan_to_num(v.y);
     return v;
+}
+
+// ---- Lanczos on a Hermitian matrix with zero diagonal stored as its strict upper triangle
+// M [ld][ld] (thth_build_kernel), run by the first NW warps of the CTA --------------------
+
+// Start vector of Eval_calc (ththmod.py:398-399): v = row n//2 of the Hermitian matrix,
+// normalised, vp = 0.  False (v left unnormalised) when that row is zero or not finite.
+// Starts with a barrier, so that a solve can restart from it, and ends with one.
+template <int NW>
+__device__ __forceinline__ bool thth_start_vector(const float2* M, int ld, int n, float2* v,
+                                                  float2* vp, double* red) {
+    __syncthreads();
+    const int c0 = lanczos_first<NW>(), h = n / 2;
+    double part0 = 0.0;
+    for (int c = c0; c < ld; c += NW * 32) {
+        float2 x = make_float2(0.f, 0.f);
+        if (c < n && c > h) x = M[(size_t)h * ld + c];
+        else if (c < h) { x = M[(size_t)c * ld + h]; x.y = -x.y; }
+        v[c] = x;
+        vp[c] = make_float2(0.f, 0.f);
+        part0 += (double)x.x * x.x + (double)x.y * x.y;
+    }
+    const double nrm2 = cta_sum<NW>(part0, red);
+    if (!(nrm2 > 0.0) || !isfinite(nrm2)) return false;
+    const float s = (float)(1.0 / sqrt(nrm2));
+    for (int c = c0; c < ld; c += NW * 32) { v[c].x *= s; v[c].y *= s; }
+    __syncthreads();
+    return true;
+}
+
+// Row a of the mat-vec over the column groups c4 = c4_0 + lane + 32 j, j = jskip .. 7 (a
+// float4 holds columns 2 c4, 2 c4 + 1): q(j, c4) is the stored element pair, zero outside
+// the row's part of the triangle.  Adds A[a][.] v to the row sums (rx, ry) and
+// conj(A[a][.]) v[a] to the column partials yc[j], so that every stored element is read once
+// per step (16 FFMA per pair).
+template <class Row>
+__device__ __forceinline__ void thth_row_fma(const Row& q, const float2* v, int ld, int c4_0,
+                                             int jskip, float2 xa, float& rx, float& ry,
+                                             float4 (&yc)[8]) {
+    const int lane = threadIdx.x & 31;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        if (j < jskip) continue;
+        const int c4 = c4_0 + lane + 32 * j;
+        const float4 p = q(j, c4);
+        const float4 x = (2 * c4 < ld) ? *reinterpret_cast<const float4*>(v + 2 * c4)
+                                       : make_float4(0.f, 0.f, 0.f, 0.f);
+        // explicit FMA chains
+        rx = fmaf(p.x, x.x, rx); rx = fmaf(-p.y, x.y, rx);
+        rx = fmaf(p.z, x.z, rx); rx = fmaf(-p.w, x.w, rx);
+        ry = fmaf(p.x, x.y, ry); ry = fmaf(p.y, x.x, ry);
+        ry = fmaf(p.z, x.w, ry); ry = fmaf(p.w, x.z, ry);
+        // conj(A) * v[a]
+        yc[j].x = fmaf(p.x, xa.x, yc[j].x); yc[j].x = fmaf(p.y, xa.y, yc[j].x);
+        yc[j].y = fmaf(p.x, xa.y, yc[j].y); yc[j].y = fmaf(-p.y, xa.x, yc[j].y);
+        yc[j].z = fmaf(p.z, xa.x, yc[j].z); yc[j].z = fmaf(p.w, xa.y, yc[j].z);
+        yc[j].w = fmaf(p.z, xa.y, yc[j].w); yc[j].w = fmaf(-p.w, xa.x, yc[j].w);
+    }
+}
+
+// Column sums of a 512-column chunk from per-lane partials (thth_row_fma; thin.cu's A^H A
+// pass): yc[j] of warp k holds columns 2 (lane + 32 j), +1 and goes through part [NW][512];
+// out[col0 + c] = the sum over warps 0 .. NW-1, for c < 512 and col0 + c < ld.  A barrier
+// before the sums and one after.
+template <int NW>
+__device__ __forceinline__ void thth_fold_columns(const float4 (&yc)[8], float2* part, float2* out,
+                                                  int col0, int ld) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (warp < NW) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+            *reinterpret_cast<float4*>(part + warp * 512 + 2 * (lane + 32 * j)) = yc[j];
+    }
+    __syncthreads();
+    for (int c = lanczos_first<NW>(); c < 512; c += NW * 32) {
+        float sx = 0.f, sy = 0.f;
+#pragma unroll
+        for (int k = 0; k < NW; ++k) { sx += part[k * 512 + c].x; sy += part[k * 512 + c].y; }
+        if (col0 + c < ld) out[col0 + c] = make_float2(sx, sy);
+    }
+    __syncthreads();
+}
+
+// Plain Lanczos, no re-orthogonalisation (only the top Ritz value is wanted), from the
+// normalised vector in v with vp = 0.  matvec() leaves the row sums of A v in w and the
+// column sums in u; warp 0 checks T_m whenever lanczos_check scheduled it.  Returns the
+// steps taken; S.theta / S.done give the outcome.
+template <int NW, class MatVec>
+__device__ __forceinline__ int thth_lanczos(LanczosShared& S, const MatVec& matvec, float2* v,
+                                            float2* vp, float2* w, const float2* u, int n,
+                                            int max_iter, double tol, double etol) {
+    lanczos_reset(S);
+    __syncthreads();
+    float beta_prev = 0.f;
+    int m = 0;
+    for (int it = 0; it < max_iter; ++it) {
+        matvec();
+        double alpha, beta;
+        lanczos_step<NW>(S, it, n, v, vp, w, u, beta_prev, alpha, beta);
+        m = it + 1;
+        const bool last = (it + 1 == max_iter);
+        if (threadIdx.x < 32 && (m >= S.next_check || last || !(beta > 0.0)))
+            lanczos_check(S, m, tol, etol);
+        __syncthreads();
+        if (S.done || !isfinite(alpha)) break;
+        lanczos_rotate<NW>(v, vp, w, n, beta);
+        beta_prev = (float)beta;
+    }
+    return m;
 }
 
 #ifndef SB_HOST_EMU
