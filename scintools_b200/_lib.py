@@ -138,7 +138,22 @@ _SIGS = {
 
 EXPORTS = tuple(_SIGS)
 
-for _name, (_res, _args) in _SIGS.items():
+
+class Brightness(ctypes.Structure):
+    """struct sb_brightness (include/scint_b200_brightness.h)"""
+    _fields_ = [("nset", c_int), ("n", c_int), ("ntd", c_int), ("nfd", c_int), ("stages", c_int),
+                ("x", vp), ("diag", vp), ("td", vp), ("par", vp), ("colx", vp), ("colq", vp),
+                ("half_df", c_dbl), ("jac_cap", c_dbl), ("jac_out", c_dbl),
+                ("rho", vp), ("B", vp), ("thetax", vp), ("thetay", vp), ("jac", vp), ("ss", vp),
+                ("lss", vp), ("acf", vp)]
+
+
+# entry points declared in include/scint_b200_brightness.h, outside scint_b200.h's set
+BRIGHTNESS_SIGS = {
+    "sb_brightness_f64": (c_int, [ctypes.POINTER(Brightness), vp]),
+}
+
+for _name, (_res, _args) in list(_SIGS.items()) + list(BRIGHTNESS_SIGS.items()):
     _fn = getattr(lib, _name)   # AttributeError here = ABI mismatch, fail loudly
     _fn.restype = _res
     _fn.argtypes = _args

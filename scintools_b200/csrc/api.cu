@@ -5,6 +5,7 @@
 #include <vector>
 
 #include "../../include/scint_b200.h"
+#include "../../include/scint_b200_brightness.h"
 #include "common.cuh"
 #include "drivers.cuh"
 
@@ -589,6 +590,11 @@ int sb_scint_fit_2d(const sb_scint_fit* fits, int32_t nfit, double* out, int32_t
 int sb_acf_model_f64(const sb_acf_model* m, double* acf, double* efield, void* stream) {
     sb::StreamFence fence(stream);
     return sb::acf_model(m, acf, efield, (cudaStream_t)stream);
+}
+
+int sb_brightness_f64(const sb_brightness* d, void* stream) {
+    sb::StreamFence fence(stream);
+    return sb::brightness(d, (cudaStream_t)stream);
 }
 
 int sb_convert_f64_f32(const double* src, float* dst, int64_t n, void* stream) {

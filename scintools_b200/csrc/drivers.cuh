@@ -2,6 +2,7 @@
 // the parameter structs it hands them.  Every file that defines one includes this header.
 #pragma once
 #include "thth.cuh"
+#include "../../include/scint_b200_brightness.h"
 
 namespace sb {
 
@@ -141,6 +142,9 @@ int scint_fit_2d(const sb_scint_fit* fits, int nfit, double* out, int* info, cud
 
 // acf_model.cu
 int acf_model(const sb_acf_model* m, double* acf, double* efield, cudaStream_t st);
+
+// brightness.cu
+int brightness(const sb_brightness* d, cudaStream_t st);
 
 // normsspec.cu
 int norm_sspec_rows(const float* sspec, int nr, int nc, const double* fdop, const double* tdel,

@@ -1,5 +1,6 @@
 """CUDA-native mirror of scintools.scint_sim.Simulation
-(reference scintools/scint_sim.py:23-311) and scint_sim.ACF (:417-765).
+(reference scintools/scint_sim.py:23-311), scint_sim.ACF (:417-765) and
+scint_sim.Brightness (:768-958).
 
 Same constructor signature and the same attributes afterwards (w, xyp, xyi,
 spe, spi, dyn, freqs, times, df, dt, eta, betaeta, ...), so the result drops
@@ -21,7 +22,8 @@ dropped), because the drop-in contract is "identical attributes" and SURVEY.md
 a12 / a15 keep this glue in Python.  It is restated reference code, not new design;
 what is new here is everything that touches the device.  ``ACF`` follows the same rule:
 its axes and scalars are the reference's numpy expressions, and the double sum of every
-lag runs in libscint_b200 (sb_acf_model_f64).
+lag runs in libscint_b200 (sb_acf_model_f64).  So does ``Brightness``, whose device half is
+sb_brightness_f64 (include/scint_b200_brightness.h).
 """
 import numpy as np
 import scipy.constants as sc
@@ -421,3 +423,302 @@ class ACF():
 
     def plot_sspec(self, display=True, vmin=None, vmax=None):
         raise NotImplementedError("plotting is outside the GPU hot path")
+
+
+# sizes the device takes (include/scint_b200_brightness.h)
+_BRIGHT_MAX_N = 1024          # lattice points per side
+_BRIGHT_MAX_Q = 4096          # len(td), len(fd)
+_BRIGHT_NPAR = 7
+_BRIGHT_EFIELD, _BRIGHT_SSPEC, _BRIGHT_ACF = 1, 2, 4
+_BRIGHT_GROUP_BYTES = 4 << 30  # device memory of one batched pass, outputs and workspace
+_BRIGHT_SET_KEYS = ("ar", "psi", "alpha", "thetagx", "thetagy", "thetarx", "thetary")
+_BRIGHT_GRID_KEYS = ("nx", "dx", "nf", "df", "nt", "dt")
+_TRIANGULATIONS = {}           # sha256 of the lattice axis -> packed diagonal bits
+
+
+def lattice_diagonals(x):
+    """The diagonal qhull splits each cell of the lattice meshgrid(x, x) along, as
+    griddata((X.ravel(), Y.ravel()), ...) triangulates it: (n-1)^2 bits, cell k = i (n-1) + j,
+    set where the cell's two triangles share the corners (x[j], x[i]) and (x[j+1], x[i+1]),
+    packed by np.packbits.  Built once per lattice (scipy.spatial.Delaunay, seconds on 600^2)
+    and cached.  Raises ValueError if any simplex is not half of a lattice cell."""
+    import hashlib
+    x = np.ascontiguousarray(x, dtype=np.float64)
+    key = hashlib.sha256(x.tobytes()).hexdigest()
+    if key not in _TRIANGULATIONS:
+        from scipy.spatial import Delaunay
+        n = len(x)
+        X, Y = np.meshgrid(x, x)
+        simp = Delaunay(np.column_stack((np.ravel(X), np.ravel(Y)))).simplices
+        i, j = simp // n, simp % n
+        i0, j0 = i.min(axis=1), j.min(axis=1)
+        corner = (i - i0[:, None]) * 2 + (j - j0[:, None])      # 0 (j,i) 1 (j+1,i) 2 3
+        half = ((i.max(axis=1) - i0 == 1) & (j.max(axis=1) - j0 == 1) &
+                (np.sort(corner, axis=1) != np.sort(corner, axis=1)[:, [1, 2, 0]]).all(axis=1))
+        if len(simp) != 2 * (n - 1) ** 2 or not half.all():
+            raise ValueError("the triangulation of the lattice has simplices that are not half "
+                             "of a lattice cell; the cell rule does not apply")
+        missing = 6 - corner.sum(axis=1)
+        main = (missing == 1) | (missing == 2)
+        cell = i0 * (n - 1) + j0
+        count = np.bincount(cell, minlength=(n - 1) ** 2)
+        nmain = np.bincount(cell, weights=main, minlength=(n - 1) ** 2)
+        nmiss = np.bincount(cell, weights=missing, minlength=(n - 1) ** 2)
+        # two triangles per cell on one diagonal: missing corners {1, 2} or {0, 3}
+        if not ((count == 2).all() and np.isin(nmain, (0, 2)).all() and (nmiss == 3).all()):
+            raise ValueError("the triangulation of the lattice does not split every cell in two "
+                             "along one diagonal; the cell rule does not apply")
+        _TRIANGULATIONS[key] = np.packbits(nmain > 0)
+    return _TRIANGULATIONS[key]
+
+
+def _efield_host(o):
+    """calc_brightness's host half (scint_sim.py:843-852): the reference's expressions."""
+    x = np.arange(-o.nx, o.nx, o.dx)
+    X, Y = np.meshgrid(x, x)
+    with np.errstate(all="ignore"):
+        R = (o.ar**2 - 1) / (o.ar**2 + 1)
+        cosa = np.cos(2 * (90 - o.psi) * np.pi/180)
+        sina = np.sin(2 * (90 - o.psi) * np.pi/180)
+        a = (1 - R * cosa) / np.sqrt(1 - R**2)
+        b = (1 + R * cosa) / np.sqrt(1 - R**2)
+        c = -2 * R * sina / np.sqrt(1 - R**2)
+    if not np.isfinite([a, b, c]).all():
+        raise ValueError("the quadratic form of ar = %r, psi = %r is not finite (a=%r, b=%r, "
+                         "c=%r)" % (o.ar, o.psi, a, b, c))
+    alph2 = o.alpha/2
+    if not np.isfinite(alph2):
+        raise ValueError("alpha must be finite")
+    if not 2 <= len(x) <= _BRIGHT_MAX_N:
+        raise ValueError("the lattice has %d points per side, outside 2..%d"
+                         % (len(x), _BRIGHT_MAX_N))
+    return x, X, Y, [float(a), float(b), float(c), float(alph2)]
+
+
+def _lattice_axis(o):
+    """The vector X, Y are the meshgrid of (calc_SS re-reads them); ValueError if they are
+    not the meshgrid of one strictly increasing vector."""
+    X, Y = np.asarray(o.X, dtype=np.float64), np.asarray(o.Y, dtype=np.float64)
+    B = np.asarray(o.B)
+    if X.ndim != 2 or X.shape[0] != X.shape[1] or Y.shape != X.shape or B.shape != X.shape:
+        raise ValueError("X, Y and B must be square arrays of one shape")
+    x = X[0]
+    if not (np.array_equal(X, np.broadcast_to(x, X.shape)) and
+            np.array_equal(Y, np.broadcast_to(x[:, None], X.shape)) and
+            np.all(np.diff(x) > 0)):
+        raise ValueError("X, Y must be meshgrid(x, x) of one strictly increasing x")
+    if not 2 <= len(x) <= _BRIGHT_MAX_N:
+        raise ValueError("the lattice has %d points per side, outside 2..%d"
+                         % (len(x), _BRIGHT_MAX_N))
+    return np.ascontiguousarray(x)
+
+
+def _sspec_host(o):
+    """calc_SS's host half (scint_sim.py:901-925): the axes, each Doppler column's thetax,
+    (thetax + thetagx)**2 by the reference's scalar power (C pow, which is not always x*x),
+    and the scalars, each by the reference's expression."""
+    import math
+    fd = np.arange(-o.nf, o.nf, o.df)
+    td = np.arange(-o.nt, o.nt, o.dt)
+    if not (1 <= len(td) <= _BRIGHT_MAX_Q and 1 <= len(fd) <= _BRIGHT_MAX_Q):
+        raise ValueError("len(td) = %d and len(fd) = %d must be within 1..%d"
+                         % (len(td), len(fd), _BRIGHT_MAX_Q))
+    colx = fd - o.thetagx + o.thetarx
+    colq = np.array([math.pow(float(v + o.thetagx), 2) for v in colx])
+    rx2, ry2 = o.thetarx**2, o.thetary**2
+    scal = dict(half_df=float(0.5*o.df), jac_cap=float(2/o.df), jac_out=float(10**(-6)))
+    return fd, td, colx, colq, [float(o.thetagy), float(rx2), float(ry2)], scal
+
+
+def _run(objs, stages):
+    """One device pass of the given stages for a list of Brightness objects that share their
+    lattice and query grid.  Stages not run here take their inputs from the objects' B and
+    SS.  The host halves run (and raise) before any device work."""
+    import torch
+    ns = len(objs)
+    par = np.zeros((ns, _BRIGHT_NPAR))
+    hosts = [None] * ns
+    x = None
+    if stages & _BRIGHT_EFIELD:
+        for k, o in enumerate(objs):
+            x, X, Y, p = _efield_host(o)
+            hosts[k] = (x, X, Y)
+            par[k, :4] = p
+    q = None
+    if stages & _BRIGHT_SSPEC:
+        if x is None:
+            x = _lattice_axis(objs[0])
+        q = [_sspec_host(o) for o in objs]
+        for k, h in enumerate(q):
+            par[k, 4:] = h[4]
+    n = len(x) if x is not None else 2
+    ntd = nfd = 1
+    if stages & _BRIGHT_SSPEC:
+        fd, td = q[0][0], q[0][1]
+        ntd, nfd = len(td), len(fd)
+    elif stages & _BRIGHT_ACF:
+        ntd, nfd = np.shape(objs[0].SS)
+    z = lambda shape: D.empty(shape, torch.float64)   # noqa: E731
+    keep = []
+
+    def up(a):
+        t = D.upload(np.ascontiguousarray(a, dtype=np.float64))
+        keep.append(t)
+        return t.data_ptr()
+    m = _lib.Brightness()
+    m.nset, m.n, m.ntd, m.nfd, m.stages = ns, n, ntd, nfd, stages
+    out = {}
+    if stages & (_BRIGHT_EFIELD | _BRIGHT_SSPEC):
+        m.x, m.par = up(x), up(par)
+    if stages & _BRIGHT_EFIELD:
+        out["acf_efield"], out["B"] = z((ns, n, n)), z((ns, n, n))
+        m.rho, m.B = out["acf_efield"].data_ptr(), out["B"].data_ptr()
+    elif stages & _BRIGHT_SSPEC:
+        m.B = up(np.stack([np.asarray(o.B, dtype=np.float64) for o in objs]))
+    if stages & _BRIGHT_SSPEC:
+        bits = lattice_diagonals(x)
+        d_bits = D.upload(bits)
+        keep.append(d_bits)
+        m.diag, m.td = d_bits.data_ptr(), up(td)
+        m.colx, m.colq = up(np.stack([h[2] for h in q])), up(np.stack([h[3] for h in q]))
+        m.half_df, m.jac_cap, m.jac_out = (q[0][5][k] for k in ("half_df", "jac_cap", "jac_out"))
+        for k in ("thetax", "thetay", "jacobian", "SS", "LSS"):
+            out[k] = z((ns, ntd, nfd))
+        m.thetax, m.thetay, m.jac = (out[k].data_ptr() for k in ("thetax", "thetay", "jacobian"))
+        m.ss, m.lss = out["SS"].data_ptr(), out["LSS"].data_ptr()
+    elif stages & _BRIGHT_ACF:
+        m.ss = up(np.stack([np.asarray(o.SS, dtype=np.float64) for o in objs]))
+    if stages & _BRIGHT_ACF:
+        out["acf"] = z((ns, ntd, nfd))
+        m.acf = out["acf"].data_ptr()
+    _lib.check(_lib.lib.sb_brightness_f64(m, D.stream_ptr()))
+    host = {k: v.cpu().numpy() for k, v in out.items()}
+    for k, o in enumerate(objs):
+        if stages & _BRIGHT_EFIELD:
+            o.x, (o.X, o.Y) = hosts[k][0], hosts[k][1:]
+        if stages & _BRIGHT_SSPEC:
+            o.fd, o.td = q[k][0], q[k][1]
+        for name, arr in host.items():
+            setattr(o, name, arr[k])
+
+
+class Brightness():
+    """The delay-Doppler model of an anisotropic scattered image interfering with an
+    unscattered wave (Yao et al. 2020, modified by Coles; scint_sim.py:768-958).
+
+    Same constructor signature, defaults and attributes afterwards: ar alpha psi thetagx
+    thetagy thetarx thetary df dt dx nf nt nx ncuts x X Y acf_efield B fd td thetax thetay
+    jacobian SS LSS acf.  calc_brightness, calc_SS and calc_acf re-read the attributes the
+    reference reads and can be called on their own; calc_acf=True with calc_sspec=False
+    raises AttributeError on SS, as the reference does.  The axes and scalars are the
+    reference's numpy expressions; the e-field ACF, both 2-D DFTs (float64 matrix products on
+    the tensor cores), the secondary spectrum and its interpolation run on the device
+    (csrc/brightness.cu).  The interpolation is griddata's linear interpolant, evaluated
+    through the lattice's triangulation (lattice_diagonals), so it agrees with griddata to
+    rounding and is NaN where griddata is.
+
+    Deviations, raised as ValueError before any device work: a non-finite quadratic form
+    (ar = 0, for example), lattices of more than 1024 points per side, len(td) or len(fd)
+    above 4096, X / Y that are not meshgrid(x, x) of one increasing x, and a triangulation
+    with a simplex that is not half a lattice cell.  ``plot=True`` and the ``plot_*``
+    methods raise NotImplementedError.  brightness_batch evaluates many parameter sets in
+    one pass, each bit-identical to its own Brightness(...).
+    """
+
+    def __init__(self, ar=1.0, psi=0, alpha=1.67, thetagx=0, thetagy=0,
+                 thetarx=0, thetary=0, df=0.02, dt=0.08, dx=0.1,
+                 nf=10, nt=80, nx=30, ncuts=5, plot=False, contour=True,
+                 figsize=(10, 8), calc_sspec=True, calc_acf=True):
+        if plot:
+            raise NotImplementedError("plotting is outside the GPU hot path")
+        self.ar = ar
+        self.alpha = alpha
+        self.thetagx = thetagx
+        self.thetagy = thetagy
+        self.thetarx = thetarx
+        self.thetary = thetary
+        self.psi = psi
+        self.df = df
+        self.dt = dt
+        self.dx = dx
+        self.nf = nf
+        self.nt = nt
+        self.nx = nx
+        self.ncuts = ncuts
+        if calc_acf and not calc_sspec:
+            self.calc_brightness()
+            self.calc_acf()     # AttributeError on self.SS, as the reference
+        _run([self], _BRIGHT_EFIELD | (_BRIGHT_SSPEC if calc_sspec else 0) |
+             (_BRIGHT_ACF if calc_acf else 0))
+
+    def calc_brightness(self):
+        """acf_efield and B = |ifftshift(fft2(fftshift(acf_efield)))| (scint_sim.py:838-869)."""
+        _run([self], _BRIGHT_EFIELD)
+
+    def calc_SS(self):
+        """thetax, thetay, jacobian, SS and LSS from B on the lattice X, Y
+        (scint_sim.py:871-951)."""
+        _run([self], _BRIGHT_SSPEC)
+
+    def calc_acf(self):
+        """acf = real(fftshift(fft2(fftshift(SS)))) / its maximum (scint_sim.py:953-958)."""
+        _run([self], _BRIGHT_ACF)
+
+    def plot_acf_efield(self, figsize=(6, 6)):
+        raise NotImplementedError("plotting is outside the GPU hot path")
+
+    def plot_brightness(self, figsize=(6, 6)):
+        raise NotImplementedError("plotting is outside the GPU hot path")
+
+    def plot_sspec(self, figsize=(6, 6)):
+        raise NotImplementedError("plotting is outside the GPU hot path")
+
+    def plot_cuts(self, figsize=(6, 6)):
+        raise NotImplementedError("plotting is outside the GPU hot path")
+
+    def plot_acf(self, figsize=(6, 6), contour=False):
+        raise NotImplementedError("plotting is outside the GPU hot path")
+
+
+def brightness_batch(params, **shared):
+    """One Brightness per dict of ``params``, computed in batched device passes.
+
+    Each dict holds any of ``ar psi alpha thetagx thetagy thetarx thetary``; ``shared`` holds
+    the grid keywords ``nx dx nf df nt dt``; every other argument takes Brightness's default.
+    The sets share one lattice, one triangulation and one set of DFT twiddle matrices and run
+    in groups of at most 4 GiB of device memory.  Each returned object is bit-identical to
+    Brightness(**dict, **shared).  Every set's host half runs (and raises) before any device
+    work."""
+    bad = set(shared) - set(_BRIGHT_GRID_KEYS)
+    if bad:
+        raise TypeError("brightness_batch: %s are not grid keywords (%s)"
+                        % (sorted(bad), " ".join(_BRIGHT_GRID_KEYS)))
+    objs = []
+    for p in params:
+        bad = set(p) - set(_BRIGHT_SET_KEYS)
+        if bad:
+            raise TypeError("brightness_batch: %s are not per-set keywords (%s)"
+                            % (sorted(bad), " ".join(_BRIGHT_SET_KEYS)))
+        o = Brightness.__new__(Brightness)
+        kw = dict(ar=1.0, psi=0, alpha=1.67, thetagx=0, thetagy=0, thetarx=0, thetary=0,
+                  df=0.02, dt=0.08, dx=0.1, nf=10, nt=80, nx=30, ncuts=5)
+        kw.update(shared)
+        kw.update(p)
+        o.__dict__.update(kw)
+        objs.append(o)
+    if not objs:
+        return []
+    for o in objs:              # every error before the first launch
+        _efield_host(o)
+        _sspec_host(o)
+    x = _efield_host(objs[0])[0]
+    fd, td = _sspec_host(objs[0])[:2]
+    lattice_diagonals(x)
+    ntd, nfd = len(td), len(fd)
+    n2, nq = len(x) ** 2, ntd * nfd
+    twiddles = 16 * max(n2, ntd * ntd + nfd * nfd)
+    per_set = 8 * (2 * n2 + 7 * nq) + 16 * max(n2, nq)
+    group = int(max(1, min(65535, (_BRIGHT_GROUP_BYTES - twiddles) // per_set)))
+    for g in range(0, len(objs), group):
+        _run(objs[g:g + group], _BRIGHT_EFIELD | _BRIGHT_SSPEC | _BRIGHT_ACF)
+    return objs
