@@ -153,7 +153,22 @@ BRIGHTNESS_SIGS = {
     "sb_brightness_f64": (c_int, [ctypes.POINTER(Brightness), vp]),
 }
 
-for _name, (_res, _args) in list(_SIGS.items()) + list(BRIGHTNESS_SIGS.items()):
+
+class ScatIm(ctypes.Structure):
+    """struct sb_scatim (include/scint_b200_scatim.h)"""
+    _fields_ = [("nitem", c_int), ("mx", c_int), ("my", c_int), ("nx", c_int), ("ny", c_int),
+                ("shift", c_int), ("pitch", c_i64), ("sspec", vp), ("offset", vp), ("eta", vp),
+                ("tx", vp), ("fx", vp), ("ty", vp), ("fy", vp), ("ax", vp), ("ay", vp),
+                ("image", vp)]
+
+
+# entry points declared in include/scint_b200_scatim.h, outside scint_b200.h's set
+SCATIM_SIGS = {
+    "sb_scattered_image_f64": (c_int, [ctypes.POINTER(ScatIm), vp]),
+}
+
+for _name, (_res, _args) in (list(_SIGS.items()) + list(BRIGHTNESS_SIGS.items()) +
+                             list(SCATIM_SIGS.items())):
     _fn = getattr(lib, _name)   # AttributeError here = ABI mismatch, fail loudly
     _fn.restype = _res
     _fn.argtypes = _args

@@ -6,6 +6,7 @@
 
 #include "../../include/scint_b200.h"
 #include "../../include/scint_b200_brightness.h"
+#include "../../include/scint_b200_scatim.h"
 #include "common.cuh"
 #include "drivers.cuh"
 
@@ -595,6 +596,11 @@ int sb_acf_model_f64(const sb_acf_model* m, double* acf, double* efield, void* s
 int sb_brightness_f64(const sb_brightness* d, void* stream) {
     sb::StreamFence fence(stream);
     return sb::brightness(d, (cudaStream_t)stream);
+}
+
+int sb_scattered_image_f64(const sb_scatim* s, void* stream) {
+    sb::StreamFence fence(stream);
+    return sb::scattered_image(s, (cudaStream_t)stream);
 }
 
 int sb_convert_f64_f32(const double* src, float* dst, int64_t n, void* stream) {

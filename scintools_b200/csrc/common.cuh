@@ -33,7 +33,7 @@ const char* last_error();
 //                 conj_spectrum_c2c and gerchberg_saxton take PLANE0..2.  Drivers that
 //                 call neither use them too: sim_screen, sim_intensity, slow_ft,
 //                 inpaint_biharmonic, scint_fit, acf_model, scale_dyn_lambda, brightness
-//                 (PLANE0..3); eta_sweep
+//                 (PLANE0..3), scattered_image (PLANE0..1); eta_sweep
 //                 keeps its fp16 copy in PLANE3, eig_half_launch its Lanczos basis in PLANE4
 //   WS_TABLE      the column table and compact copy of thth_gather_source; the partial
 //                 sums of svd_topk, bandpass_cols and the mosaic tiles

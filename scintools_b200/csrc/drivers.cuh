@@ -3,6 +3,7 @@
 #pragma once
 #include "thth.cuh"
 #include "../../include/scint_b200_brightness.h"
+#include "../../include/scint_b200_scatim.h"
 
 namespace sb {
 
@@ -145,6 +146,9 @@ int acf_model(const sb_acf_model* m, double* acf, double* efield, cudaStream_t s
 
 // brightness.cu
 int brightness(const sb_brightness* d, cudaStream_t st);
+
+// scatim.cu
+int scattered_image(const sb_scatim* s, cudaStream_t st);
 
 // normsspec.cu
 int norm_sspec_rows(const float* sspec, int nr, int nc, const double* fdop, const double* tdel,

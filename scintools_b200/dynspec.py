@@ -21,7 +21,9 @@ the port), correct_dyn (dynspec.py:3325-3410 -> sb_svd_topk + sb_svd_apply, or t
 sb_bandpass_* passes), scale_dyn('lambda') (dynspec.py:3926-3957 -> sb_scale_dyn_lambda_f32),
 thetatheta_chunks / calc_wavefield / gerchberg_saxton (:1765-1896), cut_dyn (:3158-3271 ->
 sb_sspec_tiles_f32 + sb_acf_tiles_f32, every tile in one batched pass), and, through
-``arcfit.ArcFitMixin``, norm_sspec / fit_arc (:1920-2183, :970-1346).
+``arcfit.ArcFitMixin``, norm_sspec / fit_arc (:1920-2183, :970-1346), and
+calc_scattered_image (:3412-3582 -> sb_scattered_image_f64, batched over spectra by
+scattered_image_batch).
 
 Provenance: ``prep_thetatheta`` is the reference's dynspec.py:1348-1537 with the
 astropy units stripped, line for line (host scalar bookkeeping that SURVEY.md a11
@@ -762,6 +764,240 @@ def _cut_dyn_device(dyn, fnum, tnum, nfc, ntc, dtype):
     return D.download(sec, dtype), D.download(acf, dtype)
 
 
+# ----------------------------------------------------------------------
+# scattered image (csrc/scatim.cu)
+# ----------------------------------------------------------------------
+# sizes the device takes (include/scint_b200_scatim.h)
+_SCATIM_MIN_M = 4
+_SCATIM_MAX_MX, _SCATIM_MAX_MY = 65536, 32768     # crop box: delays, Doppler columns
+_SCATIM_MAX_SAMPLING = 4096
+_SCATIM_MAX_ITEMS = 65535
+_SCATIM_GROUP_BYTES = 4 << 30   # device memory of one batched pass, coefficients and images
+_SCATIM_TABLES = {}             # sha256 of an axis -> (knots, band factors)
+
+
+def spline_knots(x):
+    """The knots RectBivariateSpline(..., s=0) puts on the axis x: [x0]*4 + x[2:-2] +
+    [x_last]*4."""
+    x = np.asarray(x, dtype=np.float64)
+    return np.concatenate([np.repeat(x[:1], 4), x[2:-2], np.repeat(x[-1:], 4)])
+
+
+def spline_basis(t, x):
+    """FITPACK's fpbisp per point: clamp x to [t_3, t_m], take the interval l (the largest in
+    [3, m-1] with t_l <= x) and the four nonzero cubic B-splines there (fpbspl's recurrence).
+    Returns (l, h [len(x)][4]); B-spline l - 3 + i has the value h[:, i]."""
+    t = np.asarray(t, dtype=np.float64)
+    m = len(t) - 4
+    x = np.clip(np.asarray(x, dtype=np.float64), t[3], t[m])
+    l = np.clip(np.searchsorted(t, x, side="right") - 1, 3, m - 1)
+    h = np.zeros((len(x), 4))
+    h[:, 0] = 1.0
+    for j in range(1, 4):
+        hh = h[:, :j].copy()
+        h[:, 0] = 0.0
+        for i in range(1, j + 1):
+            tr, tl = t[l + i], t[l + i - j]
+            same = tr == tl
+            with np.errstate(all="ignore"):
+                f = hh[:, i - 1] / (tr - tl)
+                h[:, i - 1] = np.where(same, h[:, i - 1], h[:, i - 1] + f * (tr - x))
+                h[:, i] = np.where(same, 0.0, f * (x - tl))
+    return l, h
+
+
+def spline_tables(x):
+    """Knots and band factors of the interpolating cubic spline on the strictly increasing
+    axis x (m >= 4 points), cached by content.  The collocation matrix A[i][j] = B_j(x_i)
+    has two sub- and two superdiagonals and is totally positive, so A = L U without
+    pivoting is stable (de Boor).  Factors [5][m]: L[i][i-2], L[i][i-1], 1 / U[i][i],
+    U[i][i+1], U[i][i+2] (include/scint_b200_scatim.h)."""
+    import hashlib
+    x = np.ascontiguousarray(x, dtype=np.float64)
+    key = hashlib.sha256(x.tobytes()).hexdigest()
+    if key not in _SCATIM_TABLES:
+        m = len(x)
+        t = spline_knots(x)
+        l, h = spline_basis(t, x)
+        band = np.zeros((5, m))                       # A[i][i + d] at band[d + 2][i]
+        for i4 in range(4):
+            d = l - 3 + i4 - np.arange(m)
+            nz = h[:, i4] != 0
+            if np.any(np.abs(d[nz]) > 2):
+                raise ValueError("collocation matrix is not banded")
+            band[d[nz] + 2, np.arange(m)[nz]] = h[nz, i4]
+        lo2, lo1, dg, up1, up2 = (list(map(float, r)) for r in band)
+        for k in range(m):
+            p = dg[k]
+            if k + 1 < m:
+                f = lo1[k + 1] / p
+                lo1[k + 1] = f
+                dg[k + 1] -= f * up1[k]
+                up1[k + 1] -= f * up2[k]
+            if k + 2 < m:
+                f = lo2[k + 2] / p
+                lo2[k + 2] = f
+                lo1[k + 2] -= f * up1[k]
+                dg[k + 2] -= f * up2[k]
+        fac = np.array([lo2, lo1, 1.0 / np.array(dg), up1, up2])
+        _SCATIM_TABLES[key] = (t, fac)
+    return _SCATIM_TABLES[key]
+
+
+def _scatim_crop(shape, fdop, tdel, eta):
+    """calc_scattered_image's crop (dynspec.py:3514-3525) by the reference's own expressions:
+    StopIteration where its next() raises.  Returns the row and column ranges of a spectrum
+    of the given shape and the cropped (delay, Doppler) axes."""
+    fdop = np.asarray(fdop)
+    tdel = np.asarray(tdel)
+    nf = len(fdop)
+    below = eta * fdop**2 < np.max(tdel)
+    if not np.any(below):
+        raise StopIteration
+    flim = int(np.argmax(below))
+    rows = cols = slice(None)
+    if flim == 0:
+        above = tdel > eta * fdop[0] ** 2
+        if not np.any(above):
+            raise StopIteration
+        rows = slice(None, int(np.argmax(above)))
+        tdel = fdop[rows]
+    else:
+        cols = slice(flim - int(0.02*nf), nf - flim + int(0.02*nf))
+        fdop = fdop[cols]
+    r0, r1, _ = rows.indices(shape[0])
+    c0, c1, _ = cols.indices(shape[1])
+    return (r0, max(r1, r0)), (c0, max(c1, c0)), tdel, fdop
+
+
+def _scatim_grid(fdop, sampling):
+    """The image axes (dynspec.py:3553-3555) and scipy's checks: fdop_x, fdop_y."""
+    nx, ny = 2*sampling+1, sampling+1
+    fdop_x = np.linspace(-max(fdop), max(fdop), nx)
+    fdop_y = np.linspace(0, max(fdop), ny)
+    return fdop_x, fdop_y
+
+
+def _scatim_spline_check(x, y, shape):
+    """RectBivariateSpline(x, y, z)'s argument checks in its order (ValueError), then the
+    sizes the device takes."""
+    x, y = np.ravel(x), np.ravel(y)
+    if not np.all(np.diff(x) > 0.0):
+        raise ValueError('x must be strictly increasing')
+    if not np.all(np.diff(y) > 0.0):
+        raise ValueError('y must be strictly increasing')
+    if not x.size == shape[0]:
+        raise ValueError('x dimension of z must have same number of elements as x')
+    if not y.size == shape[1]:
+        raise ValueError('y dimension of z must have same number of elements as y')
+    if x.size < _SCATIM_MIN_M or y.size < _SCATIM_MIN_M:
+        raise ValueError("Error on entry, no approximation returned: a cubic spline needs at "
+                         "least 4 points per axis (%d x %d)" % (x.size, y.size))
+    if x.size > _SCATIM_MAX_MX or y.size > _SCATIM_MAX_MY:
+        raise ValueError("scattered image: crop of %d delays x %d Doppler columns is outside "
+                         "the supported sizes (up to %d x %d)"
+                         % (x.size, y.size, _SCATIM_MAX_MX, _SCATIM_MAX_MY))
+
+
+def _scatim_values_check(crop, plot_log, nx):
+    """The spectrum values the device takes: every dB value must give a finite linear power
+    (at most about 3082 dB).  A NaN makes every coefficient and so every pixel NaN, so with
+    plot_log the reference's plot_scattered_image raises ValueError (no finite non-zero
+    pixel after the shift); otherwise, with a one-pixel image (sampling=0), it raises
+    IndexError in centres_to_edges.  Raised here before any device work."""
+    top = np.max(crop)
+    if np.isnan(top):
+        if plot_log:
+            raise ValueError("zero-size array to reduction operation maximum which has no "
+                             "identity (the scattered image is NaN: the spectrum has NaN)")
+        return
+    with np.errstate(over="ignore"):
+        if np.isinf(10**(top / 10)):
+            raise ValueError("scattered image: a dB value of %r overflows the linear spectrum"
+                             % top)
+    if plot_log and nx < 2:
+        raise IndexError("index 1 is out of bounds for axis 0 with size 1 (plotting a "
+                         "one-pixel scattered image)")
+
+
+def _scatim_plan(shape, fdop, tdel, eta, sampling):
+    """Every host step of one item before the device: crop, grid, checks and tables."""
+    rows, cols, x, y = _scatim_crop(shape, fdop, tdel, eta)
+    fdop_x, fdop_y = _scatim_grid(y, sampling)
+    _scatim_spline_check(x, y, (rows[1] - rows[0], cols[1] - cols[0]))
+    if not 0 <= sampling <= _SCATIM_MAX_SAMPLING:
+        raise ValueError("scattered image: sampling %r is outside 0..%d"
+                         % (sampling, _SCATIM_MAX_SAMPLING))
+    return dict(rows=rows, cols=cols, x=x, y=y, fdop_x=fdop_x, fdop_y=fdop_y)
+
+
+def _scatim_device(spec, pitch, offsets, etas, plan, shift):
+    """Images [len(offsets)][nx][nx] of the items of one crop (device tensor spec, row pitch
+    elements, each item's crop at offsets[k]), in groups of at most _SCATIM_GROUP_BYTES."""
+    import torch
+    tx, fx = spline_tables(plan["x"])
+    ty, fy = spline_tables(plan["y"])
+    mx, my = len(plan["x"]), len(plan["y"])
+    nx, ny = len(plan["fdop_x"]), len(plan["fdop_y"])
+    up = lambda a: D.upload(np.ascontiguousarray(a, dtype=np.float64))   # noqa: E731
+    keep = [up(v) for v in (tx, fx, ty, fy, plan["fdop_x"], plan["fdop_y"])]
+    n = len(offsets)
+    out = D.empty((n, nx, nx), torch.float64)
+    per = 8 * (mx * my + nx * nx)
+    step = int(max(1, min(_SCATIM_MAX_ITEMS, _SCATIM_GROUP_BYTES // per)))
+    d_off = D.upload(np.asarray(offsets, dtype=np.int64))
+    d_eta = up(etas)
+    for k0 in range(0, n, step):
+        k1 = min(n, k0 + step)
+        s = _lib.ScatIm()
+        s.nitem, s.mx, s.my, s.nx, s.ny, s.shift = k1 - k0, mx, my, nx, ny, 1 if shift else 0
+        s.pitch, s.sspec = pitch, spec.data_ptr()
+        s.offset, s.eta = d_off[k0:].data_ptr(), d_eta[k0:].data_ptr()
+        s.tx, s.fx, s.ty, s.fy, s.ax, s.ay = (t.data_ptr() for t in keep)
+        s.image = out[k0:].data_ptr()
+        _lib.check(_lib.lib.sb_scattered_image_f64(s, D.stream_ptr()))
+    return out
+
+
+def scattered_image_batch(sspecs, fdop, tdel, eta, sampling=64, plot_log=True):
+    """The scattered image of every secondary spectrum of a stack, in batched device passes.
+
+    sspecs [..., ntdel, nfdop] (dB, e.g. Dynspec.cutsspec), fdop [nfdop], tdel [ntdel];
+    eta a scalar or one curvature per spectrum.  Returns (images [..., nx, nx], axes) with
+    nx = 2*sampling + 1.  Image k is bit-identical to
+    Dynspec.calc_scattered_image(input_sspec=sspecs[k], input_eta=eta[k], input_fdop=fdop,
+    input_tdel=tdel, sampling=sampling, plot_log=plot_log)'s scattered_image, and the same
+    errors are raised, before any device work.  axes [..., nx] holds each spectrum's
+    scattered_image_ax (they differ only where the curvatures give different crops).
+    Spectra whose curvatures give the same crop share a device pass.  Limits as calc_scattered_image's: crops of 4..65536 delays by
+    4..32768 Doppler columns, sampling 0..4096 (ValueError)."""
+    S = np.asarray(sspecs, dtype=np.float64)
+    if S.ndim < 2:
+        raise ValueError("sspecs must be [..., ntdel, nfdop]")
+    lead = S.shape[:-2]
+    S = np.ascontiguousarray(S.reshape((-1,) + S.shape[-2:]))
+    K, nr, nc = S.shape
+    etas = np.broadcast_to(np.asarray(eta, dtype=np.float64).ravel()
+                           if np.ndim(eta) else np.float64(eta), (K,))
+    plans, groups = [], {}
+    for k in range(K):
+        p = _scatim_plan((nr, nc), fdop, tdel, etas[k], sampling)
+        _scatim_values_check(S[k, p["rows"][0]:p["rows"][1], p["cols"][0]:p["cols"][1]],
+                             plot_log, len(p["fdop_x"]))
+        plans.append(p)
+        groups.setdefault((p["rows"], p["cols"]), []).append(k)
+    nx = 2 * sampling + 1
+    images = np.empty((K, nx, nx))
+    axes = np.array([p["fdop_x"] for p in plans]).reshape((K, nx))
+    if K:
+        spec = D.upload(S)
+        for (rows, cols), ks in groups.items():
+            offs = [k * nr * nc + rows[0] * nc + cols[0] for k in ks]
+            out = _scatim_device(spec, nc, offs, etas[ks], plans[ks[0]], plot_log)
+            images[ks] = D.download(out)
+    return images.reshape(lead + (nx, nx)), axes.reshape(lead + (nx,))
+
+
 class BasicDyn:
     """Container with the attributes Dynspec.load_dyn_obj reads
     (dynspec.py:4146-4230)."""
@@ -1237,6 +1473,98 @@ class Dynspec(ArcFitMixin):
         self.cutdyn = dyn.reshape(nfc, fnum, ntc, tnum).transpose(0, 2, 1, 3).astype(np.float64)
         self.cutsspec, self.cutacf = _cut_dyn_device(dyn, fnum, tnum, nfc, ntc, dtype)
         np.seterr(divide='ignore')      # calc_sspec's side effect (:3720)
+
+    # ------------------------------------------------------------------
+    # scattered image (csrc/scatim.cu)
+    # ------------------------------------------------------------------
+    def calc_scattered_image(self, input_sspec=None, input_eta=None, input_fdop=None,
+                             input_tdel=None, sampling=64, lamsteps=False, trap=False,
+                             ref_freq=1400, clean=True, s=None, veff=None, d=None,
+                             fit_arc=True, plot_fit=False, plot=False, plot_log=True,
+                             use_angle=False, use_spatial=False):
+        """The scattered image: the secondary spectrum mapped onto the sky along the arc
+        (reference dynspec.py:3412-3582).  Sets self.scattered_image [nx][nx] (float64,
+        nx = 2*sampling + 1) and self.scattered_image_ax (fdop_x), as the reference does.
+
+        The host runs the reference's own expressions for the spectrum and axes
+        (self.lamsspec / trapsspec / sspec, made by calc_sspec if missing; the delay axis is
+        self.tdel in every mode), the curvature (fit_arc(lamsteps, log_parabola=True) when
+        neither eta nor betaeta is set; betaeta converted at ref_freq with lamsteps; the
+        last delay over the last Doppler squared with fit_arc=False), the crop (the
+        reference's: with flim == 0 the delay axis becomes fdop[:tlim], and a negative
+        column start wraps as numpy's slice does) and the image grid.  The device computes
+        10**(sspec/10) of the crop, the interpolating bicubic spline of
+        RectBivariateSpline(tdel, fdop, .) by two banded solves, and its values at
+        ((fdop_x**2 + fdop_y**2) * eta, fdop_x) as FITPACK evaluates them (clamped to the
+        data range), times fdop_y, mirrored (csrc/scatim.cu).  It agrees with scipy's
+        fit to rounding: the banded LU and FITPACK's Givens QR differ in the last bits.
+
+        plot_log=True (the default) does not draw but applies what the reference's
+        plot_scattered_image does to the stored image in place: image -= min(image);
+        image += 1e-10.  Its errors come first: TypeError for use_angle / use_spatial with
+        s, veff (or d) left as None, ValueError when the image has no finite pixel, which
+        happens exactly when the crop holds a NaN, and IndexError for sampling=0 (a one-pixel
+        axis has no pixel edges).
+
+        Deviations: ``clean`` is accepted and skipped: the reference's griddata result is
+        assigned to a variable it never reads, so no output changes.  plot=True and
+        plot_fit=True raise NotImplementedError.  The spectrum is read as float64.  Raised as
+        ValueError before any device work: crops outside 4..65536 delays by 4..32768
+        Doppler columns (scipy also needs at least 4 points per axis), sampling outside
+        0..4096, and a dB value whose linear power overflows float64 (above about
+        3082 dB).  Every reference exception (StopIteration from the crop, AttributeError
+        from the curvature, scipy's ValueErrors, the plot checks above) is raised before any
+        device work.  scattered_image_batch does the same for a stack of spectra."""
+        if plot or plot_fit:
+            raise NotImplementedError("plotting is outside the GPU hot path")
+        if input_sspec is None:
+            if lamsteps:
+                if not hasattr(self, 'lamsspec'):
+                    self.calc_sspec(lamsteps=lamsteps)
+                sspec = self.lamsspec
+            elif trap:
+                if not hasattr(self, 'trapsspec'):
+                    self.calc_sspec(trap=trap)
+                sspec = self.trapsspec
+            else:
+                if not hasattr(self, 'sspec'):
+                    self.calc_sspec(lamsteps=lamsteps)
+                sspec = self.sspec
+            fdop = cp(self.fdop)
+            tdel = cp(self.tdel)
+        else:
+            sspec, fdop, tdel = input_sspec, input_fdop, input_tdel
+        nf, nt = len(fdop), len(tdel)
+        sspec = np.asarray(sspec, dtype=np.float64)
+        if input_eta is None and fit_arc:
+            if not hasattr(self, 'betaeta') and not hasattr(self, 'eta'):
+                self.fit_arc(lamsteps=lamsteps, log_parabola=True, plot=plot_fit)
+            if lamsteps:
+                c = 299792458.0  # m/s
+                beta_to_eta = c * 1e6 / ((ref_freq * 1e6)**2)
+                eta = self.betaeta / (self.freq / ref_freq)**2
+                eta = eta*beta_to_eta
+            else:
+                eta = self.eta
+        elif input_eta is None:
+            eta = tdel[nt-1] / fdop[nf-1]**2
+        else:
+            eta = input_eta
+        plan = _scatim_plan(sspec.shape, fdop, tdel, eta, sampling)
+        if plot_log:
+            # plot_scattered_image's axis conversions (dynspec.py:916-927), for their errors
+            c = 299792458.0  # m/s
+            if use_angle or use_spatial:
+                thetarad = (plan["fdop_x"] / (1e9 * self.freq)) * (c * s / (veff * 1000))
+                if not use_angle:
+                    ((thetarad * 180 / np.pi) * 3600) * (1 - s) * d * 1000
+        (r0, r1), (c0, c1) = plan["rows"], plan["cols"]
+        rows = sspec[r0:r1]
+        _scatim_values_check(rows[:, c0:c1], plot_log, len(plan["fdop_x"]))
+        spec = D.upload(rows)
+        out = _scatim_device(spec, sspec.shape[1], [c0], [float(eta)], plan, plot_log)
+        self.scattered_image = D.download(out)[0]
+        self.scattered_image_ax = plan["fdop_x"]
 
     # ------------------------------------------------------------------
     # scintillation scales (csrc/scintfit.cu)
