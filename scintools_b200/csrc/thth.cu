@@ -98,11 +98,21 @@ __global__ void thth_indexerr_table_kernel(const ThthGeom* __restrict__ geoms,
 // --------------------------------------------------------------------------
 // build the cropped theta-theta matrix for a batch of etas: STRICT UPPER
 // triangle only (the matrix is Hermitian with zero diagonal; the eigen kernel
-// uses every stored element twice).  grid = (tile pairs, etas in batch),
-// block = 32 x 8.  M[e] is [ld][ld] float2; inside the active 32x32 tiles
-// columns >= nred and the diagonal are zero, the lower triangle is not touched.
+// uses every stored element twice).  M[e] is [ld][ld] float2; inside the active
+// 32x32 tiles columns >= nred and the diagonal are zero, the lower triangle is not
+// touched.  Two kernels, one per gather source (thth_gather_source chooses):
+// thth_build_kernel reads the spectrum itself, thth_build_copy_kernel the compact copy.
 // --------------------------------------------------------------------------
-#define SB_BUILD_EB 8
+#define SB_BUILD_EB 8      // thth_build_kernel: curvatures per CTA
+#define SB_COPY_EB 32      // thth_build_copy_kernel: curvatures per CTA, one per lane
+#define SB_COPY_RB 4       // thth_build_copy_kernel: rows of a 32 x 32 tile per band
+
+// Diagnostic builds for profiles/probe_build_split.py, never the shipped library:
+// 1 = stores only (every gathered value is a constant), 2 = gathers only (the stores sit
+// behind a predicate the compiler cannot prove false and that is never true).
+#ifndef SB_BUILD_PROBE
+#define SB_BUILD_PROBE 0
+#endif
 
 // fp32 pair -> fp16 pair (re | im << 16, round to nearest even) for eig_half.cu
 __device__ __forceinline__ unsigned pack_f16x2(float2 v) {
@@ -153,9 +163,71 @@ __global__ void cs_absmax_kernel(const float2* __restrict__ cs, long long rows, 
     if ((threadIdx.x & 31) == 0) atomicMax(out, __float_as_uint(m));
 }
 
-// PACK == 2: also write the fp16 copy Mb that eig_half.cu iterates on,
-// scaled by the power of two that puts absmax * max Jacobian of this curvature just
-// below 2^15 (absmax: device scalar from cs_absmax_kernel, span: max |theta2 - theta1|).
+// Element of a valid pair (col >= 0) as thth_map stores it: the gathered value (hit: tau_inv
+// inside the spectrum, otherwise zero) conjugated in the mirrored half, |.| for the
+// incoherent map, times the Jacobian wf = sqrt|2 eta (th2 - th1)| (ththmod.py:104-107), with
+// nan_to_num.
+__device__ __forceinline__ float2 thth_element(float2 val, bool hit, bool conj, int coherent,
+                                               float wf) {
+    float2 v = make_float2(0.f, 0.f);
+    if (hit) {
+        v = val;
+        if (conj) v.y = -v.y;
+        if (!coherent) v = make_float2(hypotf(v.x, v.y), 0.f);
+    }
+    v.x *= wf;
+    v.y *= wf;
+    if (!(fabsf(v.x) <= 3.402823466e+38f) || !(fabsf(v.y) <= 3.402823466e+38f)) {
+        v.x = nan_to_num(v.x);
+        v.y = nan_to_num(v.y);
+    }
+    return v;
+}
+
+// One warp: row la (of 32) of a tile of the fp16 copy Mw that eig_half.cu iterates on, lane =
+// column holding element v (low: below the diagonal, stored as zero), scaled by the power of
+// two hscale; woff: word offset of the lane's column group in its block row, i.e.
+// ((2 ta + (la >> 4)) * ld / 8 + b / 8) * 128 + (la & 15) * 8 for row 32 ta + la, column b.
+// Block layout of eig_half.cu's tensor-core mat-vec: 512-byte blocks of 16 rows x 8 columns,
+// block (I, G) at ((I * ld / 8 + G) * 512) bytes, a block row = [re x 8 | im x 8] (32 bytes):
+// the 8 lanes of a column group trade halves so that lane i stores 4-byte word i of it -- one
+// store instruction, four full 32-byte sectors per warp (2-byte stores would be slower).
+// Elements on / below the diagonal of a diagonal block are zeros (the MMA has no masks);
+// 16 x 16 sub-blocks entirely below the diagonal are never read.
+__device__ __forceinline__ void thth_store_f16_row(unsigned* __restrict__ Mw, unsigned woff, bool diag,
+                                                   int la, float2 v, bool low, float hscale) {
+    const int lane = threadIdx.x & 31;
+    const unsigned h = low ? 0u : pack_f16x2(make_float2(v.x * hscale, v.y * hscale));
+    const int i8 = lane & 7, s0 = (lane & ~7) + 2 * (i8 & 3);
+    const unsigned ha = __shfl_sync(0xffffffffu, h, s0);
+    const unsigned hb = __shfl_sync(0xffffffffu, h, s0 + 1);
+    const unsigned word = i8 < 4 ? ((ha & 0xffffu) | (hb << 16)) : ((ha >> 16) | (hb & 0xffff0000u));
+    if (!(diag && (lane >> 4) < (la >> 4)) && (SB_BUILD_PROBE != 2 || woff == ~0u)) {
+        // the two 16-byte halves of a block row are stored swapped in rows 4-7 and 12-15: a
+        // LINEAR copy of the block into shared memory is then conflict free for both ldmatrix
+        // forms (eig_half.cu), so a bulk copy can fetch it
+        const unsigned swz = (unsigned)(((la & 15) >> 2) & 1) << 2;
+        Mw[woff + ((unsigned)i8 ^ swz)] = word;
+    }
+}
+
+// Per-curvature power of two of the fp16 copy: the one that puts absmax * max Jacobian of
+// this curvature just below 2^15 (absmax: device scalar from cs_absmax_kernel, span: max
+// |theta2 - theta1|); 2^floor(log2(2^15 / bound)) is the exponent field of the quotient.
+__device__ __forceinline__ float thth_hscale(double eta, const unsigned* __restrict__ absmax, float span) {
+    const float seta = sqrtf((float)(2.0 * eta));
+    const float bound = __uint_as_float(*absmax) * seta * sqrtf(span);
+    float hs = 1.f;
+    if (bound > 0.f && bound < 3.0e38f) {
+        const float q = 32768.f / bound;
+        hs = q >= 1.1754944e-38f ? __uint_as_float(__float_as_uint(q) & 0x7f800000u) : 1.1754944e-38f;
+    }
+    return hs;
+}
+
+// Gather from the spectrum itself (thth_build_kernel): grid = (groups of SB_BUILD_EB etas,
+// tile pairs), block = 32 x 8, lane = column of the tile.  PACK == 0: the fp32 triangle
+// only; PACK == 2: also the fp16 copy (thth_store_f16_row).
 //
 // Everything of thth_map's index math that does not depend on eta is computed
 // once per (row, column) pair and kept in registers while the CTA walks its
@@ -168,36 +240,22 @@ __global__ void cs_absmax_kernel(const float2* __restrict__ cs, long long rows, 
 // ROWS = 4 rows of the tile per thread (block = 32 x 8 threads).  Per curvature the
 // body runs in three phases -- (1) tau_inv and the offset of every row, (2) ALL the
 // gathers back to back, (3) Jacobian, clean-up, stores -- so that ROWS independent
-// gathers are in flight per thread.
-// COPY: the gathers read the compact copy of the spectrum columns the grid reaches
-// (ThthCopy, thth.cuh), delay axis contiguous, where neighbouring curvatures of a pair fall
-// in the same or the next 32-byte sector and the whole copy is re-read from L2
-// (thth_build_copy_kernel); otherwise the spectrum itself, where every gather costs a DRAM
-// sector of its own (thth_build_kernel).  thth_gather_source chooses.
-// PACK == 0: the fp32 triangle only.  PACK == 2: also the fp16 copy in the block layout
-// of eig_half.cu's tensor-core mat-vec: 512-byte blocks of 16 rows x 8 columns, block
-// (I, G) at ((I * ld / 8 + G) * 512) bytes, a block row = [re x 8 | im x 8] (the halves
-// swapped in rows 4-7, 12-15); the part of a diagonal block on / below the diagonal is
-// written as zeros (the MMA has no masks).
-// Three CTAs per SM (80 registers; spill stores per thread in the PACK == 2 instances on
-// sm_90: 40-44 bytes reading the spectrum, 12-20 bytes reading the copy).  Measured on the
-// headline sweep from the compact copy (H100 SXM, 700 W power limit, thth_build per
-// 1024-eta launch, copy included), variants built from one source and alternated in one
-// run: 1.76 ms as is; 1.78 ms with streaming (__stcs) stores of the triangles, alone or with
-// an L2 evict-last policy on the gathers; 1.84 ms with the tile pairs ordered by diagonal;
-// 1.78 ms with four CTAs per SM (64 registers, ~170 bytes of spills), which also slows the
-// gather from the spectrum itself (2.41 against 2.23 ms on an irregular grid).  None of
-// them is kept.
-template <int PACK, typename OFF, bool COPY>
-__device__ __forceinline__ void
-thth_build_body(const ThthGeom& g, const double* __restrict__ etas, int eta0, int nbatch,
-                int ld, const int* __restrict__ idx,
-                const int* __restrict__ nred, float2* __restrict__ M,
-                unsigned* __restrict__ Mb, const unsigned* __restrict__ absmax, float span,
-                const ThthCopy& copy) {
+// gathers are in flight per thread.  Every gather costs a DRAM sector of its own: the
+// curvatures of a pair walk down a spectrum column, rows apart.
+// Three CTAs per SM (80 registers; 40-44 bytes of spill stores per thread in the PACK == 2
+// instances on sm_90).  Measured on 1024 curvatures of an irregular 512-edge grid (H100 SXM,
+// 700 W power limit, thth_build per launch, alternated in one run with the variant): 2.38 ms;
+// 2.68-2.90 ms with the lane-per-curvature structure of thth_build_copy_kernel, whose 32
+// lanes then read 32 spectrum rows, each a DRAM sector of its own, per load instruction.
+// An earlier run measured four CTAs per SM at 2.41 against 2.23 ms.
+template <int PACK, typename OFF>
+__global__ void __launch_bounds__(256, 3)
+thth_build_kernel(ThthGeom g, const double* __restrict__ etas, int eta0, int nbatch,
+                  int ld, const int* __restrict__ idx,
+                  const int* __restrict__ nred, float2* __restrict__ M,
+                  unsigned* __restrict__ Mb, const unsigned* __restrict__ absmax, float span) {
     // eta is the FAST grid index: CTAs resident at the same time work on the
-    // same 32x32 tile for neighbouring curvatures, whose gathers fall on
-    // the same / adjacent delay bins for small |theta1^2 - theta2^2| (L2 reuse)
+    // same 32x32 tile for neighbouring curvatures
     // pair index -> (ta <= tb)
     constexpr int ROWS = 4, TY = 32 / ROWS;
     int p = blockIdx.y, ta = 0;
@@ -212,35 +270,24 @@ thth_build_body(const ThthGeom& g, const double* __restrict__ etas, int eta0, in
     double thj = 0.0;
     int ci[ROWS];
     double dk[ROWS];
-    int col[ROWS];          // CS column (COPY: slot of the copy) to gather; < 0: never a valid point
+    int col[ROWS];          // CS column to gather; < 0: never a valid point
     unsigned conj = 0u;     // bit k: the point lies in the mirrored (fd < 0) half
     float wk[ROWS];
 #pragma unroll
     for (int k = 0; k < ROWS; ++k) { ci[k] = -2; dk[k] = 0.0; col[k] = -1; wk[k] = 0.f; }
     const int e_end = min(nbatch, (int)(blockIdx.x + 1) * SB_BUILD_EB);
-    // per-curvature power-of-two scale of the fp16 copy, once per CTA (it was ~40 instructions
-    // of log2f / exp2f per thread and curvature): 2^floor(log2(2^15 / bound)) is the exponent
-    // field of the quotient
+    // per-curvature power-of-two scale of the fp16 copy, once per CTA
     SB_SHARED float s_hscale[SB_BUILD_EB];
     if (PACK != 0) {
         const int lin = ty * 32 + tx;
         if (lin < SB_BUILD_EB) {
             const int e = blockIdx.x * SB_BUILD_EB + lin;
-            float hs = 1.f;
-            if (e < e_end) {
-                const float seta = sqrtf((float)(2.0 * etas[eta0 + e]));
-                const float bound = __uint_as_float(*absmax) * seta * sqrtf(span);
-                if (bound > 0.f && bound < 3.0e38f) {
-                    const float q = 32768.f / bound;
-                    hs = q >= 1.1754944e-38f ? __uint_as_float(__float_as_uint(q) & 0x7f800000u) : 1.1754944e-38f;
-                }
-            }
-            s_hscale[lin] = hs;
+            s_hscale[lin] = e < e_end ? thth_hscale(etas[eta0 + e], absmax, span) : 1.f;
         }
         __syncthreads();
     }
     // eta-independent store offsets: fp32 element (row a0 + TY k, column b) and, PACK == 2,
-    // the 4-byte word of the fp16 block row this lane stores (see phase 3)
+    // the 4-byte word of the fp16 block row this lane stores (thth_store_f16_row)
     const unsigned foff0 = (unsigned)(ta * 32 + ty) * (unsigned)ld + (unsigned)b;
     const unsigned frow = (unsigned)TY * (unsigned)ld;
     const unsigned woff0 = ((unsigned)(2 * ta) * (unsigned)(ld >> 3) + (unsigned)(b >> 3)) * 128u +
@@ -262,7 +309,7 @@ thth_build_body(const ThthGeom& g, const double* __restrict__ etas, int eta0, in
         // power of two: |element| * hscale < 2^15
         const float hscale = PACK != 0 ? s_hscale[e - blockIdx.x * SB_BUILD_EB] : 1.f;
         // ---- phase 1: offsets
-        OFF off[ROWS];          // element offset into the CS / the copy (OFF = unsigned when it fits)
+        OFF off[ROWS];          // element offset into the CS (OFF = unsigned when it fits)
         unsigned hit = 0u;
 #pragma unroll
         for (int k = 0; k < ROWS; ++k) {
@@ -283,14 +330,7 @@ thth_build_body(const ThthGeom& g, const double* __restrict__ etas, int eta0, in
                     dk[k] = __dsub_rn(__dmul_rn(th1, th1), __dmul_rn(th2, th2));
                     wk[k] = sqrtf((float)fabs(th2 - th1));
                     bool mirrored;
-                    int c = thth_pair_column(g, th1, th2, &mirrored);
-                    if (COPY && c >= 0) {
-                        c = copy.slot_of_col[c];
-                        // a column the copy does not hold: the element stays zero, no
-                        // address is formed from it
-                        if (c < 0) atomicOr(copy.err, 1);
-                    }
-                    col[k] = c;
+                    col[k] = thth_pair_column(g, th1, th2, &mirrored);
                     if (mirrored) conj |= 1u << k;
                 }
             }
@@ -300,17 +340,15 @@ thth_build_body(const ThthGeom& g, const double* __restrict__ etas, int eta0, in
                 if (tqd > 0.0 && tqd < ntau_d) {            // tau_inv > 0 and < ntau (ththmod.py:100)
                     const int tq = (int)tqd;
                     const int r = (conj >> k) & 1u ? (int)g.ntau - tq : tq;
-                    off[k] = COPY ? (OFF)col[k] * (OFF)copy.tau_pitch + (OFF)r
-                                  : (OFF)r * (OFF)g.cs_pitch + (OFF)col[k];
+                    off[k] = (OFF)r * (OFF)g.cs_pitch + (OFF)col[k];
                     hit |= 1u << k;
                 }
             }
         }
         // ---- phase 2: the gathers, all in flight together (a miss reads element 0, ignored)
         float2 val[ROWS];
-        const float2* __restrict__ from = COPY ? copy.base : g.cs;
 #pragma unroll
-        for (int k = 0; k < ROWS; ++k) val[k] = __ldg(from + off[k]);
+        for (int k = 0; k < ROWS; ++k) val[k] = SB_BUILD_PROBE == 1 ? make_float2(1.f, 0.f) : __ldg(g.cs + off[k]);
         // ---- phase 3
 #pragma unroll
         for (int k = 0; k < ROWS; ++k) {
@@ -318,69 +356,220 @@ thth_build_body(const ThthGeom& g, const double* __restrict__ etas, int eta0, in
             const bool low = ta == tb && tx < la;       // below the diagonal: fp32 copy not stored
             float2 v = make_float2(0.f, 0.f);
             if (!low) {
-                if (col[k] >= 0) {
-                    if ((hit >> k) & 1u) {
-                        v = val[k];
-                        if ((conj >> k) & 1u) v.y = -v.y;
-                        if (!g.coherent) v = make_float2(hypotf(v.x, v.y), 0.f);
-                    }
-                    // Jacobian sqrt|2 eta (th2 - th1)| (ththmod.py:107)
-                    const float wf = seta * wk[k];
-                    v.x *= wf;
-                    v.y *= wf;
-                    if (!(fabsf(v.x) <= 3.402823466e+38f) || !(fabsf(v.y) <= 3.402823466e+38f)) {
-                        v.x = nan_to_num(v.x);
-                        v.y = nan_to_num(v.y);
-                    }
-                }
-                const unsigned o = foff0 + (unsigned)k * frow;
-                Me[o] = v;
+                if (col[k] >= 0)
+                    v = thth_element(val[k], (hit >> k) & 1u, (conj >> k) & 1u, g.coherent, seta * wk[k]);
+                if (SB_BUILD_PROBE != 2 || eta0 < 0) Me[foff0 + (unsigned)k * frow] = v;
             }
-            if (PACK == 2) {
-                // block row of 8 columns = [re x 8 | im x 8] (32 bytes): the 8 lanes of a column
-                // group trade halves so that lane i stores 4-byte word i of it -- one store
-                // instruction, four full 32-byte sectors per warp (2-byte stores would be slower).
-                // Elements on / below the diagonal of a diagonal block are zeros (the MMA has
-                // no masks); 16 x 16 sub-blocks entirely below the diagonal are never read.
-                const unsigned h = low ? 0u : pack_f16x2(make_float2(v.x * hscale, v.y * hscale));
-                const int i8 = tx & 7, s0 = (tx & ~7) + 2 * (i8 & 3);
-                const unsigned ha = __shfl_sync(0xffffffffu, h, s0);
-                const unsigned hb = __shfl_sync(0xffffffffu, h, s0 + 1);
-                const unsigned word = i8 < 4 ? ((ha & 0xffffu) | (hb << 16)) : ((ha >> 16) | (hb & 0xffff0000u));
-                if (!(ta == tb && (tx >> 4) < (la >> 4))) {
-                    // row a = 32 ta + ty + TY k: block row 2 ta + (la >> 4), row (la & 15) in it
-                    unsigned* Mw = Mb + (size_t)e * ld * ld;
-                    // the two 16-byte halves of a block row are stored swapped in rows 4-7 and
-                    // 12-15: a LINEAR copy of the block into shared memory is then conflict free for
-                    // both ldmatrix forms (eig_half.cu), so a bulk copy can fetch it
-                    const unsigned swz = (unsigned)(((la & 15) >> 2) & 1) << 2;
-                    Mw[woff0 + (unsigned)(la >> 4) * (unsigned)(ld >> 3) * 128u + (unsigned)((la & 15) - ty) * 8u +
-                       ((unsigned)i8 ^ swz)] = word;
-                }
-            }
+            if (PACK == 2)
+                thth_store_f16_row(Mb + (size_t)e * ld * ld, woff0 + (unsigned)(la >> 4) * (unsigned)(ld >> 3) * 128u +
+                                   (unsigned)((la & 15) - ty) * 8u, ta == tb, la, v, low, hscale);
         }
     }
 }
 
-template <int PACK, typename OFF>
-__global__ void __launch_bounds__(256, 3)
-thth_build_kernel(ThthGeom g, const double* __restrict__ etas, int eta0, int nbatch,
-                  int ld, const int* __restrict__ idx,
-                  const int* __restrict__ nred, float2* __restrict__ M,
-                  unsigned* __restrict__ Mb, const unsigned* __restrict__ absmax, float span) {
-    thth_build_body<PACK, OFF, false>(g, etas, eta0, nbatch, ld, idx, nred, M, Mb, absmax, span,
-                                      ThthCopy{nullptr, 0, 0, nullptr, nullptr});
+// Everything of thth_map's index math that does not depend on eta, for the pair of row
+// centre i and column centre j (th1 = theta of the column, th2 = theta of the row,
+// ththmod.py:86-87): d = theta1^2 - theta2^2, the slot in the copy of the spectrum column
+// of fd_inv with the Hermitian half-plane conjugation flag, and sqrt|theta2 - theta1|.
+// col < 0: the pair is never a valid point (i or j cropped, on / below the diagonal, on the
+// anti-diagonal, outside the fd axis, or a column the copy does not hold -- then the error
+// word is raised and no address is formed from it).
+struct ThthPair {
+    double d;
+    int col;
+    float w;
+    bool conj;
+};
+
+__device__ __forceinline__ ThthPair thth_pair_state(const ThthGeom& g, int i, int j,
+                                                    const ThthCopy& copy) {
+    ThthPair s{0.0, -1, 0.f, false};
+    if (i >= 0 && j > i && i + j != g.n - 1) {
+        const double th1 = g.th[j], th2 = g.th[i];
+        s.d = __dsub_rn(__dmul_rn(th1, th1), __dmul_rn(th2, th2));
+        s.w = sqrtf((float)fabs(th2 - th1));
+        int c = thth_pair_column(g, th1, th2, &s.conj);
+        if (c >= 0) {
+            c = copy.slot_of_col[c];
+            if (c < 0) atomicOr(copy.err, 1);
+        }
+        s.col = c;
+    }
+    return s;
 }
 
+// Gather from the compact copy of the spectrum columns the grid reaches (ThthCopy,
+// thth.cuh), delay axis contiguous.  grid = (groups of SB_COPY_EB = 32 etas, tile pairs),
+// block = 32 x 8; lane l of every warp works on curvature e0 + l, and a CTA whose group
+// starts past the batch returns at once.
+// * The crop of the 32 curvatures (idx rows, -1 past nred) for the tile's rows and columns
+//   is staged in shared memory once per CTA.  The pair state (ThthPair) of every element is
+//   computed once, by one thread, for the crop of the first curvature that has the tile (the
+//   reference); a lane whose own crop puts other centres on the element's row or column (bit
+//   masks per lane, made once) computes its own.  At the benchmark's sizes every curvature
+//   of a group has the same crop.  The states of the next band are computed while the
+//   current one is stored (two buffers).
+// * Gathers, per band of SB_COPY_RB rows: a warp walks elements, its 32 lanes gather the
+//   element for 32 neighbouring curvatures, whose delay bins are close: on the benchmark's
+//   grid one load instruction touches 15 distinct 32-byte sectors of the copy on average
+//   (counted on the host from its axes) instead of 32, one per lane, when the lanes ran
+//   over columns.  Per lane only tau_inv = floor((eta d - tau0 + dtau/2) / dtau)
+//   remains (the same fp64 operations in the same order as thth_point, so the bins stay
+//   bit-exact).  K = 2 elements per step (offsets, both gathers, then the elements) into a
+//   shared tile [curvature][element].
+// * Stores: per curvature and row, a warp writes the 32 columns of the fp32 triangle (256
+//   coalesced bytes) and, PACK == 2, the row of the fp16 blocks (thth_store_f16_row).
+// Four CTAs per SM: 64 registers, no spills, 47 KB of static shared memory each.  Measured on
+// the headline sweep (H100 SXM, 700 W power limit, thth_build per 1024-eta launch, the 0.24
+// ms copy included; variants built from one source and alternated with the previous kernel,
+// 1.72-1.76 ms, in two runs): 1.35-1.37 ms; 1.45-1.47 ms with three CTAs per SM and K = 4;
+// 1.63 ms with K = 8 (spills); 1.58 ms with one band per CTA, no band loop; 1.85-1.98 ms
+// with 128-thread CTAs of two-row bands.  The lane-per-column kernel before it took 1.76 ms,
+// and 1.78-1.84 ms with streaming stores of the triangles, an L2 evict-last policy on the
+// gathers, the tile pairs ordered by diagonal, or four CTAs per SM.
 template <int PACK, typename OFF>
-__global__ void __launch_bounds__(256, 3)
+__global__ void __launch_bounds__(256, 4)
 thth_build_copy_kernel(ThthGeom g, const double* __restrict__ etas, int eta0, int nbatch,
                        int ld, const int* __restrict__ idx,
                        const int* __restrict__ nred, float2* __restrict__ M,
                        unsigned* __restrict__ Mb, const unsigned* __restrict__ absmax, float span,
                        ThthCopy copy) {
-    thth_build_body<PACK, OFF, true>(g, etas, eta0, nbatch, ld, idx, nred, M, Mb, absmax, span,
-                                     copy);
+    constexpr int EB = SB_COPY_EB, RB = SB_COPY_RB, NEL = RB * 32, NW = 8, K = 2;
+    static_assert(EB == 32 && NEL % (NW * K) == 0 && NEL + 32 <= NW * 32,
+                  "one curvature per lane, whole steps, a spare warp for the masks");
+    // pair index -> (ta <= tb)
+    int p = blockIdx.y, ta = 0;
+    const int T = ld / 32;
+    while (p >= T - ta) { p -= T - ta; ++ta; }
+    const int tb = ta + p;
+    const bool diag = ta == tb;
+    const int lane = threadIdx.x, warp = threadIdx.y, tid = warp * 32 + lane;
+    const int e0 = blockIdx.x * EB, ne = min(EB, nbatch - e0);
+
+    SB_SHARED int s_i[EB][33];                   // row centres of each curvature, -1: none
+    SB_SHARED int s_j[EB][33];                   // column centres
+    SB_SHARED float s_hscale[EB];
+    SB_SHARED unsigned s_act;                    // bit l: curvature e0 + l has this tile
+    SB_SHARED unsigned s_mi[EB], s_mj[EB];       // bit r / c: same row / column centre as the reference
+    SB_SHARED ThthPair s_ref[2][NEL];            // pair states of a band under the reference crop
+    SB_SHARED float2 s_v[EB][NEL + 1];           // gathered elements (+1: lanes on different banks)
+
+    for (int t = tid; t < EB * 64; t += NW * 32) {
+        const int l = t >> 6, c = t & 63;
+        int v = -1;
+        if (l < ne) {
+            const int x = c < 32 ? tb * 32 + c : ta * 32 + (c - 32);
+            if (x < nred[eta0 + e0 + l]) v = idx[(size_t)(eta0 + e0 + l) * ld + x];
+        }
+        if (c < 32) s_j[l][c] = v;
+        else s_i[l][c - 32] = v;
+    }
+    if (warp == 0) {
+        bool act = false;
+        float hs = 1.f;
+        if (lane < ne) {
+            const int e = eta0 + e0 + lane;
+            act = tb * 32 < nred[e];                 // otherwise never read by the eigen kernel
+            if (PACK != 0) hs = thth_hscale(etas[e], absmax, span);
+        }
+        s_hscale[lane] = hs;
+        const unsigned m = __ballot_sync(0xffffffffu, act);
+        if (lane == 0) s_act = m;
+    }
+    __syncthreads();
+    const unsigned act = s_act;
+    if (act == 0u) return;
+    const int ref = __ffs(act) - 1;
+    // pair states of band `band` under the reference crop, one element per thread tid < NEL
+    auto ref_states = [&](int band, ThthPair* out) {
+        const int r = band * RB + (tid >> 5), c = tid & 31;
+        out[tid] = diag && c < r ? ThthPair{0.0, -1, 0.f, false}
+                                 : thth_pair_state(g, s_i[ref][r], s_j[ref][c], copy);
+    };
+    if (tid < NEL) {
+        ref_states(0, s_ref[0]);
+    } else if (tid < NEL + 32) {
+        const int l = tid - NEL;
+        unsigned mi = 0u, mj = 0u;
+#pragma unroll
+        for (int c = 0; c < 32; ++c) {
+            mi |= (unsigned)(s_i[l][c] == s_i[ref][c]) << c;
+            mj |= (unsigned)(s_j[l][c] == s_j[ref][c]) << c;
+        }
+        s_mi[l] = mi;
+        s_mj[l] = mj;
+    }
+    __syncthreads();
+
+    const bool mine = (act >> lane) & 1u;
+    const double eta = mine ? etas[eta0 + e0 + lane] : 0.0;
+    const float seta = sqrtf((float)(2.0 * eta));
+    const unsigned mi = s_mi[lane], mj = s_mj[lane];
+    const double ntau_d = (double)g.ntau;
+    int buf = 0;
+    for (int band = 0; band < 32 / RB; ++band, buf ^= 1) {
+        const int r0 = band * RB;                // first tile row of the band
+        // ---- gathers: lane = curvature e0 + lane, warp w on elements w, w + NW, ...
+        const ThthPair* sref = s_ref[buf];
+#pragma unroll 1
+        for (int q0 = warp; q0 < NEL; q0 += NW * K) {
+            ThthPair ps[K];
+            OFF off[K];         // element offset into the copy (OFF = unsigned when it fits)
+            unsigned hit = 0u;
+#pragma unroll
+            for (int k = 0; k < K; ++k) {
+                const int el = q0 + NW * k, r = r0 + (el >> 5), c = el & 31;
+                off[k] = 0;
+                ps[k].col = -1;
+                if (!mine || (diag && c < r)) continue;     // lower triangle: not stored
+                if ((mi >> r) & (mj >> c) & 1u) ps[k] = sref[el];
+                else ps[k] = thth_pair_state(g, s_i[lane][r], s_j[lane][c], copy);
+                if (ps[k].col >= 0) {
+                    const double aa = __dadd_rn(__dsub_rn(__dmul_rn(eta, ps[k].d), g.tau0), g.half_dtau);
+                    const double tqd = floor_div_fast(aa, g.dtau, g.inv_dtau);
+                    if (tqd > 0.0 && tqd < ntau_d) {        // tau_inv > 0 and < ntau (ththmod.py:100)
+                        const int tq = (int)tqd;
+                        const int rr = ps[k].conj ? (int)g.ntau - tq : tq;
+                        off[k] = (OFF)ps[k].col * (OFF)copy.tau_pitch + (OFF)rr;
+                        hit |= 1u << k;
+                    }
+                }
+            }
+            // all K gathers in flight together (a miss reads element 0, ignored)
+            float2 val[K];
+#pragma unroll
+            for (int k = 0; k < K; ++k)
+                val[k] = SB_BUILD_PROBE == 1 ? make_float2(1.f, 0.f) : __ldg(copy.base + off[k]);
+#pragma unroll
+            for (int k = 0; k < K; ++k) {
+                const int el = q0 + NW * k;
+                if (!mine || (diag && (el & 31) < r0 + (el >> 5))) continue;
+                s_v[lane][el] = ps[k].col >= 0 ? thth_element(val[k], (hit >> k) & 1u, ps[k].conj,
+                                                              g.coherent, seta * ps[k].w)
+                                               : make_float2(0.f, 0.f);
+            }
+        }
+        __syncthreads();
+        // the next band's reference states, while this one is stored
+        if (tid < NEL && band + 1 < 32 / RB) ref_states(band + 1, s_ref[buf ^ 1]);
+
+        // ---- stores: warp w on (curvature, band row) q = w, w + NW, ..., lane = column
+#pragma unroll 1
+        for (int q = warp; q < EB * RB; q += NW) {
+            const int l = q / RB, la = r0 + q % RB;
+            if (!((act >> l) & 1u)) continue;
+            const bool low = diag && lane < la;     // below the diagonal: fp32 copy not stored
+            const float2 v = low ? make_float2(0.f, 0.f) : s_v[l][(la - r0) * 32 + lane];
+            const size_t e = (size_t)(e0 + l);
+            if (!low && (SB_BUILD_PROBE != 2 || eta0 < 0))
+                M[e * ld * ld + (unsigned)(ta * 32 + la) * (unsigned)ld + (unsigned)(tb * 32 + lane)] = v;
+            if (PACK == 2)
+                thth_store_f16_row(Mb + e * ld * ld, ((unsigned)(2 * ta + (la >> 4)) * (unsigned)(ld >> 3) +
+                                   (unsigned)((tb * 32 + lane) >> 3)) * 128u + (unsigned)(la & 15) * 8u,
+                                   diag, la, v, low, s_hscale[l]);
+        }
+        __syncthreads();
+    }
 }
 
 // --------------------------------------------------------------------------
@@ -795,21 +984,24 @@ static void thth_build_launch(const ThthGeom& g, const ThthCopy& copy, const dou
                               float2* d_M, unsigned* d_Mb, const unsigned* d_absmax, float span,
                               cudaStream_t st) {
     const int T = ld / 32;
-    const dim3 grid((nb + SB_BUILD_EB - 1) / SB_BUILD_EB, T * (T + 1) / 2), block(32, 8);
+    const dim3 block(32, 8);
     if (copy.base) {
+        const dim3 grid((nb + SB_COPY_EB - 1) / SB_COPY_EB, T * (T + 1) / 2);
         if ((unsigned long long)copy.nslots * (unsigned long long)copy.tau_pitch < (1ull << 32))
             thth_build_copy_kernel<PACK, unsigned><<<grid, block, 0, st>>>(
                 g, d_etas, e0, nb, ld, d_idx, d_nred, d_M, d_Mb, d_absmax, span, copy);
         else
             thth_build_copy_kernel<PACK, size_t><<<grid, block, 0, st>>>(
                 g, d_etas, e0, nb, ld, d_idx, d_nred, d_M, d_Mb, d_absmax, span, copy);
-    } else if ((unsigned long long)g.ntau * (unsigned long long)g.cs_pitch < (1ull << 32)) {
+        return;
+    }
+    const dim3 grid((nb + SB_BUILD_EB - 1) / SB_BUILD_EB, T * (T + 1) / 2);
+    if ((unsigned long long)g.ntau * (unsigned long long)g.cs_pitch < (1ull << 32))
         thth_build_kernel<PACK, unsigned><<<grid, block, 0, st>>>(g, d_etas, e0, nb, ld, d_idx,
                                                                   d_nred, d_M, d_Mb, d_absmax, span);
-    } else {
+    else
         thth_build_kernel<PACK, size_t><<<grid, block, 0, st>>>(g, d_etas, e0, nb, ld, d_idx,
                                                                 d_nred, d_M, d_Mb, d_absmax, span);
-    }
 }
 
 // fp32 strict upper triangles [nb][ld][ld] of etas e0 .. e0 + nb - 1 (no fp16 copy)
