@@ -167,8 +167,14 @@ SCATIM_SIGS = {
     "sb_scattered_image_f64": (c_int, [ctypes.POINTER(ScatIm), vp]),
 }
 
+# entry points declared in include/scint_b200_clean.h, outside scint_b200.h's set
+CLEAN_SIGS = {
+    "sb_dyn_zero_counts_f64": (c_int, [vp, c_int, c_int, c_int, c_int, vp, vp, vp]),
+    "sb_zap_f64": (c_int, [vp, c_i64, c_dbl, vp, vp]),
+}
+
 for _name, (_res, _args) in (list(_SIGS.items()) + list(BRIGHTNESS_SIGS.items()) +
-                             list(SCATIM_SIGS.items())):
+                             list(SCATIM_SIGS.items()) + list(CLEAN_SIGS.items())):
     _fn = getattr(lib, _name)   # AttributeError here = ABI mismatch, fail loudly
     _fn.restype = _res
     _fn.argtypes = _args

@@ -7,6 +7,7 @@
 #include "../../include/scint_b200.h"
 #include "../../include/scint_b200_brightness.h"
 #include "../../include/scint_b200_scatim.h"
+#include "../../include/scint_b200_clean.h"
 #include "common.cuh"
 #include "drivers.cuh"
 
@@ -574,6 +575,18 @@ int sb_medfilt_masked_f64(const double* img, int32_t nf, int32_t nt, const int32
                           int32_t kh, int32_t kw, double nan_value, double* out, void* stream) {
     sb::StreamFence fence(stream);
     return sb::medfilt_masked(img, nf, nt, pix, n, kh, kw, nan_value, out, (cudaStream_t)stream);
+}
+
+int sb_dyn_zero_counts_f64(const double* dyn, int32_t nf, int32_t nt, int32_t row0, int32_t row1,
+                           int32_t* row_counts, int32_t* col_counts, void* stream) {
+    sb::StreamFence fence(stream);
+    return sb::dyn_zero_counts(dyn, nf, nt, row0, row1, row_counts, col_counts,
+                               (cudaStream_t)stream);
+}
+
+int sb_zap_f64(double* dyn, int64_t n, double sigma, double* stats, void* stream) {
+    sb::StreamFence fence(stream);
+    return sb::zap(dyn, n, sigma, stats, (cudaStream_t)stream);
 }
 
 int sb_scint_fit_1d(const sb_scint_fit* fits, int32_t nfit, double* out, int32_t* info,

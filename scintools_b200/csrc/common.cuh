@@ -22,10 +22,11 @@ const char* last_error();
 //   WS_SCALARS    the ScalarBlock below
 //   WS_INDEX      index tables of eta_sweep, thin_sweep, chisq_sweep; rev_map's bin counts;
 //                 vlbi_retrieval's and asymmetry_batch's per-call arrays; the chirp-z result
-//                 of conj_spectrum_c2c; the per-tile sums of sspec_tiles and acf_tiles
+//                 of conj_spectrum_c2c; the per-tile sums of sspec_tiles and acf_tiles;
+//                 zap's select state and digit histogram
 //   WS_BATCH      the batch slab of eta_sweep, thin_sweep, chisq_sweep, vlbi_retrieval,
 //                 asymmetry_batch; herm_eigvec's basis; the padded chunk of
-//                 conj_spectrum_c2c; gerchberg_saxton; svd_topk
+//                 conj_spectrum_c2c; gerchberg_saxton; svd_topk; zap's candidate keys
 //   WS_PLANE0..4  the FFT engine: chirp_fft2 takes all five (through ifft2_chirp,
 //                 ifft2_planes, ifft2_conj_any and the chirp-z conj_spectrum); the radix
 //                 2-D transforms of sspec, acf, acf_sspec, sspec_tiles, acf_tiles,

@@ -4,6 +4,7 @@
 #include "thth.cuh"
 #include "../../include/scint_b200_brightness.h"
 #include "../../include/scint_b200_scatim.h"
+#include "../../include/scint_b200_clean.h"
 
 namespace sb {
 
@@ -136,6 +137,11 @@ int inpaint_biharmonic(const double* img, int nf, int nt, const int* pix, int n,
                        cudaStream_t st);
 int medfilt_masked(const double* img, int nf, int nt, const int* pix, int n, int kh, int kw,
                    double nan_value, double* out, cudaStream_t st);
+
+// clean.cu
+int dyn_zero_counts(const double* dyn, int nf, int nt, int row0, int row1, int* row_counts,
+                    int* col_counts, cudaStream_t st);
+int zap(double* x, long long n, double sigma, double* stats, cudaStream_t st);
 
 // scintfit.cu
 int scint_fit_1d(const sb_scint_fit* fits, int nfit, double* out, int* info, cudaStream_t st);

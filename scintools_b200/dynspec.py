@@ -9,15 +9,18 @@ the reference for the arc-measurement hot path:
   thetatheta_single  dynspec.py:1539-1655  -> sb_cs_f32 + sb_eta_sweep
   fit_thetatheta     dynspec.py:1657-1763  -> per chunk ththmod.single_search
 
-Everything outside that path (file I/O, cleaning other than refill, plotting, the lmfit
-models other than get_scint_params's) is deliberately not here: use the reference for
-those and hand the arrays over with ``BasicDyn`` exactly as the reference's tutorials do.
+Real data starts here too: ``Dynspec(filename=...)`` reads a psrflux file (load_file,
+remove_short_subs, info, auto_processing; dynspec.py:144-257, :422-440, :4130-4143, host
+only, with np.loadtxt), ``trim_edges`` (:259-328) takes its zero counts from
+sb_dyn_zero_counts_f64 and crops once on the host, ``zap`` (:3856-3870 -> sb_zap_f64) finds
+both medians by a radix select on the device, and ``crop_dyn`` (:3816-3854) and ``__add__``
+(:81-142) are the reference's indexing on the host.  Not here: write_file, sort_dyn,
+plotting, and the lmfit models other than get_scint_params's.
 Units: times in s, freqs in MHz, eta in s^3, edges in mHz, tau in us.
 
 Also here: get_scint_params / get_acf_tilt (dynspec.py:2283-3156 -> sb_scint_fit_1d /
 sb_scint_fit_2d, batched over spectra by get_scint_params_batch), refill (dynspec.py:3273-3323 -> sb_inpaint_biharmonic_f64 or
-sb_medfilt_masked_f64; the first step of real data, so this is the one piece of cleaning in
-the port), correct_dyn (dynspec.py:3325-3410 -> sb_svd_topk + sb_svd_apply, or the
+sb_medfilt_masked_f64), correct_dyn (dynspec.py:3325-3410 -> sb_svd_topk + sb_svd_apply, or the
 sb_bandpass_* passes), scale_dyn('lambda') (dynspec.py:3926-3957 -> sb_scale_dyn_lambda_f32),
 thetatheta_chunks / calc_wavefield / gerchberg_saxton (:1765-1896), cut_dyn (:3158-3271 ->
 sb_sspec_tiles_f32 + sb_acf_tiles_f32, every tile in one batched pass), and, through
@@ -29,8 +32,11 @@ Provenance: ``prep_thetatheta`` is the reference's dynspec.py:1348-1537 with the
 astropy units stripped, line for line (host scalar bookkeeping that SURVEY.md a11
 keeps in Python; identical attributes are the contract).  The chunk loops of
 ``fit_thetatheta`` / ``thetatheta_chunks`` follow :1680-1712 / :1790-1828 the same
-way.  Restated reference glue, not new design.
+way, and so do load_file, remove_short_subs, info, auto_processing, crop_dyn,
+__add__ and trim_edges's bookkeeping.  Restated reference glue, not new design.
 """
+import os
+import time
 from copy import deepcopy as cp
 
 import numpy as np
@@ -998,6 +1004,37 @@ def scattered_image_batch(sspecs, fdop, tdel, eta, sampling=64, plot_log=True):
     return images.reshape(lead + (nx, nx)), axes.reshape(lead + (nx,))
 
 
+# ----------------------------------------------------------------------
+# band edges (csrc/clean.cu)
+# ----------------------------------------------------------------------
+def _zero_counts(dyn):
+    """Each row's count of entries of dyn that are 0 or NaN, and a function of the kept rows
+    (r0, r1) that returns each column's count over them (sb_dyn_zero_counts_f64).  The array
+    is read once for the first, and the smaller of the trimmed bands and the kept rows once
+    more for the second."""
+    import torch
+    nr, nc = np.shape(dyn)
+    d = D.upload(np.ascontiguousarray(dyn, dtype=np.float64))
+    rows = D.empty((nr,), torch.int32)
+    cols = D.empty((3, nc), torch.int32)
+
+    def count(a, b, rc, cc):
+        _lib.check(_lib.lib.sb_dyn_zero_counts_f64(d.data_ptr(), nr, nc, a, b, D.ptr(rc),
+                                                   D.ptr(cc), D.stream_ptr()))
+
+    def kept(r0, r1):
+        if nr - (r1 - r0) <= r1 - r0:
+            count(0, r0, None, cols[1])
+            count(r1, nr, None, cols[2])
+            c = D.download(cols).astype(np.int64)
+            return c[0] - c[1] - c[2]
+        count(r0, r1, None, cols[1])
+        return D.download(cols[1]).astype(np.int64)
+
+    count(0, nr, rows, cols[0])
+    return D.download(rows).astype(np.int64), kept
+
+
 class BasicDyn:
     """Container with the attributes Dynspec.load_dyn_obj reads
     (dynspec.py:4146-4230)."""
@@ -1030,9 +1067,9 @@ class Dynspec(ArcFitMixin):
                  lamsteps=False, remove_short_subs=True, subint_thresh=2.33,
                  mjd=None):
         if filename:
-            raise NotImplementedError(
-                "psrflux file I/O is outside the GPU hot path: load with "
-                "scintools.Dynspec and pass the object as dyn=")
+            self.load_file(filename, verbose=verbose, process=process,
+                           lamsteps=lamsteps, subint_thresh=subint_thresh,
+                           remove_short_subs=remove_short_subs, mjd=mjd)
         elif dyn is not None:
             self.load_dyn_obj(dyn, verbose=verbose, process=process,
                               lamsteps=lamsteps)
@@ -1064,6 +1101,229 @@ class Dynspec(ArcFitMixin):
             self.calc_sspec(lamsteps=lamsteps)
         if verbose:
             print("LOADED DYNSPEC OBJECT {0}".format(self.name))
+
+    # ------------------------------------------------------------------
+    # psrflux files and joining (host only: parsing, indexing, bookkeeping)
+    # ------------------------------------------------------------------
+    def __add__(self, other):
+        """Concatenation in time with the gap between the observations zero-filled
+        (reference dynspec.py:81-142).  ``a += b`` goes through here too."""
+        print("Now adding {} ...".format(other.name))
+        if self.freq != other.freq \
+                or self.bw != other.bw or self.df != other.df:
+            print("WARNING: Code does not yet account for different \
+                  frequency properties")
+        bw = self.bw
+        df = self.df
+        freqs = self.freqs
+        freq = self.freq
+        nchan = self.nchan
+        dt = self.dt
+        timegap = round((other.mjd - self.mjd)*86400
+                        - self.tobs, 1)  # time between two dynspecs
+        extratimes = np.arange(0, timegap, dt)
+        if timegap < dt:
+            extratimes = [0]
+            nextra = 0
+        else:
+            nextra = len(extratimes)
+        dyngap = np.zeros([np.shape(self.dyn)[0], nextra])
+        name = self.name.split('.')[0] + "+" + other.name.split('.')[0] \
+            + ".dynspec"
+        header = self.header + other.header
+        nsub = self.nsub + nextra + other.nsub
+        tobs = self.tobs + timegap + other.tobs
+        times = np.linspace(0, tobs, nsub)
+        mjd = np.min([self.mjd, other.mjd])  # mjd for earliest dynspec
+        newdyn = np.concatenate((self.dyn, dyngap, other.dyn), axis=1)
+        newdyn = BasicDyn(newdyn, name=name, header=header, times=times,
+                          freqs=freqs, nchan=nchan, nsub=nsub, bw=bw,
+                          df=df, freq=freq, tobs=tobs, dt=dt, mjd=mjd)
+        return Dynspec(dyn=newdyn, verbose=False, process=False)
+
+    def load_file(self, filename, verbose=True, process=False, lamsteps=False,
+                  remove_short_subs=True, subint_thresh=2.33, mjd=None):
+        """Load a psrflux dynamic spectrum (reference dynspec.py:144-230): the first
+        ``MJD0:`` header line gives self.mjd unless ``mjd`` is given (neither:
+        AttributeError), rows are flipped into ascending frequency when the file lists
+        them descending, and short leading sub-integrations are removed when the
+        sub-integration times vary.  A file of other than nsub x nchan samples raises
+        numpy's reshape ValueError."""
+        if verbose:
+            start = time.time()
+            print("LOADING {0}...".format(filename))
+        head = []
+        with open(filename, "r") as file:
+            for line in file:
+                if line.startswith("#"):
+                    headline = str.strip(line[1:])
+                    head.append(headline)
+                    if str.split(headline) != []:
+                        if str.split(headline)[0] == 'MJD0:':
+                            if not hasattr(self, 'mjd'):  # first occurrence
+                                self.mjd = float(str.split(headline)[1])
+        self.name = os.path.basename(filename)
+        self.filename = filename
+        self.header = head
+        rawdata = np.loadtxt(filename).transpose()
+        self.times = np.unique(rawdata[2]*60)  # leading edge of integration (s)
+        if mjd is not None:
+            self.mjd = mjd
+        else:
+            self.mjd = self.mjd + self.times[0] / 86400
+        self.times = self.times - self.times[0]
+        self.freqs = rawdata[3]
+        fluxes = rawdata[4]
+        self.nchan = int(np.max(rawdata[1])) + 1
+        self.bw = self.freqs[-1] - self.freqs[0]
+        self.df = round(self.bw/self.nchan, 5)
+        self.bw = round(self.bw + self.df, 2)
+        self.nsub = int(np.max(rawdata[0])) + 1
+        self.dt = np.mean(np.diff(self.times))
+        self.tobs = np.max(self.times) + self.dt
+        self.freqs = np.unique(self.freqs)
+        self.freq = round(np.mean(self.freqs), 2)
+        fluxes = fluxes.reshape([self.nsub, self.nchan]).transpose()
+        if self.df < 0:  # ascending frequency, like self.freqs
+            self.df = -self.df
+            self.bw = -self.bw
+            fluxes = np.flip(fluxes, 0)
+        self.dyn = fluxes
+        if remove_short_subs and np.std(np.diff(self.times)) != 0:
+            self.remove_short_subs(threshold=subint_thresh)
+        self.lamsteps = lamsteps
+        if process:
+            self.auto_processing(lamsteps=lamsteps)
+        if verbose:
+            end = time.time()
+            print("...LOADED in {0} seconds\n".format(round(end - start, 2)))
+            self.info()
+
+    def remove_short_subs(self, threshold=2.33):
+        """Drop leading sub-integrations shorter than the mean of the others by more than
+        threshold standard deviations (reference dynspec.py:232-257)."""
+        dt0 = np.abs(np.diff(self.times))[0]
+        dt = np.mean(np.abs(np.diff(self.times))[1:])
+        sdt = np.std(np.abs(np.diff(self.times))[1:])
+        while dt0 - dt <= -threshold*sdt and sdt >= 0:
+            self.dyn = np.delete(self.dyn, (0), axis=1)
+            self.times = np.delete(self.times, (0))
+            dt0 = np.abs(np.diff(self.times))[0]
+            dt = np.mean(np.abs(np.diff(self.times))[1:])
+            sdt = np.std(np.abs(np.diff(self.times))[1:])
+        self.mjd += np.min(self.times)/86400
+        self.times -= np.min(self.times)
+        self.nsub = len(self.times)
+        self.dt = round(np.mean(np.diff(self.times)), 3)
+        self.tobs = round(max(self.times) + self.dt, 3)
+
+    def auto_processing(self, lamsteps=False, remove_short_sub=True):
+        """trim_edges, refill, calc_acf, scale_dyn (lamsteps), calc_sspec (reference
+        dynspec.py:422-440)."""
+        self.trim_edges(remove_short_sub=remove_short_sub)
+        self.refill()
+        self.calc_acf()
+        if lamsteps:
+            self.scale_dyn()
+        self.calc_sspec(lamsteps=lamsteps)
+
+    def info(self):
+        """Print the observation's properties (reference dynspec.py:4130-4143)."""
+        print("\t OBSERVATION PROPERTIES\n")
+        print("filename:\t\t\t{0}".format(self.name))
+        print("MJD:\t\t\t\t{0}".format(self.mjd))
+        print("Centre frequency (MHz):\t\t{0}".format(self.freq))
+        print("Bandwidth (MHz):\t\t{0}".format(self.bw))
+        print("Channel bandwidth (MHz):\t{0}".format(self.df))
+        print("Integration time (s):\t\t{0}".format(self.tobs))
+        print("Subintegration time (s):\t{0}".format(self.dt))
+        return
+
+    def crop_dyn(self, fmin=0, fmax=np.inf, tmin=0, tmax=np.inf):
+        """Keep frequencies in [fmin, fmax] MHz and times in [tmin, tmax] minutes
+        (reference dynspec.py:3816-3854)."""
+        crop_array = np.array((self.freqs >= fmin)*(self.freqs <= fmax))
+        self.dyn = self.dyn[crop_array, :]
+        self.freqs = self.freqs[crop_array]
+        self.nchan = len(self.freqs)
+        self.bw = round(max(self.freqs) - min(self.freqs) + self.df, 2)
+        self.freq = round(np.mean(self.freqs), 2)
+        tmin = tmin*60  # to seconds
+        tmax = tmax*60
+        if tmax < self.tobs:
+            self.tobs = tmax - tmin
+        else:
+            self.tobs = self.tobs - tmin
+        crop_array = np.array((self.times >= tmin)*(self.times <= tmax))
+        self.dyn = self.dyn[:, crop_array]
+        self.nsub = len(self.dyn[0, :])
+        self.times = self.times[crop_array]
+        self.mjd += np.min(self.times)/86400
+        self.times -= np.min(self.times)
+
+    # ------------------------------------------------------------------
+    # band edges and zapping (csrc/clean.cu)
+    # ------------------------------------------------------------------
+    def trim_edges(self, bandwagon_frac=0.5, remove_short_sub=True):
+        """Remove the band edges (reference dynspec.py:259-328): bottom rows first, then
+        top rows, then left and right columns, each while its count of zero or NaN entries
+        is greater than bandwagon_frac * n or it is all zero.  n is the column count for
+        rows and the row count before trimming for columns (the reference's), while a
+        column's zeros are counted over the rows kept.  NaN entries of self.dyn become 0;
+        the bookkeeping attributes follow the reference's expressions.
+
+        The zero counts come from the device in one read of the array; the host picks the
+        kept box and takes one crop.  Deviation: when every row or every column would go,
+        the reference's IndexError is raised before anything is changed (the reference has
+        set NaN to 0 by then).  remove_short_sub is accepted and unused, as there."""
+        dyn = self.dyn
+        nr, nc = np.shape(dyn)
+        if nr == 0 or nc == 0:
+            raise IndexError("index 0 is out of bounds for axis 0 with size 0")
+        rz, cz = _zero_counts(dyn)
+        gone = (rz > bandwagon_frac*nc) | (rz == nc)
+        if np.all(gone):
+            raise IndexError("index 0 is out of bounds for axis 0 with size 0")
+        r0, r1 = int(np.argmin(gone)), nr - int(np.argmin(gone[::-1]))
+        cz = cz(r0, r1)
+        gone = (cz > bandwagon_frac*nr) | (cz == r1 - r0)
+        if np.all(gone):
+            raise IndexError("index 0 is out of bounds for axis 1 with size 0")
+        c0, c1 = int(np.argmin(gone)), nc - int(np.argmin(gone[::-1]))
+        dyn[np.isnan(dyn)] = 0
+        if (r0, r1, c0, c1) != (0, nr, 0, nc):
+            self.dyn = dyn[r0:r1, c0:c1].copy()
+        if (r0, r1) != (0, nr):
+            self.freqs = np.delete(self.freqs, np.r_[0:r0, r1:nr])
+        if (c0, c1) != (0, nc):
+            self.times = np.delete(self.times, np.r_[0:c0, c1:nc])
+        self.mjd += np.min(self.times)/86400
+        self.times -= np.min(self.times)  # start at 0
+        self.nchan = len(self.freqs)
+        self.bw = round(max(self.freqs) - min(self.freqs) + self.df, 3)
+        self.freq = round(np.mean(self.freqs), 3)
+        self.nsub = len(self.times)
+        self.dt = round(np.mean(np.diff(self.times)), 3)
+        self.tobs = round(max(self.times) + self.dt, 3)
+        self.df = self.bw / self.nchan
+
+    def zap(self, sigma=7):
+        """Basic RFI zapping (reference dynspec.py:3856-3870): NaN where
+        |dyn - med| / mdev > sigma, med the median of the pixels that are not NaN and mdev
+        the median of the deviations that are not NaN, both exactly numpy's.  Runs on the
+        device; a float64 C-contiguous self.dyn is changed in place, any other is replaced
+        by its float64 result."""
+        import torch
+        d = D.upload(np.ascontiguousarray(self.dyn, dtype=np.float64))
+        stats = D.empty((2,), torch.float64)
+        _lib.check(_lib.lib.sb_zap_f64(d.data_ptr(), d.numel(), float(sigma),
+                                       stats.data_ptr(), D.stream_ptr()))
+        dyn = self.dyn
+        if isinstance(dyn, np.ndarray) and dyn.dtype == np.float64 and \
+                dyn.flags.c_contiguous and dyn.flags.writeable:
+            torch.from_numpy(dyn).copy_(d)
+        else:
+            self.dyn = D.download(d)
 
     # ------------------------------------------------------------------
     # gap filling (csrc/inpaint.cu)
